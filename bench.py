@@ -1,16 +1,18 @@
-"""bench.py -- env-steps/sec of the env.step hot path (random actions), contract per the round driver.
+"""bench.py -- env-steps/sec of the env.step hot path (random actions); prints one JSON line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--env ID] [--envs-per-gpu E] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--env ID] [--envs-per-gpu E] [--impl reference] [--dump-outputs DIR]
 
 Own arm: one "step" = ONE control step (10 physics substeps + obs/reward/done/auto-reset) of every env on
 every rank.  `value` = env-steps/s with actions already resident in HBM; `e2e` = the same through
 MyoVecEnv.step_host (pinned host action -> H2D, step, D2H of obs/reward/done inside the timed region).
 Reference arm (--impl reference): the reference's CPU implementation of the path on the host cores.  MuJoCo
-is not installable here (no network, not in /opt/wheelhouse), so this is the CPU oracle port
-(oracle/libmyo_oracle.so) -- labelled kind="port".
+is not a dependency of this project, so this is the CPU oracle port (oracle/myo_oracle.c) -- labelled kind="port".
 Each env differs (per-env random state and actions); the working set lives in shared memory and the HBM traffic per
 step is the compulsory state/action/obs I/O (8 MB for 4096 hand envs, smaller than L2), so L2 is evicted between
-timed steps by a 192 MiB write inside the timed region (config.l2; --no-l2-flush turns it off; it costs < 1 %).
+timed steps by a write of twice the device's L2 size inside the timed region (config.l2; --no-l2-flush turns it off).
+--dump-outputs DIR: after the timed steps, what the last timed step returned to the caller (obs, reward, done, truncated and
+the info arrays of rank 0's envs) as DIR/<name>.npy (float32 / float64, at most 64 MB in all: a fixed, seeded sample of env rows
+beyond that).  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -127,7 +129,7 @@ class ClockSampler:
 
 def _cpu_worker(args):
     """One host core: a single env stepped in a loop (reference protocol:
-    /root/reference/benchmarks/mjx_benchmark_baseline.py:8-25 -- gym.make, reset, timeit(env.step(random action)))."""
+    benchmarks/mjx_benchmark_baseline.py:8-25 of MyoSuite -- gym.make, reset, timeit(env.step(random action)))."""
     env_id, budget_s, seed, u01 = (tuple(args) + (False,))[:4]          # budget_s: wall-clock seconds of stepping (a bounded sample; the oracle's rate varies 10x with the contact load)
     import numpy as np
     from myosuite_b200 import assets, blob, vec_env
@@ -172,12 +174,34 @@ def cpu_baseline(env_id, budget_s, threads=1, u01=False):
     return sum(r[0] for r in res) / max(r[1] for r in res), sum(r[0] for r in res)
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(env, out_dir):
+    """What MyoVecEnv.step returned in the last step (obs, reward, done, truncated, info arrays) as out_dir/<name>.npy.  Integer and
+    bool arrays are widened to float32.  If all rows exceed DUMP_LIMIT_BYTES, a fixed (seed 0) sorted sample of env rows is written."""
+    import numpy as np
+    t = env.t
+    arrays = {"obs": t["obs"], "reward": t["reward"], "done": t["done"], "truncated": t["truncated"],
+              "last_return": t["last_return"], "time": t["time"], "overflow": t["overflow"]}
+    arrays = {k: v.detach().cpu().numpy() for k, v in arrays.items()}
+    arrays = {k: (v if v.dtype in (np.float32, np.float64) else v.astype(np.float32)) for k, v in arrays.items()}
+    n = env.num_envs
+    row_bytes = sum(v.nbytes for v in arrays.values()) / n
+    if row_bytes * n > DUMP_LIMIT_BYTES:
+        rows = np.sort(np.random.default_rng(0).choice(n, int(DUMP_LIMIT_BYTES // row_bytes), replace=False))
+        arrays = {k: v[rows] for k, v in arrays.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.ascontiguousarray(v))
+
+
 MUJOCO_PUBLISHED = {"myoHandPoseRandom-v0": "reference's own CPU MuJoCo single-env figure on the hand model (myoHandReachRandom, derived from its plot): ~1.9 k env-steps/s on 1 core (BASELINE.md section 1)",
                     "myoElbowPose1D6MRandom-v0": "reference's own CPU MuJoCo single-env figure on this model (derived from its plot): ~10 k env-steps/s on 1 core (BASELINE.md section 1)"}
 
 
 def reference_arm(args, W):
-    """bench.py --impl reference: the CPU implementation of the path on the box's host cores.  MuJoCo is not installable here, so this is
+    """bench.py --impl reference: the CPU implementation of the path on the host cores.  MuJoCo is not a dependency of this project, so this is
     the oracle PORT (kind = "port"), built -O3 -march=native on this machine, one single-env loop per usable core."""
     from oracle import oracle_py
     os.environ["MYO_ORACLE_LIB"] = oracle_py.build_native()        # inherited by the forked workers
@@ -212,7 +236,8 @@ def main():
     ap.add_argument("--actions", default="u11", choices=["u11", "u01"], help="u11: U[-1,1] = action_space.sample() (default); u01: U(0,1), the reference benchmark's protocol (benchmarks/mjx_benchmark_baseline.py:15)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip config.extra (the other BASELINE configs, the U(0,1) variant, the sustained run)")
-    ap.add_argument("--no-l2-flush", action="store_true", help="do not evict L2 between timed steps (default: a 192 MiB write per step)")
+    ap.add_argument("--no-l2-flush", action="store_true", help="do not evict L2 between timed steps (default: a write of twice the L2 size per step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step returned as DIR/<name>.npy")
     ap.add_argument("--maxcon", type=int, default=0, help="contact capacity per env (0 = library default 32); experiments only")
     ap.add_argument("--barrier-mode", type=int, default=0)
     ap.add_argument("--lockstep-groups", type=int, default=0)
@@ -229,16 +254,16 @@ def main():
 
     import torch
     import torch.distributed as dist
-    from myosuite_b200 import build, vec_env
+    from myosuite_b200 import vec_env
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device -- the product path has no CPU fallback")
-    build.build()
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     dev = torch.device("cuda", local_rank)
-    # L2 (126 MB) is evicted between timed steps by writing a 192 MiB buffer: step k+1 reads the state step k wrote from HBM, not from L2
-    flush_buf = None if args.no_l2_flush else torch.empty(192 << 20, dtype=torch.uint8, device=dev)
+    # L2 is evicted between timed steps by writing a buffer twice its size: step k+1 reads the state step k wrote from HBM, not from L2
+    flush_mib = 2 * torch.cuda.get_device_properties(dev).L2_cache_size >> 20
+    flush_buf = None if args.no_l2_flush else torch.empty(flush_mib << 20, dtype=torch.uint8, device=dev)
 
     def flush_l2(i):
         if flush_buf is not None:
@@ -291,6 +316,8 @@ def main():
     if rank == 0:
         sampler.start()
     ms, launches = timed(env, ring, args.steps, W)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(env, args.dump_outputs)
     ms_e2e, _ = timed(env, ring_host, args.steps, 3, host=True)        # end to end through the public API with host buffers
     clocks = sampler.stop() if rank == 0 else None
     # the one collective of the path: gather finished-episode returns at rollout end (SURVEY.md section 8e), timed on its own
@@ -308,21 +335,15 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))      # fallback: the H100 SXM data-sheet HBM3 bandwidth
 
     def roofline(env_id, n_env, ms_total, n_steps):
         # dominant kernel = the env-step kernel, launched once per control step; its launch duration is bounded above by the timed region
-        # per step (which also holds the one-CTA regroup kernel, 0.2 %, and the L2 flush, 1 %: profiles/r02_launches_timed_region.csv)
+        # per step (which also holds the one-CTA regroup kernel and the L2 flush)
         aio = A_IO.get(env_id, 0)
         achieved = aio * n_env / (ms_total * 1e-3 / max(n_steps, 1)) / 1e9
-        traffic = None
-        for tf in ("r02_traffic.json", "r01_traffic.json"):
-            f = os.path.join(ROOT, "profiles", tf)
-            if os.path.exists(f):
-                traffic = json.load(open(f)).get(env_id)
-                break
-        return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                "note": "fused step is issue/latency bound, not HBM bound (SURVEY 8d): algorithmic bytes %d B/env-step; peak = %s" % (aio, "measured" if peaks else "fallback")}
+        return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+                "note": "fused step is issue/latency bound, not HBM bound (SURVEY 8d): algorithmic bytes %d B/env-step; peak = %s" % (aio, "measured" if peaks else "H100 SXM data sheet")}
 
     extra = {}
     if not args.no_extra:
@@ -355,7 +376,7 @@ def main():
                 "warmup": W, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64",
                 "data": "synthetic", "impl": "b200",
                 "config": {"workload": "%s, %d envs/GPU, frame_skip 10, random actions %s, auto-reset" % (args.env, n, "U(0,1)" if args.actions == "u01" else "U[-1,1]"),
-                           "l2": ("not flushed (--no-l2-flush)" if args.no_l2_flush else "flushed between timed steps: a 192 MiB write per step inside the timed region (inputs, 8 MB of state per step, are smaller than L2)"), "parallelism": "env-sharded x%d, no data-path collective" % world,
+                           "l2": ("not flushed (--no-l2-flush)" if args.no_l2_flush else "flushed between timed steps: a %d MiB write (twice the L2) per step inside the timed region (inputs, 8 MB of state per step, are smaller than L2)" % flush_mib), "parallelism": "env-sharded x%d, no data-path collective" % world,
                            "contact_overflow_env_fraction": overflow_frac, "rollout_end_allgather_us": allgather_us, "extra": extra},
                 "e2e": {"value": e2e, "unit": "env-steps/s", "h2d_bytes_per_step": world * n * nu * 4, "d2h_bytes_per_step": world * n * (max(A_OBS.get(args.env, 0), 0) * 4 + 4 + 1)},      # whole job, like `value`
                 "gpu_launches": int(launches),

@@ -1,13 +1,13 @@
 /* myo_b200.h -- C-ABI of the B200-native batched musculoskeletal simulator (libmyo_b200.so).
  *
  * Drop-in boundary for ONE hot path of MyoSuite: `env.step` of
- *   /root/reference/myosuite/envs/myo/base_v0.py:82-118  (BaseV0.step)
+ *   myosuite/envs/myo/base_v0.py:82-118  (BaseV0.step)
  * for thousands of parallel envs.  The reference has no FFI seam of its own on this path; what the
  * library semantically replaces is the MuJoCo C API the reference reaches through pybind11:
- *   mj_step      /root/reference/myosuite/robot/robot.py:861
- *   mj_forward   /root/reference/myosuite/robot/robot.py:607,1002 ; envs/env_base.py:91-92
- *   mj_resetData /root/reference/myosuite/robot/robot.py:999
- *   MjSpec.from_file().compile()  /root/reference/myosuite/envs/env_base.py:70-72,96-106
+ *   mj_step      myosuite/robot/robot.py:861
+ *   mj_forward   myosuite/robot/robot.py:607,1002 ; envs/env_base.py:91-92
+ *   mj_resetData myosuite/robot/robot.py:999
+ *   MjSpec.from_file().compile()  myosuite/envs/env_base.py:70-72,96-106
  * plus the per-step Python glue that must run on the device to keep envs resident in HBM:
  *   sigmoid action remap            base_v0.py:86-94
  *   3CC-r fatigue                   envs/myo/fatigue.py:38-76,82-99

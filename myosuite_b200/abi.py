@@ -60,7 +60,7 @@ def lib(variant=None):
             if variant not in _build.VARIANTS:
                 raise MyoError("unknown library variant %r" % (variant,))
             path = _build.variant_path(variant)
-            if not os.path.exists(path):          # (mtimes do not survive the snapshot to a GPU box: existence only, like the product library)
+            if not os.path.exists(path):          # (mtimes need not survive a copy of the tree: existence only, like the product library)
                 path = _build.build_variant(variant, _build.VARIANTS[variant])
             _VARIANTS[variant] = _bind(ctypes.CDLL(path))
         return _VARIANTS[variant]

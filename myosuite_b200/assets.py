@@ -1,7 +1,7 @@
 """Model assets: name -> compiled Model.
 
 Models are compiled from the simhive MJCF files when a MyoSuite checkout is reachable
-(``MYOSUITE_ROOT`` env var, an installed ``myosuite`` package, or /root/reference/myosuite), otherwise the
+(``MYOSUITE_ROOT`` env var, or an installed ``myosuite`` package), otherwise the
 pre-compiled fixtures committed under ``myosuite_b200/assets/`` (made by tools/compile_assets.py with this
 repo's own compiler) are used.
 """

@@ -1,4 +1,4 @@
-"""In-tree build of libmyo_b200.so (sm_100a only)."""
+"""In-tree build of libmyo_b200.so (H100, sm_90a only)."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ SRC = os.path.join(HERE, "csrc", "myo_b200.cu")
 DEPS = [SRC, os.path.join(HERE, "csrc", "myo_device.cuh"), os.path.join(HERE, "csrc", "myo_solver.cuh"),
         os.path.join(HERE, "..", "include", "myo_b200.h"), os.path.join(HERE, "..", "include", "myo_blob_layout.h")]
 LIB = os.path.join(HERE, "libmyo_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
 
 

@@ -1,5 +1,5 @@
 // myo_b200.cu -- kernels + C-ABI of libmyo_b200.so (see include/myo_b200.h for the boundary contract).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -shared -Xcompiler -fPIC
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -shared -Xcompiler -fPIC
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -11,9 +11,8 @@
 
 // ------------------------------------------------------------------ kernel arguments
 #ifndef MYO_BMASK
-#define MYO_BMASK 0x40      /* phases of the product kernels that start with a CTA barrier (bit k = phase k).  Measured round 2 at 14 warps per CTA with
-                               load-sorted rounds (hand, env-steps/s): 0xFF 1.129 M, 0x55 1.138 M, 0x51 1.140 M, 0x41 1.143 M, 0x40 (only the solver entry, whose
-                               inner barriers need aligned warps anyway) 1.147 M, 0x01 1.117 M, 0x00 1.129 M.  (At 10 warps without the sort, 0xFF had won.) */
+#define MYO_BMASK 0x40      /* phases of the product kernels that start with a CTA barrier (bit k = phase k).  0x40: only the solver entry, whose inner
+                               barriers need aligned warps anyway; with load-sorted rounds the warps of a CTA stay close without the other phase barriers. */
 #endif
 struct StepArgs {
   myo_buffers b; myo_task_cfg cfg;
@@ -260,7 +259,7 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
   const bool integrate = a.mode == 0 || (DBG && a.mode == 1 && a.n_substeps > 0);
   const bool prof = DBG && b.tap_phase_cycles != nullptr;
   // env e belongs to CTA e % gridDim.x: every CTA gets floor or ceil of n_env / gridDim.x envs, so no CTA runs a full extra round
-  // while the others idle (4096 envs on 148 SMs: rounds of 10, 10, 8 warps everywhere instead of 10, 10, 10 on three quarters of the SMs)
+  // while the others idle (4096 envs on 132 SMs at 11 warps: rounds of 11, 11, 9 or 10 everywhere instead of 11, 11, 11 on four fifths of the SMs)
   // With a.perm (big models, env steps of the product kernels) the slot -> env map is the load-sorted one: the envs of a round carry
   // similar contact loads, so the lockstep barriers wait for a slowest env that is close to the average one.
   const bool regrouped = !DBG && a.perm != nullptr;

@@ -5,7 +5,7 @@
 // read (int16 index lists + f64 tables, staged once per CTA with a bulk async copy) live in shared
 // memory; HBM is touched only for the per-step state / action / observation rows.
 // What is computed is what the reference's mujoco.mj_step computes for these models
-// (/root/reference/myosuite/robot/robot.py:856-861; SURVEY.md Appendix A), but the formulation is
+// (myosuite/robot/robot.py:856-861; SURVEY.md Appendix A), but the formulation is
 // this project's own: origin-centred spatial algebra over dynamic bodies only, compile-time folded
 // constant tendon segments, structural-non-zero tendon moments, tree-sparse LDL / dense Newton.
 #pragma once
@@ -67,7 +67,7 @@ enum { CNT_ncon, CNT_nefc, CNT_nlimrow, CNT_niter, CNT_overflow, CNT_ncand, CNT_
 #define CI(name) ((const idx_t*)(smem + m.nD) + m.hoff[MYO_SEC_##name])
 #define CD(name) ((const double*)smem + m.hoff[MYO_SEC_##name])
 #ifdef MYO_COLD_L2ONLY
-#define LDC(p) __ldcg(p)                                      // (measured round 2: bypassing L1 costs 5 % at 14 warps -- the L1 hit rate of these loads is 97 %)
+#define LDC(p) __ldcg(p)                                      // (experiment: bypass L1 for the cold tables; the default keeps them in L1)
 #else
 #define LDC(p) __ldg(p)
 #endif
@@ -107,9 +107,9 @@ __device__ __forceinline__ double warp_sum(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
   return v; }
 
-// Reciprocal and square root without libdevice's IEEE special-case paths: MUFU seed (~20 bits) + two Newton steps, 1-2 ulp.  Measured on the
-// B200 (profiles/r02_ubench_latencies.txt): a dependent f64 division costs 141 cycles, a DFMA 10 -- these run in ~65 / ~90.  Arguments
-// must be normal numbers; m_sqrt(0) = 0.  (acos costs 645 cycles against asin's 337: the wrap arc uses pi/2 - asin.)
+// Reciprocal and square root without libdevice's IEEE special-case paths: MUFU seed (~20 bits) + two Newton steps, 1-2 ulp.  Dependent
+// latencies of these and of the libdevice calls they replace: tools/ubench/ubench.cu.  Arguments must be normal numbers; m_sqrt(0) = 0.
+// (acos is slower than asin: the wrap arc uses pi/2 - asin.)
 __device__ __forceinline__ double m_rcp(double x) { double y; asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x)); double e = fma(-x, y, 1.0); y = fma(y, e, y); e = fma(-x, y, 1.0); return fma(y, e, y); }
 __device__ __forceinline__ double m_sqrt(double x) { double y; asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
   const double h = 0.5*x; double t = fma(-h*y, y, 0.5); y = fma(y, t, y); t = fma(-h*y, y, 0.5); y = fma(y, t, y);

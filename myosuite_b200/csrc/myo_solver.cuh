@@ -252,7 +252,7 @@ __device__ __noinline__ void chol_rs(double* H, double* x, int n, int lane) {
     if (lane == k) x[k] = b;                         // z_k of the forward substitution is final (x has chol_pad(n) slots)
     __syncwarp();
     // all broadcast loads of this step are issued as ONE batch, ahead of the reciprocal's dependent chain (left to itself ptxas
-    // alternates LDS / DFMA through a single register: 29 cycles of shared-memory latency per trailing entry, 14 k cycles per solve)
+    // alternates LDS / DFMA through a single register: one shared-memory latency per trailing entry)
     double col[NMAX];
     #pragma unroll
     for (int j = k+1; j < NMAX; j++) col[j] = H[TRI(j,k)];
@@ -280,7 +280,7 @@ __device__ __noinline__ void chol_rs(double* H, double* x, int n, int lane) {
 // rows ride along DISTRIBUTED over the lanes (lane j keeps B[q][j]): at step k lane k publishes its now final entries, every lane j > k
 // applies the same rank-1 update to its border entries with its own U[j][k].  The e x e Schur complement C - L21 D L21' and the border
 // right-hand side are warp sums; the small system is solved redundantly by every lane.  Replaces the shuffle-based chol_reg32b below
-// (two 32-double register arrays, 800 spill instructions): measured round 2 on the legs model, 48.7 k cycles per solve before.
+// (two 32-double register arrays, 800 spill instructions).
 template <int E>
 __device__ __noinline__ void chol_rs32b(double* H, double* x, int n, int lane) {
   SHARED_PTR(H); SHARED_PTR(x);
@@ -300,7 +300,7 @@ __device__ __noinline__ void chol_rs32b(double* H, double* x, int n, int lane) {
       for (int q = 0; q < E; q++) H[TRI(32+q, k)] = bq[q]; }
     __syncwarp();
     // the trailing columns are loaded in at most two batches of CH: with 64 row registers, a full batch of 31 and the border values
-    // the function overflowed its register budget (196 LDL / 169 STL in SASS, 31 k cycles per solve with 7 warps)
+    // the function overflowed its register budget (196 LDL / 169 STL in SASS)
     constexpr int CH = 18;
     double col[32], bk[E];
     #pragma unroll
@@ -419,12 +419,11 @@ __device__ __noinline__ void chol_reg32b(const double* H, int n, double* x, int 
 // The same L D L' with a ROLLED elimination loop: after column k is eliminated every lane shifts its row registers left by one (the shift is
 // folded into the destination of the update FMA), so the pivot column is r[0] at EVERY step and the loop body has static register
 // indices.  Why it matters: the unrolled variant above is ~2 500 straight-line instructions (40 KB) that every call streams from L2 at the
-// ~3.8 B/cycle the SM's instruction fetch sustains for uncached code (profiles/r02_ubench_icache.txt): 10.7 k cycles per solve inside
-// the step kernel against 5-7 k when the code is warm (tools/ubench/ubench_chol.cu).  The rolled body (~100 instructions) stays in the
+// rate the SM's instruction fetch sustains for uncached code (tools/ubench/ubench_icache.cu), so a solve inside the step kernel
+// is slower than one whose code is warm (tools/ubench/ubench_chol.cu).  The rolled body (~100 instructions) stays in the
 // instruction cache; it pays with FMAs on columns that are already finished (NMAX - 1 per step instead of n - 1 - k).
-// MEASURED (round 2, tools/ubench/ubench_chol.cu and the step kernel): 27.6 k cycles per 23 x 23 solve with 10 warps per SM against 7.0 k
-// for the unrolled variant (30 k vs 10.7 k inside the step kernel) -- the clamped address chain and the dead-column FMAs cost far more than
-// the instruction fetch they save.  Kept as an experiment behind MYO_CHOL_ROLLED; the unrolled variant is the product path.
+// It was measured slower than the unrolled variant, in isolation and inside the step kernel: the clamped address chain and the dead-column
+// FMAs cost more than the instruction fetch they save.  Kept as an experiment behind MYO_CHOL_ROLLED; the unrolled variant is the product path.
 // H: packed lower triangle, n rows (no padding needed: reads past the last row are clamped onto it and only feed dead slots); destroyed.
 template <int NMAX>
 __device__ __noinline__ void chol_rot(double* H, double* x, int n, int lane) {
@@ -527,7 +526,7 @@ __device__ void ldl_solve(const DevModel& m, const Warp w, const double* LD, con
 // ------------------------------------------------------------------ Newton solver: leaves qacc in S_a
 // Called by EVERY warp of the CTA when cta_sync is set (live = this warp holds an env): the warps still iterating are re-aligned by CTA
 // barriers at the top of each Newton iteration and before the Cholesky, so that they keep sharing instruction fetches inside the
-// phase too (a lone 23x23 register Cholesky costs 29 k cycles out of step with the other warps, 21 k in step); finished and idle
+// phase too (a lone register Cholesky out of step with the other warps fetches its code alone); finished and idle
 // warps only take part in the barriers.  The total wait is unchanged: the CTA leaves the phase with its slowest env either way.
 // __forceinline__: as a real call the function receives the DevModel by address and every m.field becomes a generic load that is repeated
 // after each shared-memory store (measured round 2: 310 LD.E in the solver of the launch_bounds(448) kernel, which had not inlined it).
@@ -587,8 +586,8 @@ __device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, dou
     // hits SOME lane and the warp runs the hit path 9 x ncon times.)  Two contacts at a time, one per half-warp, 16 lanes over the lower
     // triangle of the contact's block: a finger-finger block has 36 entries -- two passes of 32 lanes with 4 busy in the second, now
     // three passes of 16 for TWO contacts.  The two halves may touch the same H entry, so their read-modify-writes take turns
-    // (half 0 first: a fixed order).  MEASURED (round 2, hand, 14 warps): 1.144 M env-steps/s against 1.147 M for the one-contact loop below --
-    // the two ordered updates and the wider predication eat the saved pass.  Kept as an experiment behind -DMYO_H_PAIRED.
+    // (half 0 first: a fixed order).  It did not beat the one-contact loop below: the two ordered updates and the wider
+    // predication eat the saved pass.  Kept as an experiment behind -DMYO_H_PAIRED.
 #ifdef MYO_H_PAIRED
     for (int c0 = 0; c0 < ncon; c0 += 2) { const int half = w.lane >> 4, hl = w.lane & 15, c = c0 + half;
       bool ok = c < ncon; int nr = 0, rb = 0; double W[6] = {0,0,0,0,0,0};  // nn n1 n2 11 12 22

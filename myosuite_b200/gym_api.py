@@ -1,6 +1,6 @@
 """Gym-level drop-in surface of the reference's env classes (SURVEY.md section 8b "must be preserved"), host side only.
 
-What the reference exposes on `env.unwrapped` and its tests exercise (/root/reference/myosuite/tests/test_envs.py:54-123):
+What the reference exposes on `env.unwrapped` and its tests exercise (myosuite/tests/test_envs.py:54-123):
   action_space / observation_space      envs/env_base.py:145-155, 210-218      (Box(-1, 1, nu) f32 ; Box(-10, 10, obs_dim) f32)
   obs_dict / rwd_dict                   envs/env_base.py:409-432               (per-key views of the observation; reward terms)
   get_obs_dict / get_reward_dict        myobase/pose_v0.py:100-140, reach_v0.py:98-160, obj_hold_v0.py:79-121, walk_v0.py:268-319

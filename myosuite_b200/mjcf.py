@@ -1,7 +1,7 @@
 """MJCF loader + model compiler for the subset of MJCF used by the MyoSuite hot-path models.
 
 Replaces the reference's loader seam ``mujoco.MjSpec.from_file(path).compile()``
-(/root/reference/myosuite/envs/env_base.py:70-72,96-106).  MuJoCo itself is third-party and absent,
+(myosuite/envs/env_base.py:70-72,96-106).  MuJoCo itself is third-party and absent,
 so the compile rules below restate MuJoCo's documented XML semantics (SURVEY.md Appendix A.7/B.3):
 includes, nested default classes + childclass, euler/fromto/zaxis frames, explicit and geom-derived
 inertia (incl. binary-STL mesh inertia), the <muscle> shortcut, spatial tendons with sphere/cylinder
@@ -355,7 +355,7 @@ def compile_mjcf(path, mesh_inertia="legacy", drop_geoms=()):
     """Parse + compile an MJCF file into a :class:`Model`.
 
     drop_geoms: geom names removed from collision (the Walk task moves the hfield out of reach,
-    /root/reference/myosuite/envs/myo/myobase/walk_v0.py:262-266 -- mirrored by dropping it).
+    myosuite/envs/myo/myobase/walk_v0.py:262-266 -- mirrored by dropping it).
     """
     root, main_dir = load_xml(path)
     comp = dict(angle="degree", eulerseq="xyz", inertiafromgeom="auto", balanceinertia=False,

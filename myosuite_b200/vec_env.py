@@ -1,8 +1,8 @@
 """Batched env mirror of the reference's BaseV0 / PoseEnvV0 stack on top of the C-ABI library.
 
 Reference interface mirrored (same names, argument meaning, return layout):
-  * ``gym.make(id)`` registry ids + kwargs      /root/reference/myosuite/envs/myo/myobase/__init__.py:124-138,402-415
-  * ``env.reset() -> (obs, info)``               /root/reference/myosuite/envs/env_base.py:647-654
+  * ``gym.make(id)`` registry ids + kwargs      myosuite/envs/myo/myobase/__init__.py:124-138,402-415
+  * ``env.reset() -> (obs, info)``               myosuite/envs/env_base.py:647-654
   * ``env.step(a) -> (obs, reward, terminated, truncated, info)``   envs/env_base.py:403-407, envs/myo/base_v0.py:82-118
   * muscle-condition variants myoFati*/myoSarc*/myoReaf*           myobase/__init__.py:17-49, base_v0.py:60-79
 All per-env state lives in torch CUDA tensors owned here and bound to the library by pointer.

@@ -8,7 +8,7 @@ import numpy as np
 
 
 def action_to_ctrl(a, normalize_act=True):
-    """/root/reference/myosuite/envs/myo/base_v0.py:83-96 (all actuators of the hot-path models are muscles)."""
+    """myosuite/envs/myo/base_v0.py:83-96 (all actuators of the hot-path models are muscles)."""
     a = np.array(a, dtype=np.float64, copy=True)
     if normalize_act:
         a = 1.0 / (1.0 + np.exp(-5.0 * (a - 0.5)))
@@ -16,7 +16,7 @@ def action_to_ctrl(a, normalize_act=True):
 
 
 class Fatigue:
-    """3CC-r cumulative fatigue, /root/reference/myosuite/envs/myo/fatigue.py:8-99."""
+    """3CC-r cumulative fatigue, myosuite/envs/myo/fatigue.py:8-99."""
 
     def __init__(self, n, dt, tauact=0.01, taudeact=0.04):
         self.r, self.F, self.R = 10 * 15, 0.00912, 0.1 * 0.00094      # fatigue.py:9-11
@@ -43,13 +43,13 @@ class Fatigue:
 
 
 def pose_obs(qpos, qvel, act, target, dt):
-    """/root/reference/myosuite/envs/myo/myobase/pose_v0.py:100-111 + envs/obs_vec_dict.py:76-88
+    """myosuite/envs/myo/myobase/pose_v0.py:100-111 + envs/obs_vec_dict.py:76-88
     (keys qpos, qvel, pose_err, act in that order; float32)."""
     return np.concatenate([qpos, np.asarray(qvel) * dt, np.asarray(target) - qpos, act]).astype(np.float32)
 
 
 def pose_reward(qpos, act, target, pose_thd, weights=(1.0, 4.0, 1.0, 50.0), far_th=4 * np.pi / 2):
-    """/root/reference/myosuite/envs/myo/myobase/pose_v0.py:113-140 -> dict(dense, solved, done, pose, bonus, penalty, act_reg).
+    """myosuite/envs/myo/myobase/pose_v0.py:113-140 -> dict(dense, solved, done, pose, bonus, penalty, act_reg).
     TorsoEnvV0 (torso_v0.py:98-125) is the same rule with far_th = pi."""
     pose_dist = np.linalg.norm(np.asarray(target) - qpos)
     act_mag = np.linalg.norm(act) / (len(act) if len(act) else 1)

@@ -2,11 +2,11 @@
  *
  * A scalar, f64, single-env restatement of what the reference's hot path computes per physics
  * substep: `mujoco.mj_step(model, data)` as called from
- *   /root/reference/myosuite/robot/robot.py:856-861 (Robot._advance)  and the
- * `mujoco.mj_forward` of /root/reference/myosuite/robot/robot.py:607 (Robot.sensor2sim).
+ *   myosuite/robot/robot.py:856-861 (Robot._advance)  and the
+ * `mujoco.mj_forward` of myosuite/robot/robot.py:607 (Robot.sensor2sim).
  *
- * MuJoCo (pinned mujoco 3.5.0, /root/reference/uv.lock:1739-1740) is a third-party dependency that
- * is ABSENT from /root/reference and from this container.  The algorithm below restates MuJoCo's
+ * MuJoCo (pinned mujoco 3.5.0, uv.lock:1739-1740) is a third-party dependency that
+ * is not part of the reference checkout nor of this project.  The algorithm below restates MuJoCo's
  * published pipeline (MuJoCo documentation, "Computation" chapter; SURVEY.md Appendix A) stage by
  * stage, in MuJoCo's own formulation (subtree-COM-centred spatial algebra, mj_crb/mj_rne/mj_tendon/
  * mju_wrap/mj_makeConstraint/Newton), deliberately different from the restructured formulation

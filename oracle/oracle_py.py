@@ -2,6 +2,7 @@
 import ctypes
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -18,10 +19,9 @@ def build(force=False):
 
 
 def build_native():
-    """-O3 -march=native build for the timed CPU arm (bench.py --impl reference), compiled ON the machine that runs it:
-    oracle/_native/libmyo_oracle_native.so.  Falls back to the portable build if the compiler refuses."""
-    d = os.path.join(_HERE, "_native"); os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, "libmyo_oracle_native.so")
+    """-O3 -march=native build for the timed CPU arm (bench.py --impl reference), compiled ON the machine that runs it into a fresh
+    temporary directory (the source tree may be read-only).  Falls back to the portable build if the compiler refuses."""
+    so = os.path.join(tempfile.mkdtemp(prefix="myo_oracle_native_"), "libmyo_oracle_native.so")
     try:
         subprocess.check_call(["gcc", "-O3", "-march=native", "-fPIC", "-std=c11", "-ffp-contract=off", "-shared", "-o", so, os.path.join(_HERE, "myo_oracle.c"), "-lm"],
                               stderr=subprocess.DEVNULL)

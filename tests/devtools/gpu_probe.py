@@ -1,4 +1,4 @@
-"""GPU parity + timing probe (developer tool; run under gpurun).  Compares the CUDA path with the CPU oracle."""
+"""GPU parity + timing probe (developer tool; needs a GPU).  Compares the CUDA path with the CPU oracle."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import numpy as np, torch

@@ -7,6 +7,7 @@ generate golden vectors.  Used only by the golden-vector generators in this dire
 import importlib
 import importlib.machinery
 import importlib.util
+import os
 import sys
 import types
 
@@ -31,7 +32,8 @@ class _Stub(types.ModuleType):
         return (object,)
 
 
-def install(ref_root="/root/reference"):
+def install(ref_root=None):
+    ref_root = ref_root or os.environ["MYOSUITE_CHECKOUT"]
     for name in ("mujoco", "gym", "gymnasium", "termcolor", "flatten_dict", "h5py", "imageio", "click", "skvideo", "skvideo.io",
                  "PIL", "PIL.Image", "dm_control", "git", "torchvision", "gymnasium.utils", "gym.utils", "gymnasium.envs", "gymnasium.envs.registration"):
         if name not in sys.modules:

@@ -1,12 +1,12 @@
 """Generate golden vectors by RUNNING THE REFERENCE'S OWN PYTHON CODE (unmodified, imported from
-/root/reference with third-party imports stubbed, see _ref_stubs.py).  Output: tests/golden/pylogic.npz
+a MyoSuite checkout, MYOSUITE_CHECKOUT=<its root>, with third-party imports stubbed, see _ref_stubs.py).  Output: tests/golden/pylogic.npz
 
 Covers the Python-side part of the hot path that is independent of MuJoCo:
   * CumulativeFatigue.compute_act / reset      (envs/myo/fatigue.py:38-99)
   * BaseV0.step action->ctrl remap (+fatigue)   (envs/myo/base_v0.py:82-118)  -- robot.step stubbed to record ctrl
   * PoseEnvV0.get_obs_dict / get_reward_dict     (envs/myo/myobase/pose_v0.py:100-140)
   * ObsVecDict.obsdict2obsvec                    (envs/obs_vec_dict.py:76-88)
-Run here (needs /root/reference):  python tests/golden/make_golden.py
+Run with MYOSUITE_CHECKOUT set:  python tests/golden/make_golden.py
 """
 import os
 import sys

@@ -1,7 +1,7 @@
 """Golden vectors for the Walk / ObjHold / Reach task logic, produced by RUNNING THE REFERENCE'S OWN CLASSES
 (WalkEnvV0 / ObjHoldFixedEnvV0 / ReachEnvV0 get_obs_dict, get_reward_dict and helpers, unmodified, created with __new__ so that no
 simulator is constructed) on mj_data-like records filled from this repo's CPU oracle.  Output: tests/golden/tasks.npz
-Run here (needs /root/reference and oracle/libmyo_oracle.so):  python tests/golden/make_golden_tasks.py
+Run with a MyoSuite checkout (MYOSUITE_CHECKOUT=<its root>) and oracle/libmyo_oracle.so built:  python tests/golden/make_golden_tasks.py
 """
 import os
 import sys

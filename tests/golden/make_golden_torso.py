@@ -1,6 +1,6 @@
 """Golden vectors for the Torso task, produced by RUNNING THE REFERENCE'S OWN TorsoEnvV0 (get_obs_dict / get_reward_dict and the target
 rule of _setup, unmodified, instance created with __new__ so that no simulator is constructed) on random states of the torso model.
-Output: tests/golden/torso.npz.   Run here (needs /root/reference):  python tests/golden/make_golden_torso.py"""
+Output: tests/golden/torso.npz.   Run with MYOSUITE_CHECKOUT set:  python tests/golden/make_golden_torso.py"""
 import json
 import os
 import sys

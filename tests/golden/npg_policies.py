@@ -5,7 +5,7 @@ unpickle them with torch alone.  Forward pass restated from mjrl (policies/gauss
     x = (obs - in_shift) / (in_scale + 1e-8) ; tanh after every layer but the last ; mean = out * out_scale + out_shift
     action = mean + exp(log_std) * N(0, 1)          (evaluation mode: action = mean)
 `python tests/golden/npg_policies.py` extracts the weights and the logged scores of the envs this repo implements into
-tests/golden/npg_policies.npz (small: 32x32 MLPs), so that the GPU box -- which has no /root/reference -- can replay them.
+tests/golden/npg_policies.npz (small: 32x32 MLPs), so that the tests replay them without a MyoSuite checkout.
 """
 import csv
 import glob
@@ -17,7 +17,7 @@ import types
 
 import numpy as np
 
-REF = "/root/reference/myosuite/agents/baslines_NPG"
+REF = os.path.join(os.environ.get("MYOSUITE_CHECKOUT", "."), "myosuite/agents/baslines_NPG")
 ENVS = ["myoElbowPose1D6MFixed-v0", "myoElbowPose1D6MRandom-v0", "myoHandPoseFixed-v0", "myoHandPoseRandom-v0", "myoHandReachFixed-v0",
         "myoHandReachRandom-v0", "myoHandObjHoldFixed-v0", "myoHandObjHoldRandom-v0", "myoHandKeyTurnFixed-v0", "myoHandKeyTurnRandom-v0",
         "myoHandPenTwirlFixed-v0", "myoHandPenTwirlRandom-v0"]

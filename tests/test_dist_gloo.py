@@ -46,7 +46,7 @@ def test_env_sharding_and_return_gather_world2():
 
 
 def test_bench_reference_arm_contract():
-    """`bench.py --impl reference` (the CPU arm the driver runs beside the GPU arm) prints one JSON line with the contract's keys;
+    """`bench.py --impl reference` (the CPU arm run beside the GPU arm) prints one JSON line with the contract's keys;
     under torchrun only rank 0 prints.  Runs on the host cores (oracle port), no GPU needed."""
     import json, os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -77,7 +77,7 @@ def _assert_close(a, b, atol=1e-5, rtol=1e-8):
 @pytest.mark.gpu
 @pytest.mark.parametrize("env_id", ["myoElbowPose1D6MRandom-v0", "myoHandPoseRandom-v0", "myoFatiLegWalk-v0", "myoHandObjHoldRandom-v0"])
 def test_env_contract_like_reference_test_envs(env_id):
-    """Mirror of /root/reference/myosuite/tests/test_envs.py:54-123 (check_env)."""
+    """Mirror of myosuite/tests/test_envs.py:54-123 (check_env)."""
     import myosuite_b200 as myo
     input_seed = 1234
     env1 = myo.make(env_id, seed=input_seed).unwrapped

@@ -1,8 +1,8 @@
 """Compile the reference's MJCF models into committed fixtures (myosuite_b200/assets/*.npz).
 
-The GPU box has no /root/reference, so the four hot-path models are compiled HERE by this repo's own
+The tests and the GPU runs need no MyoSuite checkout: the hot-path models are compiled by this repo's own
 MJCF compiler from the reference's XML/STL inputs and committed as data fixtures.  Run:
-    python tools/compile_assets.py [/root/reference/myosuite]
+    python tools/compile_assets.py <MyoSuite checkout root>/myosuite
 """
 import os
 import sys
@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from myosuite_b200 import mjcf  # noqa: E402
 from myosuite_b200.assets import MODEL_XML  # noqa: E402
 
-root = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/myosuite"
+root = sys.argv[1]
 out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "myosuite_b200", "assets")
 for name, (rel, kwargs) in MODEL_XML.items():
     m = mjcf.compile_mjcf(os.path.join(root, rel), **kwargs)

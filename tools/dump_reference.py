@@ -1,6 +1,6 @@
 """Dump golden physics vectors from a REAL MuJoCo + the reference's own envs (SURVEY.md section 8c, "plan when MuJoCo becomes importable").
 
-NOT runnable in the build container or on the GPU box of this round (neither has `mujoco` / `gymnasium`): this script is the recipe a
+NOT runnable without `mujoco` and `gymnasium` (neither is a dependency of this project): this script is the recipe a
 maintainer runs once on a machine where `pip install myosuite` works, to turn the oracle's "parity unpinned" status into pinned goldens.
 It uses only the reference's public API (gym.make, env.step) and MuJoCo's Python bindings; nothing from this repository is imported.
 

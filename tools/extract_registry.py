@@ -1,15 +1,15 @@
 """Dump the registry kwargs of the hot-path env ids from the reference into a JSON fixture.
 
-Executes /root/reference/myosuite/envs/myo/myobase/__init__.py UNMODIFIED with `gym.register` and
+Executes myosuite/envs/myo/myobase/__init__.py UNMODIFIED with `gym.register` and
 `register_env_variant` stubbed to recorders (no gym / mujoco needed), and writes
-myosuite_b200/assets/registry.json.  Run:  python tools/extract_registry.py [/root/reference]
+myosuite_b200/assets/registry.json.  Run:  python tools/extract_registry.py <MyoSuite checkout root>
 """
 import json
 import os
 import sys
 import types
 
-ref = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+ref = sys.argv[1]
 src = os.path.join(ref, "myosuite/envs/myo/myobase/__init__.py")
 records, variants = {}, {}
 

@@ -1,4 +1,4 @@
-"""Per-phase SM-cycle breakdown + contact-count histogram over a rollout (developer tool, run under gpurun)."""
+"""Per-phase SM-cycle breakdown + contact-count histogram over a rollout (developer tool; needs a GPU)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -1,4 +1,4 @@
-"""How predictable is an env's solver work from its previous step?  (developer probe for work-sorted env placement; run under gpurun)"""
+"""How predictable is an env's solver work from its previous step?  (developer probe for work-sorted env placement; needs a GPU)"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

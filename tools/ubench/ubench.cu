@@ -1,7 +1,7 @@
-// Latency micro-benchmarks for the quantities the step kernel's cycle model depends on (B200, sm_100a):
+// Latency micro-benchmarks for the quantities the step kernel's cycle model depends on (H100 SXM, sm_90a; one CTA per SM on its 132 SMs):
 // dependent-chain latency of the f64 ops, shared-memory load->use, warp shuffles, and the cost of streaming never-seen
 // straight-line code (instruction fetch) for 1 warp and for 10 lockstep warps per SM.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench ubench.cu && ./ubench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench ubench.cu && ./ubench
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N 256
@@ -47,8 +47,8 @@ int main() {
   for (int r = 0; r < 2; r++) { k_lds<<<1, 32>>>(out, cyc, 7); cudaMemcpy(h, cyc, 8, cudaMemcpyDeviceToHost); } printf("%-10s %7.1f cycles per dependent LDS.64 (pointer chase)\n", "lds", (double)h[0] / N);
   for (int r = 0; r < 2; r++) { k_sts_lds<<<1, 32>>>(out, cyc); cudaMemcpy(h, cyc, 8, cudaMemcpyDeviceToHost); } printf("%-10s %7.1f cycles per STS -> syncwarp -> LDS(other lane) -> DADD -> syncwarp\n", "sts_lds", (double)h[0] / N);
   // instruction streaming: code bodies of 4*REP DFMAs (16 B each)
-  #define CODE(REP) for (int w = 1; w <= 10; w += 9) for (int iters = 1; iters <= 4; iters += 3) { for (int r = 0; r < 2; r++) { k_code<REP><<<148, 32 * w>>>(out, cyc, 1.0, 0.999, iters); cudaMemcpy(h, cyc, 8 * 148, cudaMemcpyDeviceToHost); } \
-      double m = 0; for (int i = 0; i < 148; i++) m += h[i]; m /= 148; printf("code %5d KB  warps/SM %2d  passes %d: %7.2f cycles per instruction (dependent DFMA chain)\n", (REP) * 4 * 16 / 1024, w, iters, m / ((double)(REP) * 4 * iters)); }
+  #define CODE(REP) for (int w = 1; w <= 10; w += 9) for (int iters = 1; iters <= 4; iters += 3) { for (int r = 0; r < 2; r++) { k_code<REP><<<132, 32 * w>>>(out, cyc, 1.0, 0.999, iters); cudaMemcpy(h, cyc, 8 * 132, cudaMemcpyDeviceToHost); } \
+      double m = 0; for (int i = 0; i < 132; i++) m += h[i]; m /= 132; printf("code %5d KB  warps/SM %2d  passes %d: %7.2f cycles per instruction (dependent DFMA chain)\n", (REP) * 4 * 16 / 1024, w, iters, m / ((double)(REP) * 4 * iters)); }
   CODE(256) CODE(2048) CODE(8192) CODE(16384)
   printf("%s\n", cudaGetErrorString(cudaDeviceSynchronize()));
   return 0; }

@@ -1,5 +1,5 @@
 // Isolated timing of the dense solver (row-register LDL') exactly as the step kernel compiles it: cycles per solve for one warp,
-// and with 10 warps per SM (all solving).  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I../../myosuite_b200/csrc -o ubench_chol ubench_chol.cu
+// and with 10 warps per SM (all solving).  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I../../myosuite_b200/csrc -o ubench_chol ubench_chol.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "myo_solver.cuh"
@@ -23,7 +23,7 @@ int main() {
   for (int mode = 0; mode < 2; mode++) for (int w = 1; w <= 10; w += 9) {
     size_t sm = (size_t)w*(23*24/2 + 2*23 + 8)*8;
     cudaFuncSetAttribute(k<23>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    for (int r = 0; r < 2; r++) { k<23><<<148, 32*w, sm>>>(out, cyc, 20, mode); cudaMemcpy(h, cyc, 8*148*w, cudaMemcpyDeviceToHost); }
-    double m = 0; for (int i = 0; i < 148*w; i++) m += h[i]; printf("%s n=23: %d warps/SM: %.0f cycles per solve, x[0..2] check below (%s)\n", mode ? "chol_rs (unrolled)" : "chol_rot (rolled)", w, m/(148*w), cudaGetErrorString(cudaGetLastError())); }
+    for (int r = 0; r < 2; r++) { k<23><<<132, 32*w, sm>>>(out, cyc, 20, mode); cudaMemcpy(h, cyc, 8*132*w, cudaMemcpyDeviceToHost); }
+    double m = 0; for (int i = 0; i < 132*w; i++) m += h[i]; printf("%s n=23: %d warps/SM: %.0f cycles per solve, x[0..2] check below (%s)\n", mode ? "chol_rs (unrolled)" : "chol_rot (rolled)", w, m/(132*w), cudaGetErrorString(cudaGetLastError())); }
   double hx[64]; cudaMemcpy(hx, out, 64*8, cudaMemcpyDeviceToHost); printf("solution head: %.12g %.12g %.12g\n", hx[0], hx[1], hx[2]);
   return 0; }

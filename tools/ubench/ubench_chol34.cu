@@ -1,5 +1,5 @@
 // Isolated timing of the bordered 34 x 34 solve (legs model): shuffle-based chol_reg32b vs the row-register chol_rs32b, and chol_rs<32> for scale.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I../../myosuite_b200/csrc -o ubench_chol34 ubench_chol34.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I../../myosuite_b200/csrc -o ubench_chol34 ubench_chol34.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "myo_solver.cuh"
@@ -22,8 +22,8 @@ int main() {
   for (int mode = 0; mode < 3; mode++) for (int w = 1; w <= 7; w += 6) {
     size_t sm = (size_t)w*(36*37/2 + 2*36 + 8)*8; int n = mode == 2 ? 32 : 34;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    for (int r = 0; r < 2; r++) { k<<<148, 32*w, sm>>>(out, cyc, 20, mode, n); cudaMemcpy(h, cyc, 8*148*w, cudaMemcpyDeviceToHost); }
-    double m = 0; for (int i = 0; i < 148*w; i++) m += h[i];
+    for (int r = 0; r < 2; r++) { k<<<132, 32*w, sm>>>(out, cyc, 20, mode, n); cudaMemcpy(h, cyc, 8*132*w, cudaMemcpyDeviceToHost); }
+    double m = 0; for (int i = 0; i < 132*w; i++) m += h[i];
     double hx[8]; cudaMemcpy(hx, out, 64, cudaMemcpyDeviceToHost);
-    printf("%s n=%d: %d warps/SM: %.0f cycles per solve (%s); x0 %.12g x1 %.12g x32 %.12g\n", nm[mode], n, w, m/(148*w), cudaGetErrorString(cudaGetLastError()), hx[0], hx[2], hx[1]); }
+    printf("%s n=%d: %d warps/SM: %.0f cycles per solve (%s); x0 %.12g x1 %.12g x32 %.12g\n", nm[mode], n, w, m/(132*w), cudaGetErrorString(cudaGetLastError()), hx[0], hx[2], hx[1]); }
   return 0; }

@@ -14,10 +14,10 @@ template <int REP, typename T> __global__ void k_code(T* out, long long* cyc, T 
   long long t1 = clock64(); if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
   T s = 0; for (int j = 0; j < 8; j++) s += x[j]; out[blockIdx.x*blockDim.x + threadIdx.x] = s; }
 template <int REP, typename T> void run(const char* name, void* out, long long* cyc) {
-  long long h[148];
+  long long h[132];
   for (int w = 1; w <= 10; w += 9) for (int iters = 1; iters <= 3; iters += 2) {
-    for (int r = 0; r < 2; r++) { k_code<REP, T><<<148, 32*w>>>((T*)out, cyc, (T)0.999, (T)0.001, iters); cudaMemcpy(h, cyc, 8*148, cudaMemcpyDeviceToHost); }
-    double m = 0; for (int i = 0; i < 148; i++) m += h[i]; m /= 148;
+    for (int r = 0; r < 2; r++) { k_code<REP, T><<<132, 32*w>>>((T*)out, cyc, (T)0.999, (T)0.001, iters); cudaMemcpy(h, cyc, 8*132, cudaMemcpyDeviceToHost); }
+    double m = 0; for (int i = 0; i < 132; i++) m += h[i]; m /= 132;
     printf("%s code %5d KB  warps/SM %2d  passes %d: %6.2f cycles per instruction  (%.2f bytes of code per cycle per SM)\n", name, REP*8*16/1024, w, iters, m/((double)REP*8*iters), (double)REP*8*16*iters/m); } }
 int main() {
   void* out; long long* cyc; cudaMalloc(&out, 1 << 22); cudaMalloc(&cyc, 4096);
