@@ -68,6 +68,11 @@ typedef struct {
   int32_t task_i[16];        /* task-specific indices, filled by the host mirror (vec_env.py): WALK body/joint ids, HOLD object ids, REACH [ntip, tip body x ntip] */
   double task_d[24];         /* task-specific constants: WALK targets / thresholds / torso quaternion offset, HOLD object site, REACH tip-site offsets [3 x ntip] then far_th */
   double reserved[2];        /* [0] != 0 with the phase-cycle tap bound: record the barrier wait before each phase instead of its work (profiling) */
+  /* REACH reward shape: reach = c_off - d - c_vel |qvel dt| ; act_reg = -c_act |act|/na ; bonus thresholds near and 2 near with near = ntip near_per_tip.
+   * {c_off, c_vel, c_act, near_per_tip}; all zero = reach_v0.py:120-160 (0, 0, 1, 0.0125).  The leg stand task (walk_v0.py:104-140) is (10, 10, 100, 0.05). */
+  double reach_shape[4];
+  /* REACH reset, when hi > lo: for every joint j, qpos[jnt_qposadr[j]] = clip(init_qpos[.] + U(lo, hi), jnt_range[j]) (walk_v0.py:142-186) */
+  double joint_random[2];
 } myo_task_cfg;
 
 /* caller-owned device buffers; nullable ones are marked.  f64 state, f32 I/O like the reference

@@ -26,7 +26,8 @@ class MyoDims(ctypes.Structure):
 class MyoTaskCfg(ctypes.Structure):
     _fields_ = [(n, c_i32) for n in ("task", "frame_skip", "max_episode_steps", "normalize_act", "muscle_condition",
                                       "auto_reset", "reset_random", "maxcon", "reaf_dst", "reaf_src", "barrier_mode", "reserved_i", "fatigue_reset")] + \
-               [("pose_thd", c_f64), ("weights", c_f64 * 8), ("solver_tolerance", c_f64), ("task_i", c_i32 * 16), ("task_d", c_f64 * 24), ("reserved", c_f64 * 2)]
+               [("pose_thd", c_f64), ("weights", c_f64 * 8), ("solver_tolerance", c_f64), ("task_i", c_i32 * 16), ("task_d", c_f64 * 24), ("reserved", c_f64 * 2),
+                ("reach_shape", c_f64 * 4), ("joint_random", c_f64 * 2)]
 
 
 BUFFER_FIELDS = ["action", "qpos", "qvel", "act", "qacc_warmstart", "time", "fatigue", "target", "target_range", "init_qpos", "init_qvel", "env_prm",

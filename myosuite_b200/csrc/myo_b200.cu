@@ -89,6 +89,14 @@ __device__ void env_reset(const DevModel& m, const Warp w, const StepArgs& a, in
       if (b.target && b.target_range) b.target[(size_t)env*m.nq+qa] = b.target_range[2*qa] + u0*(b.target_range[2*qa+1]-b.target_range[2*qa]);
       if (a.cfg.reset_random) W_(qpos)[qa] = jrange[2*j] + u1*(jrange[2*j+1]-jrange[2*j]); }
   }
+  if (a.cfg.task == MYO_TASK_REACH && a.cfg.joint_random[1] > a.cfg.joint_random[0]) {
+    // ReachEnvV0.generate_qpos (walk_v0.py:152-167): the first qpos coordinate of EVERY joint (the free root's x included) += U(lo, hi), then
+    // clipped to jnt_range whether or not the joint is limited.  Rounded as numpy's uniform (low + (high - low) u) and sum, without FMA.
+    const double lo = a.cfg.joint_random[0], span = a.cfg.joint_random[1] - lo;
+    for (int j = w.lane; j < m.njnt; j += 32) { const int qa = jq[j];
+      const double q = __dadd_rn(W_(qpos)[qa], __dadd_rn(lo, __dmul_rn(span, philox_uniform(rng))));
+      W_(qpos)[qa] = fmin(fmax(q, jrange[2*j]), jrange[2*j+1]); }
+    __syncwarp(); }
   if (a.cfg.task == MYO_TASK_REACH && b.target && b.target_range) {
     // ReachEnvV0.generate_target_pose (reach_v0.py:163-170): every target site ~ U(span) per coordinate
     for (int k = w.lane; k < 3*a.cfg.task_i[0]; k += 32) { double u = philox_uniform(rng); b.target[(size_t)env*m.nq+k] = b.target_range[2*k] + u*(b.target_range[2*k+1]-b.target_range[2*k]); } }
@@ -190,6 +198,11 @@ __device__ void hold_observe(const DevModel& m, const Warp w, const StepArgs& a,
   *done_out = drop;
 }
 
+// |qvel dt| of the state in shared memory (the leg stand task's velocity term); out of line, so that the reach epilogue keeps its registers
+__device__ __noinline__ double qvel_dt_norm(const DevModel& m, const Warp w, const StepArgs& a) {
+  double v2 = 0; for (int i = w.lane; i < m.nv; i += 32) { const double v = W_(qvel)[i]*a.dt; v2 += v*v; }
+  return sqrt(warp_sum(v2)); }
+
 // ReachEnvV0 obs / reward / done (reach_v0.py:98-160): needs kinematics of the post-step state in scratch.  tnow = mjData.time of that state
 __device__ void reach_observe(const DevModel& m, const Warp w, const StepArgs& a, int env, double tnow, double* rw_out, bool* done_out) {
   const myo_buffers& b = a.b; const int* ti = a.cfg.task_i; const double* td = a.cfg.task_d; const int ntip = ti[0];
@@ -201,9 +214,13 @@ __device__ void reach_observe(const DevModel& m, const Warp w, const StepArgs& a
   if (o) { for (int i = w.lane; i < m.nq; i += 32) o[i] = (float)W_(qpos)[i]; for (int i = w.lane; i < m.nv; i += 32) o[m.nq+i] = (float)(W_(qvel)[i]*a.dt); }
   for (int i = w.lane; i < m.na; i += 32) { a2 += W_(act)[i]*W_(act)[i]; if (o) o[base + 6*ntip + i] = (float)W_(act)[i]; }      // base_v0.py:33-37 appends "act"
   double dist = sqrt(warp_sum(d2)), am = sqrt(warp_sum(a2)); if (m.na) am /= m.na;
+  // reward shape: reach_v0.py (all zero) or the leg stand task's 10 - d - 10 |qvel dt|, 100 act_reg and 0.05 near threshold (walk_v0.py:104-140)
+  const double* rs = a.cfg.reach_shape;
+  double reach = -dist, c_act = 1.0, near_tip = 0.0125;
+  if (rs[3] != 0) { reach = rs[0] - dist - (rs[1] != 0 ? rs[1]*qvel_dt_norm(m, w, a) : 0.0); c_act = rs[2]; near_tip = rs[3]; }
   bool armed = tnow > 2*a.dt;                                   // far_th = inf for the first control steps (reach_v0.py:134-138)
-  double far_th = td[3*ntip]*ntip, near_th = ntip*0.0125; bool far = armed && dist > far_th;
-  *rw_out = a.cfg.weights[0]*(-dist) + a.cfg.weights[1]*((dist < 2*near_th ? 1.0 : 0.0) + (dist < near_th ? 1.0 : 0.0)) + a.cfg.weights[2]*(-am) + a.cfg.weights[3]*(far ? -1.0 : 0.0);
+  double far_th = td[3*ntip]*ntip, near_th = ntip*near_tip; bool far = armed && dist > far_th;
+  *rw_out = a.cfg.weights[0]*reach + a.cfg.weights[1]*((dist < 2*near_th ? 1.0 : 0.0) + (dist < near_th ? 1.0 : 0.0)) + a.cfg.weights[2]*(-c_act*am) + a.cfg.weights[3]*(far ? -1.0 : 0.0);
   *done_out = far;
 }
 

@@ -3,7 +3,7 @@
 What the reference exposes on `env.unwrapped` and its tests exercise (myosuite/tests/test_envs.py:54-123):
   action_space / observation_space      envs/env_base.py:145-155, 210-218      (Box(-1, 1, nu) f32 ; Box(-10, 10, obs_dim) f32)
   obs_dict / rwd_dict                   envs/env_base.py:409-432               (per-key views of the observation; reward terms)
-  get_obs_dict / get_reward_dict        myobase/pose_v0.py:100-140, reach_v0.py:98-160, obj_hold_v0.py:79-121, walk_v0.py:268-319
+  get_obs_dict / get_reward_dict        myobase/pose_v0.py:100-140, reach_v0.py:98-160, obj_hold_v0.py:79-121, walk_v0.py:80-140,268-319
   get_env_infos                         envs/env_base.py:585-616
   get_env_state / set_env_state         envs/env_base.py:688-759
   seed / get_input_seed / pickling      envs/env_base.py:119-123, gym.utils.EzPickle (pose_v0.py:32)
@@ -72,7 +72,7 @@ def obs_layout(task, nq, nv, na, ntip=0):
     """[(key, width)] in the order of the reference's DEFAULT_OBS_KEYS + "act" (base_v0.py:33-37)."""
     if task == "pose":
         return [("qpos", nq), ("qvel", nv), ("pose_err", nq), ("act", na)]
-    if task == "reach":
+    if task in ("reach", "stand"):
         return [("qpos", nq), ("qvel", nv), ("tip_pos", 3 * ntip), ("reach_err", 3 * ntip), ("act", na)]
     if task == "hold":
         return [("hand_qpos", nq - 7), ("hand_qvel", nv - 6), ("obj_pos", 3), ("obj_err", 3), ("act", na)]
@@ -94,7 +94,7 @@ def obs_dict_from_vec(task, obs, time, nq, nv, na, ntip=0):
 
 # --------------------------------------------------------------------------------------------- rwd_dict
 def reward_dict(task, obs_dict, weights, cfg):
-    """The reference's get_reward_dict for the four device tasks, on an obs_dict (batched over leading dims).
+    """The reference's get_reward_dict for the device tasks, on an obs_dict (batched over leading dims).
     cfg: task constants (pose_thd ; far_th, ntip, dt ; walk targets, hip_period ...).  Returns OrderedDict incl. sparse / solved / done / dense."""
     na = obs_dict["act"].shape[-1]
     act_mag = np.linalg.norm(obs_dict["act"], axis=-1) / na if na else 0.0
@@ -107,6 +107,11 @@ def reward_dict(task, obs_dict, weights, cfg):
         far_th = np.where(np.asarray(obs_dict["time"]) > 2 * cfg["dt"], cfg["far_th"] * ntip, np.inf); near = ntip * 0.0125
         r = collections.OrderedDict((("reach", -1.0 * d), ("bonus", 1.0 * (d < 2 * near) + 1.0 * (d < near)), ("act_reg", -1.0 * act_mag), ("penalty", -1.0 * (d > far_th)),
                                      ("sparse", -1.0 * d), ("solved", d < near), ("done", d > far_th)))
+    elif task == "stand":                                                  # walk_v0.py:104-140 (ReachEnvV0 of the legs)
+        d = np.linalg.norm(obs_dict["reach_err"], axis=-1); v = np.linalg.norm(obs_dict["qvel"], axis=-1); ntip = cfg["ntip"]
+        far_th = np.where(np.squeeze(obs_dict["time"]) > 2 * cfg["dt"], cfg["far_th"] * ntip, np.inf); near = ntip * 0.050       # (squeezed as the reference does)
+        r = collections.OrderedDict((("reach", 10.0 - 1.0 * d - 10.0 * v), ("bonus", 1.0 * (d < 2 * near) + 1.0 * (d < near)), ("act_reg", -100.0 * act_mag),
+                                     ("penalty", -1.0 * (d > far_th)), ("sparse", -1.0 * d), ("solved", d < near), ("done", d > far_th)))
     elif task == "hold":                                                   # obj_hold_v0.py:92-121
         d = np.abs(np.linalg.norm(obs_dict["obj_err"], axis=-1)); th = 0.010; drop = d > 0.300
         r = collections.OrderedDict((("goal_dist", -1.0 * d), ("bonus", 1.0 * (d < 2 * th) + 1.0 * (d < th)), ("act_reg", -1.0 * act_mag), ("penalty", -1.0 * drop),
@@ -134,6 +139,7 @@ def reward_dict(task, obs_dict, weights, cfg):
 DEFAULT_WEIGHTS = {
     "pose": {"pose": 1.0, "bonus": 4.0, "act_reg": 1.0, "penalty": 50},                                               # pose_v0.py:18-23
     "reach": {"reach": 1.0, "bonus": 4.0, "penalty": 50},                                                              # reach_v0.py:18-22
+    "stand": {"reach": 1.0, "bonus": 4.0, "penalty": 50, "act_reg": 1},                                              # walk_v0.py:18-24
     "hold": {"goal_dist": 100.0, "bonus": 4.0, "penalty": 10},                                                         # obj_hold_v0.py:17-21
     "walk": {"vel_reward": 5.0, "done": -100, "cyclic_hip": -10, "ref_rot": 10.0, "joint_angle_rew": 5.0},          # walk_v0.py:205-211
 }
@@ -156,7 +162,7 @@ def compute_path_rewards(task, paths, key_widths, weights, cfg, rwd_mode="dense"
     """MujocoEnv.compute_path_rewards (env_base.py:763-780): vectorised rewards / done flags of paths["observations"] [num_traj, horizon, obs_dim],
     time-aligned the way the reference does it (entry t takes the value computed from observation t+1; the last entry is redundant)."""
     od = obsvec2obsdict(paths["observations"], key_widths)
-    if task == "reach" and "time" not in od:
+    if task in ("reach", "stand") and "time" not in od:
         raise KeyError("the reach reward needs obs_dict['time'] (reach_v0.py:127-131), which an observation vector does not carry")
     rd = reward_dict(task, od, weights, cfg)
     rewards, done = np.array(rd[rwd_mode], dtype=np.float64), np.array(rd["done"])

@@ -4,6 +4,7 @@ lazily from it (numpy arrays or torch tensors, any device) instead of costing th
 
   pose  (pose_v0.py:113-140):     dist = |pose_err|,   sparse = -dist, solved = dist < pose_thd
   reach (reach_v0.py:120-160):    dist = |reach_err|,  sparse = -dist, solved = dist < 0.0125 * ntip
+  stand (walk_v0.py:104-140):     dist = |reach_err|,  sparse = -dist, solved = dist < 0.050 * ntip
   hold  (obj_hold_v0.py:92-121):  dist = |obj_err|,    sparse = -dist, solved = dist < 0.010
 """
 
@@ -20,9 +21,9 @@ def info_from_obs(task, obs, nq, nv, na, pose_thd=None, ntip=None):
     distance-type success signal (walk)."""
     if task == "pose":
         err, thd = obs[..., nq + nv:nq + nv + nq], pose_thd
-    elif task == "reach":
+    elif task in ("reach", "stand"):
         base = nq + nv + 3 * ntip
-        err, thd = obs[..., base:base + 3 * ntip], 0.0125 * ntip
+        err, thd = obs[..., base:base + 3 * ntip], (0.0125 if task == "reach" else 0.050) * ntip
     elif task == "hold":
         base = (nq - 7) + (nv - 6) + 3
         err, thd = obs[..., base:base + 3], 0.010

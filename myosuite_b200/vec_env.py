@@ -47,6 +47,32 @@ def registered_ids():
 _MODEL_OF_XML = {v[0]: k for k, v in assets.MODEL_XML.items()}
 
 
+def stand_target_centre(m, tips, init_qpos):
+    """[ntip, 3] world positions the leg stand task samples its targets around.  The reference samples them around the tip sites of
+    a first generate_qpos() draw (walk_v0.py:142-174), then starts the episode from an independent second draw.  That centre is a
+    constant only when no draw moves a tip site: every joint between a tip's body and the world has a range of zero width (the draw
+    clips the one coordinate it touches to that range; the other coordinates of a free or ball joint keep init_qpos).  On the legs
+    the pelvis hangs from the free root, whose range [0, 0] pins x.  Any other structure raises instead of sampling a different
+    distribution."""
+    from . import mjcf
+    q = np.array(init_qpos, dtype=np.float64)
+    for j in range(m.njnt):                         # the first draw, on the coordinates it pins
+        if m.jnt_range[j][0] == m.jnt_range[j][1]:
+            q[m.jnt_qposadr[j]] = m.jnt_range[j][0]
+    kin, centre = mjcf.kinematics(m, q), []
+    for name in tips:
+        sid = m.name2id("site", name)
+        b = int(m.site_bodyid[sid])
+        while b != 0:
+            for j in range(int(m.body_jntadr[b]), int(m.body_jntadr[b]) + int(m.body_jntnum[b])):
+                if m.jnt_range[j][0] != m.jnt_range[j][1]:
+                    raise NotImplementedError("stand task: joint %d moves tip site %r under the randomised reset, so its target centre is not constant" % (j, name))
+            b = int(m.body_parentid[b])
+        b = int(m.site_bodyid[sid])
+        centre.append(kin["xpos"][b] + np.reshape(kin["xmat"][b], (3, 3)) @ m.site_pos[sid])
+    return np.array(centre)
+
+
 class MyoVecEnv:
     """n independent envs of one registry id, resident on one GPU.  Tensors in, tensors out."""
 
@@ -70,10 +96,14 @@ class MyoVecEnv:
         self.kwargs = kw
         self._check_kwargs(kw)
         self.torso = entry is not None and entry.endswith("torso_v0:TorsoEnvV0")        # TorsoEnvV0 = the pose task with a fixed mean-of-range target, far_th = pi, pose_thd 0.25
+        # "stand": walk_v0.py's ReachEnvV0 (myoLegStandRandom), the device's reach task with its own reward shape and randomised joint reset
         self.task = ("none" if entry is None else "pose" if (entry.endswith("pose_v0:PoseEnvV0") or self.torso) else "walk" if entry.endswith("walk_v0:WalkEnvV0")
-                     else "hold" if "obj_hold_v0:ObjHold" in entry else "reach" if entry.endswith("reach_v0:ReachEnvV0") else None)
+                     else "hold" if "obj_hold_v0:ObjHold" in entry else "reach" if entry.endswith("reach_v0:ReachEnvV0")
+                     else "stand" if entry.endswith("walk_v0:ReachEnvV0") else None)
         if self.task is None:
-            raise NotImplementedError("device task for %s (%s) is not built yet (pose, torso, walk, hold, reach are; MyoVecEnv.from_model gives physics only)" % (env_id, entry))
+            raise NotImplementedError("device task for %s (%s) is not built yet (pose, torso, walk, hold, reach, stand are; MyoVecEnv.from_model gives physics only)" % (env_id, entry))
+        if kw.get("joint_random_range") is not None and self.task != "stand":
+            raise NotImplementedError("joint_random_range is implemented for the leg stand task (walk_v0.py ReachEnvV0) only")
         self.hold_random = entry is not None and entry.endswith("ObjHoldRandomEnvV0")
         self.mj_model = m = model if model is not None else assets.load(_MODEL_OF_XML[kw["model_path"]])
         self.muscle_condition = kw.get("muscle_condition", "")
@@ -94,7 +124,7 @@ class MyoVecEnv:
             raise ValueError("row_storage must be 'p48' or 'f64'")
         self.dev_model = abi.DeviceModel(self.I, self.D, variant="f64rows" if self.row_storage == "f64" else None)
         cfg = abi.MyoTaskCfg()
-        cfg.task = {"none": abi.TASK_NONE, "pose": abi.TASK_POSE, "walk": abi.TASK_WALK, "hold": abi.TASK_HOLD, "reach": abi.TASK_REACH}[self.task]
+        cfg.task = {"none": abi.TASK_NONE, "pose": abi.TASK_POSE, "walk": abi.TASK_WALK, "hold": abi.TASK_HOLD, "reach": abi.TASK_REACH, "stand": abi.TASK_REACH}[self.task]
         cfg.frame_skip = self.n_frames
         cfg.max_episode_steps = int(self.max_episode_steps or 0)
         cfg.normalize_act = int(bool(kw.get("normalize_act", True)))
@@ -131,10 +161,13 @@ class MyoVecEnv:
                 cfg.weights[i] = w[k]
             init_qpos[:-7] = 0.0; init_qpos[0] = -1.5                                                  # obj_hold_v0.py:61-62
             cfg.reset_random = int(self.hold_random)
-        elif self.task == "reach":
-            w = kw.get("weighted_reward_keys", {"reach": 1.0, "bonus": 4.0, "penalty": 50})                 # reach_v0.py:18-22
+        elif self.task in ("reach", "stand"):
+            w = kw.get("weighted_reward_keys", {"reach": 1.0, "bonus": 4.0, "penalty": 50} if self.task == "reach"      # reach_v0.py:18-22
+                       else {"reach": 1.0, "bonus": 4.0, "penalty": 50, "act_reg": 1})                                     # walk_v0.py:18-24
             for i, k in enumerate(("reach", "bonus", "act_reg", "penalty")):
                 cfg.weights[i] = w.get(k, 0.0)
+            if self.task == "stand":     # walk_v0.py:65-66: init_qpos / init_qvel = keyframe 0
+                init_qpos, init_qvel = m.key_qpos[0].copy(), m.key_qvel[0].copy()
         cfg.solver_tolerance = float(kw.get("solver_tolerance", 0.0))
         cfg.maxcon = int(kw.get("maxcon", 0))
         cfg.barrier_mode = int(kw.get("barrier_mode", 0))
@@ -145,8 +178,10 @@ class MyoVecEnv:
             cfg.reaf_dst, cfg.reaf_src = m.name2id("actuator", "EPL"), m.name2id("actuator", "EIP")
         if self.task == "hold":
             self._setup_hold(m, cfg)
-        if self.task == "reach":
+        if self.task in ("reach", "stand"):
             self._setup_reach(m, kw, cfg)
+        if self.task == "stand":
+            self._setup_stand(m, kw, cfg, init_qpos)
         self.cfg = cfg
         self.device_index = int(device)
         self.device = torch.device("cuda", self.device_index)
@@ -189,9 +224,10 @@ class MyoVecEnv:
         elif kw.get("target_jnt_value") is not None:
             v = np.asarray(kw["target_jnt_value"], dtype=np.float64)
             tr[:, 0] = tr[:, 1] = v
-        elif self.task == "reach":       # rows 3k..3k+2: span of target site k (reach_v0.py:163-170); `target` rows hold the sampled site positions
-            for k, span in enumerate(kw["target_reach_range"].values()):
-                tr[3 * k:3 * k + 3, 0], tr[3 * k:3 * k + 3, 1] = span[0], span[1]
+        elif self.task in ("reach", "stand"):       # rows 3k..3k+2: span of target site k (reach_v0.py:163-170); `target` rows hold the sampled site positions
+            for k, span in enumerate(kw["target_reach_range"].values()):         # stand: around the constant tip position of the first draw (walk_v0.py:142-150)
+                c = self.target_center[k] if self.task == "stand" else 0.0
+                tr[3 * k:3 * k + 3, 0], tr[3 * k:3 * k + 3, 1] = c + np.asarray(span[0], dtype=np.float64), c + np.asarray(span[1], dtype=np.float64)
         t["target_range"] = torch.as_tensor(tr, device=dv).contiguous()
         t["init_qpos"] = torch.as_tensor(init_qpos, device=dv).contiguous()
         t["init_qvel"] = torch.as_tensor(init_qvel, device=dv).contiguous()
@@ -223,7 +259,7 @@ class MyoVecEnv:
     # kwargs of the reference's env classes this backend implements; anything else with a non-default value is an error, not a silent no-op
     _KNOWN = {"model_path", "normalize_act", "frame_skip", "muscle_condition", "reset_type", "target_type", "pose_thd", "weighted_reward_keys", "target_jnt_range",
               "target_jnt_value", "viz_site_targets", "target_reach_range", "far_th", "min_height", "max_rot", "hip_period", "target_x_vel", "target_y_vel", "target_rot",
-              "obs_keys", "fatigue_reset_vec", "fatigue_reset_random", "weight_bodyname", "weight_range",
+              "obs_keys", "fatigue_reset_vec", "fatigue_reset_random", "weight_bodyname", "weight_range", "joint_random_range",
               # backend knobs
               "solver_tolerance", "maxcon", "barrier_mode", "lockstep_groups", "profile_waits", "row_storage"}
 
@@ -284,6 +320,18 @@ class MyoVecEnv:
                 cfg.task_d[3 * k + c] = float(m.site_pos[sid][c])
         cfg.task_d[3 * len(tips)] = float(kw.get("far_th", 0.35))
         self.tip_names = tips
+
+    STAND_SHAPE = (10.0, 10.0, 100.0, 0.05)      # walk_v0.py:104-140: reach = 10 - d - 10 |qvel dt|, act_reg = -100 |act|/na, near_th = 0.05 ntip
+
+    def _setup_stand(self, m, kw, cfg, init_qpos):
+        """walk_v0.py ReachEnvV0 (walk_v0.py:49-79,104-186): reward shape, randomised joint reset, target centre (stand_target_centre)."""
+        lo, hi = (float(x) for x in kw.get("joint_random_range", (0.0, 0.0)))
+        if not hi > lo:
+            raise NotImplementedError("stand task without joint randomisation: the reference then samples the target around the previous episode's last state")
+        for i, v in enumerate(self.STAND_SHAPE):
+            cfg.reach_shape[i] = v
+        cfg.joint_random[0], cfg.joint_random[1] = lo, hi
+        self.target_center = stand_target_centre(m, self.tip_names, init_qpos)
 
     def _setup_hold(self, m, cfg):
         """ObjHold constants (obj_hold_v0.py:46-62,126-145)."""
@@ -630,7 +678,7 @@ def register_gym():
     for eid in registered_ids():
         try:
             steps, _, entry = env_spec(eid)
-            if not any(entry.endswith(x) for x in ("pose_v0:PoseEnvV0", "walk_v0:WalkEnvV0", "reach_v0:ReachEnvV0", "torso_v0:TorsoEnvV0")) and "obj_hold_v0:ObjHold" not in entry:
+            if not any(entry.endswith(x) for x in ("pose_v0:PoseEnvV0", "walk_v0:WalkEnvV0", "reach_v0:ReachEnvV0", "torso_v0:TorsoEnvV0", "walk_v0:ReachEnvV0")) and "obj_hold_v0:ObjHold" not in entry:
                 continue
             g.register(id=eid, entry_point="myosuite_b200.vec_env:MyoEnv", max_episode_steps=steps, kwargs={"env_id": eid})
             done.append(eid)

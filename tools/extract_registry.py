@@ -33,7 +33,8 @@ g = {"__file__": src, "__name__": "myobase_registry"}
 exec(compile(open(src).read(), src, "exec"), g)
 
 WANT = ["myoElbowPose1D6MRandom-v0", "myoHandPoseRandom-v0", "myoLegWalk-v0", "myoHandObjHoldRandom-v0",
-        "myoElbowPose1D6MFixed-v0", "myoHandPoseFixed-v0", "myoHandObjHoldFixed-v0", "myoHandReachFixed-v0", "myoHandReachRandom-v0", "myoTorsoPoseFixed-v0"]
+        "myoElbowPose1D6MFixed-v0", "myoHandPoseFixed-v0", "myoHandObjHoldFixed-v0", "myoHandReachFixed-v0", "myoHandReachRandom-v0", "myoTorsoPoseFixed-v0",
+        "myoLegStandRandom-v0"]
 pkg = os.path.join(ref, "myosuite")
 
 
