@@ -91,7 +91,7 @@ typedef struct {
   const double* init_qvel;   /* [nv]     reset velocity (nullable = zeros), in ([2,nv] alongside a [2,nq] init_qpos) */
   double* env_prm;           /* [n, 8]   per-env model overrides (HOLD: goal site pos[3], object geom size[3]); nullable */
   int32_t* step_count;       /* [n] */
-  int64_t* episode_count;    /* [n]  also the Philox stream counter */
+  int64_t* episode_count;    /* [n]  also keys the reset's Philox streams (myo_batch_reset) */
   float* obs;                /* [n, obs_dim] out */
   float* reward;             /* [n] out (rwd_dense) */
   uint8_t* done;             /* [n] out (terminated) */
@@ -129,7 +129,12 @@ void myo_batch_destroy(myo_batch* b);
 int myo_batch_obs_dim(const myo_batch* b);
 
 /* Reset envs whose mask byte is non-zero (mask == NULL: all).  Per-env Philox streams keyed
- * (seed, env_offset + env, episode_count).  Replaces env.reset() (pose_v0.py:174-257, robot.py:996-1002). */
+ * (seed, env_offset + env, episode_count).  Replaces env.reset() (pose_v0.py:174-257, robot.py:996-1002).
+ * Each lane of an env's warp draws from its own Philox4x32-10 stream: key (k0, k1) = (seed lo, seed hi), counter
+ *   c0 = draw block    c1 = lane | (u32)(env >> 20) << 5    c2 = (u32)env ^ (u32)(episode << 20)    c3 = (u32)(env >> 32) ^ (u32)(episode >> 12) ^ 0x4D594F42
+ * with env the global index env_offset + i.  Distinct (seed, env, episode, lane) get distinct streams for env < 2^47 and episode < 2^44;
+ * below 2^20 envs, c1 is the lane alone.  The call fails when env_offset < 0 or env_offset + n_env > MYO_RESET_ENV_LIMIT. */
+#define MYO_RESET_ENV_LIMIT (1LL << 47)
 int myo_batch_reset(myo_batch* b, const uint8_t* mask_dev_or_null, uint64_t seed, int64_t env_offset, void* stream);
 
 /* One control step for every env: action->ctrl, [fatigue], frame_skip x (forward + Euler), obs,

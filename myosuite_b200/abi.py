@@ -4,6 +4,7 @@ Host code stays Python over torch tensors: tensors are passed as ``data_ptr()`` 
 cross the ABI.  There is NO CPU fallback: if the library or a CUDA device is missing the calls raise.
 """
 import ctypes
+import operator
 import os
 
 import numpy as np
@@ -15,6 +16,7 @@ _LIB = None
 c_i32, c_i64, c_u64, c_f64, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64, ctypes.c_double, ctypes.c_void_p
 
 TASK_NONE, TASK_POSE, TASK_WALK, TASK_HOLD, TASK_REACH = 0, 1, 2, 3, 4
+RESET_ENV_LIMIT = 1 << 47           # MYO_RESET_ENV_LIMIT: global env ids below it key distinct reset streams
 COND_NONE, COND_FATIGUE = 0, 2
 
 
@@ -156,6 +158,14 @@ class Batch:
         _check(self.L.myo_batch_bind(self.handle, ctypes.byref(b)), self.L)
 
     def reset(self, mask=None, seed=0, env_offset=0, stream=None):
+        """Reset the masked envs (all when mask is None) from the Philox streams of (seed, env_offset + env, episode_count): seed in
+        [0, 2^64), global env ids in [0, 2^47) (RESET_ENV_LIMIT), where distinct keys give distinct streams.  Checked here, before ctypes
+        would wrap an out-of-range integer into another key."""
+        seed, env_offset = operator.index(seed), operator.index(env_offset)
+        if not 0 <= seed < 1 << 64:
+            raise ValueError("reset seed must be in [0, 2**64), got %d" % seed)
+        if env_offset < 0 or env_offset + self.n_env > RESET_ENV_LIMIT:
+            raise ValueError("env_offset must be in [0, 2**47 - n_env] = [0, %d], got %d" % (RESET_ENV_LIMIT - self.n_env, env_offset))
         _check(self.L.myo_batch_reset(self.handle, mask.data_ptr() if mask is not None else None, seed, env_offset, stream), self.L)
 
     def step(self, stream=None):

@@ -39,8 +39,10 @@ __device__ __forceinline__ void philox_gen(Philox& p) {
     uint32_t n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0; c0 = n0; c1 = n1; c2 = n2; c3 = n3;
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
   p.o0 = c0; p.o1 = c1; p.o2 = c2; p.o3 = c3; p.have = 4; if (++p.c0 == 0) ++p.c1; }
+// Stream key (include/myo_b200.h, myo_batch_reset): c1 carries the lane and env bits 20-46, c2 env bits 0-19 and, above them, episode bits
+// 0-11, c3 env bits 32-63 and episode bits 12-43.  Injective for env < 2^47, episode < 2^44, lane < 32; c1 == lane for env < 2^20.
 __device__ __forceinline__ void philox_init(Philox& p, unsigned long long seed, unsigned long long env, unsigned long long episode, uint32_t lane) {
-  p.k0 = (uint32_t)seed; p.k1 = (uint32_t)(seed >> 32); p.c0 = 0; p.c1 = lane; p.c2 = (uint32_t)env ^ (uint32_t)(episode << 20); p.c3 = (uint32_t)(env >> 32) ^ (uint32_t)(episode >> 12) ^ 0x4D594F42u; p.have = 0; }
+  p.k0 = (uint32_t)seed; p.k1 = (uint32_t)(seed >> 32); p.c0 = 0; p.c1 = lane | ((uint32_t)(env >> 20) << 5); p.c2 = (uint32_t)env ^ (uint32_t)(episode << 20); p.c3 = (uint32_t)(env >> 32) ^ (uint32_t)(episode >> 12) ^ 0x4D594F42u; p.have = 0; }
 __device__ __noinline__ double philox_uniform(Philox& p) {   // [0,1) with 53 random bits; consumes the outputs in pairs (0,1) then (2,3)
   if (p.have < 2) philox_gen(p);
   uint32_t a = p.have == 4 ? p.o0 : p.o2, b = p.have == 4 ? p.o1 : p.o3; p.have -= 2;
@@ -675,6 +677,7 @@ extern "C" int myo_batch_step(myo_batch* b, void* stream) {
 }
 extern "C" int myo_batch_reset(myo_batch* b, const uint8_t* mask, uint64_t seed, int64_t env_offset, void* stream) {
   if (!b) return fail("null batch");
+  if (env_offset < 0 || env_offset > MYO_RESET_ENV_LIMIT - b->n_env) return fail("myo_batch_reset: env_offset must be in [0, 2^47 - n_env] (global env ids key the reset streams)");
   StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 2; a.reset_mask = mask; b->seed = seed; b->env_offset = env_offset;
   return launch(b, a, stream);
 }
