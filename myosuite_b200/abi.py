@@ -69,7 +69,7 @@ def lib(variant=None):
             _VARIANTS[variant] = _bind(ctypes.CDLL(path))
         return _VARIANTS[variant]
     if _LIB is None:
-        path = os.environ.get("MYO_B200_LIB") or _build.LIB      # MYO_B200_LIB: a variant build (developer experiments)
+        path = _build.LIB
         if not os.path.exists(path):
             path = _build.build()
         _LIB = _bind(ctypes.CDLL(path))

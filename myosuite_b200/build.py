@@ -35,7 +35,7 @@ def build(force=False, verbose=False):
 
 
 def build_variant(tag, defines, verbose=False):
-    """libmyo_b200_<tag>.so with extra -D flags (VARIANTS above; also register-budget experiments selected at run time by MYO_B200_LIB)."""
+    """libmyo_b200_<tag>.so with extra -D flags (VARIANTS above)."""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     out = variant_path(tag)
     subprocess.check_call([nvcc] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + ["-o", out, SRC])

@@ -10,10 +10,8 @@
 #include "myo_solver.cuh"
 
 // ------------------------------------------------------------------ kernel arguments
-#ifndef MYO_BMASK
 #define MYO_BMASK 0x40      /* phases of the product kernels that start with a CTA barrier (bit k = phase k).  0x40: only the solver entry, whose inner
                                barriers need aligned warps anyway; with load-sorted rounds the warps of a CTA stay close without the other phase barriers. */
-#endif
 struct StepArgs {
   myo_buffers b; myo_task_cfg cfg;
   int n_env, obs_dim, mode;     // mode 0: env step ; 1: debug forward (ctrl verbatim, optional substeps) ; 2: reset only
@@ -28,6 +26,7 @@ struct StepArgs {
   unsigned long long seed; long long env_offset;
   double tol, dt;
 };
+static const int LOAD_WN = 2, LOAD_WI = 3;      // the load key's weights (StepArgs.load_wn / load_wi) for the product kernels' env steps
 
 // ------------------------------------------------------------------ Philox4x32-10 (counter-based RNG, one stream per (seed, env, episode))
 struct Philox { uint32_t c0, c1, c2, c3, k0, k1, o0, o1, o2, o3; int have; };   // scalars only: indexed arrays would live in local memory
@@ -342,12 +341,8 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
       PH(3, phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w));
       PH(4, phase_collision(m, w); overflow_seen |= WI_(overflow));
       PH(5, phase_constraints(m, w); if (tap) write_taps_contacts(m, w, a, env));
-#ifdef MYO_SOLVE_NOSYNC
-      const bool solver_aligned = DBG && ngroups == 1 && m.solve_sync;
-#else
-      const bool solver_aligned = ngroups == 1 && (!DBG || m.solve_sync);
-#endif
-      if (solver_aligned) {   // every warp enters the solver: its inner CTA barriers need the idle warps too (the unaligned variant is a debug-kernel experiment)
+      const bool solver_aligned = ngroups == 1;
+      if (solver_aligned) {   // every warp enters the solver: its inner CTA barriers need the idle warps too (lockstep groups run it unaligned)
         long long tb_ = prof ? clock64() : 0; if (bmask & (1 << 6)) __syncthreads(); long long t0_ = prof ? clock64() : 0;
         phase_solve(m, w, a.tol, (prof && live) ? cyc : nullptr, live, true);
         if (prof) cyc[6] += waitprof ? t0_ - tb_ : clock64() - t0_;
@@ -386,36 +381,15 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
     }
   }
 }
-// product kernel: up to 10 env-warps per CTA (204 registers per thread)
-// Register budget of the product kernel.  ptxas keeps ~36 registers back for the callees of a kernel that makes ABI calls: the entry function
-// gets 168 under launch_bounds(320) (10 env-warps per CTA) and 128 under launch_bounds(448) (14).  __maxnreg__(200) spills a third as much
-// but the kernel then launches with at most 8 warps per CTA (measured round 2: "too many resources requested" at 9).
-#if defined(MYO_LB_MODE) && MYO_LB_MODE == 0
-#define MYO_LB __maxnreg__(200)
-#elif defined(MYO_LB_MODE) && MYO_LB_MODE == 3
-#define MYO_LB __launch_bounds__(448)
-#elif defined(MYO_LB_MODE) && MYO_LB_MODE == 4
-#define MYO_LB __launch_bounds__(384)
-#else
-#define MYO_LB __launch_bounds__(320)
-#endif
-extern "C" __global__ void MYO_LB myo_env_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320>(m, a); }
+// product kernel: up to 10 env-warps per CTA.  ptxas keeps ~36 registers back for the callees of a kernel that makes ABI calls: the entry
+// function gets 168 under launch_bounds(320) and 128 under launch_bounds(448) (14).  __maxnreg__(200) spills a third as much but the kernel
+// then launches with at most 8 warps per CTA (measured round 2: "too many resources requested" at 9).
+extern "C" __global__ void __launch_bounds__(320) myo_env_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320>(m, a); }
 // the same product body under launch_bounds(448): 128 registers for the entry function, up to 14 env-warps per CTA.  Chosen when the model's
 // shared-memory footprint lets that many warps cut the number of rounds (hand, 4096 envs: 2 rounds of 14 instead of 3 of 10).
-#ifndef MYO_EXPERIMENT_NO_W14
-#ifndef MYO_W14_REGS
-#define MYO_W14_REGS 144
-#endif
 extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
-#else
-#define myo_env_kernel_w14 myo_env_kernel
-#endif
 // parity taps / forward-debug / profiling counters / tuning knobs
-#ifndef MYO_EXPERIMENT_NO_DBG     // (compile-time experiments build the product kernel only)
 extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<true, 320>(m, a); }
-#else
-#define myo_env_kernel_dbg myo_env_kernel
-#endif
 
 // ================================================================== host side (C-ABI)
 static thread_local std::string g_err;
@@ -441,7 +415,7 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
 }
 
 struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
-  int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool force_dbg; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots, load_wn, load_wi; bool perm_built; long long launches; unsigned long long seed; long long env_offset; };
+  int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 1; }
@@ -471,7 +445,6 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   d.npair = P[PD_NPAIR]; d.npair_an = P[PD_NPAIR_ANALYTIC]; d.maxpath = P[PD_MAXPATH]; d.ndepth = P[PD_NDEPTH]; d.eq_tree = P[PD_EQ_TREE];
   const double* opt = MYO_DSEC(I, D, MYO_SEC_opt); d.timestep = opt[0]; d.gx = opt[1]; d.gy = opt[2]; d.gz = opt[3]; d.tolerance = opt[4]; d.meaninertia = opt[6];
   d.ovr_geom = (cfg && cfg->task == MYO_TASK_HOLD) ? cfg->task_i[1] : -1;
-  { const char* e = getenv("MYO_B200_SOLVE_SYNC"); d.solve_sync = e ? atoi(e) : 1; }   // CTA barriers inside the Newton loop (0 = warps run the solver phase unaligned)
   int mc = cfg && cfg->maxcon > 0 ? cfg->maxcon : 32; if (mc > 64) mc = 64; if (mc > 2*d.npair) mc = 2*d.npair; /* (the contact-order merge handles up to 64) */ d.maxcon = mc; d.nlimrow = P[PD_NLIMROW] > 0 ? P[PD_NLIMROW] : 2*d.nlim; d.maxefc = d.neq + d.nlimrow + 4*mc;
   int o = 0;
   #define TAKE(field, n) d.field = o; o += al2(n)
@@ -538,7 +511,7 @@ extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const
   if (e != cudaSuccess || ndev == 0) return fail("myo_batch_create: no CUDA device available (this library has no CPU fallback)");
   if (device < 0 || device >= ndev) return fail("myo_batch_create: bad device index");
   CUDA_OK(cudaSetDevice(device));
-  myo_batch* b = new myo_batch(); memset(&b->bufs, 0, sizeof(b->bufs)); b->model = m; b->device = device; b->n_env = n_env; b->cfg = *cfg; b->bound = false; b->force_dbg = getenv("MYO_B200_DEBUG_KERNEL") && atoi(getenv("MYO_B200_DEBUG_KERNEL")); b->launches = 0; b->seed = 0; b->env_offset = 0;
+  myo_batch* b = new myo_batch(); memset(&b->bufs, 0, sizeof(b->bufs)); b->model = m; b->device = device; b->n_env = n_env; b->cfg = *cfg; b->bound = false; b->launches = 0; b->seed = 0; b->env_offset = 0;
   fill_devmodel(m, cfg, b->dm);
   if (b->cfg.frame_skip <= 0) b->cfg.frame_skip = 1;
   if (cfg->task == MYO_TASK_POSE && b->dm.nq != b->dm.nv) { delete b; return fail("pose task needs nq == nv"); }
@@ -586,8 +559,7 @@ extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const
   { int c = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_env_kernel_dbg, wd*32, b->dbg_smem); if (c < 1) c = 1; int need = (n_env + wd - 1)/wd, cap = sms*c; b->dbg_grid = need < cap ? need : cap; }
   // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
   b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
-  b->dLoad = nullptr; b->dPerm = nullptr; b->perm_rounds = 0; b->perm_slots = 0; b->perm_built = false; b->load_wn = 2; b->load_wi = 3;
-  if (const char* e = getenv("MYO_B200_LOADKEY")) sscanf(e, "%d,%d", &b->load_wn, &b->load_wi);      // tuning: weights of contacts and Newton iterations in the load key
+  b->dLoad = nullptr; b->dPerm = nullptr; b->perm_rounds = 0; b->perm_slots = 0; b->perm_built = false;
   if (b->regroup) { const int per_cta = (n_env + b->grid - 1)/b->grid; b->perm_rounds = (per_cta + wpc - 1)/wpc; b->perm_slots = b->grid*wpc*b->perm_rounds;
     CUDA_OK(cudaMalloc(&b->dLoad, (size_t)n_env*4)); CUDA_OK(cudaMemset(b->dLoad, 0, (size_t)n_env*4)); CUDA_OK(cudaMalloc(&b->dPerm, (size_t)b->perm_slots*4)); }
   if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
@@ -660,13 +632,13 @@ static int launch(myo_batch* b, StepArgs& a, void* stream) {
   a.tol = b->cfg.solver_tolerance > 0 ? b->cfg.solver_tolerance : 1e-10;
   // the debug instantiation serves forward-debug calls, bound parity taps / cycle counters and the barrier / lockstep tuning knobs
   const myo_buffers& q = b->bufs;
-  const bool dbg = a.mode == 1 || b->force_dbg || b->cfg.barrier_mode != 0 || b->cfg.reserved_i > 1 || q.tap_qacc || q.tap_actuator_force || q.tap_ten_length || q.tap_qfrc_smooth ||
+  const bool dbg = a.mode == 1 || b->cfg.barrier_mode != 0 || b->cfg.reserved_i > 1 || q.tap_qacc || q.tap_actuator_force || q.tap_ten_length || q.tap_qfrc_smooth ||
                    q.tap_ncon || q.tap_contact_pair || q.tap_contact_dist || q.tap_moment || q.tap_qM || q.tap_phase_cycles;
   if (dbg) { a.balanced = b->dbg_smem > 100*1024; myo_env_kernel_dbg<<<b->dbg_grid, b->dbg_warps*32, b->dbg_smem, (cudaStream_t)stream>>>(b->dm, a); }
   else { a.balanced = b->smem_bytes > 100*1024;
     if (a.mode == 0 && b->regroup) {      // env steps: regroup by last step's load first (same stream), then step through the permutation
       myo_regroup_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->dLoad, b->dPerm, b->n_env, b->grid, b->warps_per_cta, b->perm_slots);
-      a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = b->load_wn; a.load_wi = b->load_wi; b->perm_built = true; b->launches++; }
+      a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; b->perm_built = true; b->launches++; }
     if (b->use_w14) myo_env_kernel_w14<<<b->grid, b->warps_per_cta*32, b->smem_bytes, (cudaStream_t)stream>>>(b->dm, a);
     else myo_env_kernel<<<b->grid, b->warps_per_cta*32, b->smem_bytes, (cudaStream_t)stream>>>(b->dm, a); }
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;

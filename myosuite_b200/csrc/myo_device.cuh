@@ -43,7 +43,7 @@ struct DevModel {
   int32_t nq, nv, nu, na, nM, njnt;
   int32_t nbd, nlevel, nsp, nwe, nta, nnz, nlim, neq, npair, npair_an, maxpath, ndepth, eq_tree;
   int32_t tg_sp[3], tg_we[3], tg_ta[3], tg_nz[3];          // tendon groups A / B (two passes through the tendon scratch): ranges of segments, wrap elements, tendons, moment non-zeros
-  int32_t maxcon, maxefc, nlimrow, ovr_geom, ngc, s_gpose, solve_sync, nvp;          // ovr_geom: collision geom whose size comes from the per-env overrides (-1: none); nvp: nv padded to the dense solver's order
+  int32_t maxcon, maxefc, nlimrow, ovr_geom, ngc, s_gpose, nvp;          // ovr_geom: collision geom whose size comes from the per-env overrides (-1: none); nvp: nv padded to the dense solver's order
   double timestep, gx, gy, gz, meaninertia, tolerance;
   // per-warp shared-memory layout, in doubles.  Persistent part:
   int32_t o_qpos, o_qvel, o_act, o_qws, o_dax, o_dan, o_qM, o_fsm, o_eprm, neprm, o_wz, nwz, o_cnt, o_scr, n_per_warp;
@@ -66,11 +66,7 @@ struct Warp { int base, lane; };   // by value: offset (doubles) of this warp's 
 enum { CNT_ncon, CNT_nefc, CNT_nlimrow, CNT_niter, CNT_overflow, CNT_ncand, CNT_na, CNT_N = 8 };   // per-warp int counters (m.o_cnt)
 #define CI(name) ((const idx_t*)(smem + m.nD) + m.hoff[MYO_SEC_##name])
 #define CD(name) ((const double*)smem + m.hoff[MYO_SEC_##name])
-#ifdef MYO_COLD_L2ONLY
-#define LDC(p) __ldcg(p)                                      // (experiment: bypass L1 for the cold tables; the default keeps them in L1)
-#else
 #define LDC(p) __ldg(p)
-#endif
 #define GD(name) (m.gD + m.hoff[MYO_SEC_##name])              // cold f64 tables (blob.py COLD_D): read from HBM / L2 through the read-only path (__ldg)
 #define W_(f) (smem + w.base + m.o_##f)                       // persistent per-env arrays
 #define WI_(f) (((int*)(smem + w.base + m.o_cnt))[CNT_##f])   // per-env counters

@@ -102,17 +102,6 @@ __device__ void rows_applyT_add(const DevModel& m, const Warp w, double* wgt, do
   for (int pass = 0; pass < 2; pass++) {
     for (int r = w.lane; r < nlimrow; r += 32) { int dsc = S_lrow[r]; int neg = (dsc >> 8) & 1; if (neg == pass) vec[dsc & 0xff] += (neg ? -1.0 : 1.0)*wgt[m.neq + r]; }
     __syncwarp(); }
-#ifdef MYO_OLD_GRAD
-  { const idx_t* pr = CI(PPAIR); const double* pd = CD(PPAIR_d); const idx_t* path = CI(PPATH);
-  for (int c = 0; c < ncon; c++) { const int rn = S_crown[c], nr = CNR(rn); if (!nr) continue;
-    const idx_t* q = pr + PPAIR_ISTRIDE*S_cpair[c]; const JacRef J = S_jac(c); int rb = CROW(rn); double wn, w1 = 0, w2 = 0;
-    if (nr == 1) wn = wgt[rb];
-    else { wn = wgt[rb]+wgt[rb+1]+wgt[rb+2]+wgt[rb+3]; w1 = wgt[rb]-wgt[rb+1]; w2 = wgt[rb+2]-wgt[rb+3]; }
-    for (int e = w.lane; e < q[4]; e += 32) vec[path[q[3]+e] >> 1] += J[3*e]*wn + J[3*e+1]*w1 + J[3*e+2]*w2;
-    __syncwarp(); } }
-}
-#else
-
   for (int c = w.lane; c < ncon; c += 32) { const int rn = S_crown[c], nr = CNR(rn), rb = CROW(rn);      // fold the pyramid edges: (wn, w1, w2) into wgt[rb .. rb+2]
     if (nr == 4) { const double a0 = wgt[rb], a1 = wgt[rb+1], a2 = wgt[rb+2], a3 = wgt[rb+3];
       wgt[rb] = a0+a1+a2+a3; wgt[rb+1] = a0-a1; wgt[rb+2] = a2-a3; } }
@@ -124,7 +113,6 @@ __device__ void rows_applyT_add(const DevModel& m, const Warp w, double* wgt, do
     vec[d] += acc; }
   __syncwarp();
 }
-#endif
 
 // ------------------------------------------------------------------ constraint assembly
 __device__ void phase_constraints(const DevModel& m, const Warp w) {
@@ -163,13 +151,9 @@ __device__ void phase_constraints(const DevModel& m, const Warp w) {
   for (int s = 0; s < 2; s++) { const int c = w.lane + 32*s;
     if (c < ncon) { const idx_t* q = pr + PPAIR_ISTRIDE*S_cpair[c]; const double* P = pd + q[6]*PPAIR_STRIDE;
       nrs[s] = (S_con[c*CON_STRIDE] < P[0]-P[1]) ? (q[2] == 1 ? 1 : 4) : 0;
-#ifdef MYO_NO_RANK
-      rank[s] = c;
-#else
       const int k = key[c]; int cnt = 0;
       if (c < na) { for (int q2 = na; q2 < ncon; q2++) cnt += key[q2] < k; rank[s] = c + cnt; }
       else { for (int q2 = 0; q2 < na; q2++) cnt += key[q2] < k; rank[s] = (c - na) + cnt; }
-#endif
       S_crown[rank[s]] = nrs[s]; } }
   __syncwarp();
   #pragma unroll
@@ -257,9 +241,7 @@ __device__ __noinline__ void chol_rs(double* H, double* x, int n, int lane) {
     #pragma unroll
     for (int j = k+1; j < NMAX; j++) col[j] = H[TRI(j,k)];
     const double dk = H[TRI(k,k)], zk = x[k];
-#ifndef MYO_CHOL_NOBATCH
     asm volatile("" ::: "memory");
-#endif
     const double invd = m_rcp(fmax(dk, MYO_MINVAL));
     if (lane == k) invd_own = invd;
     const double t = r[k]*invd;                      // L[lane][k] on lanes > k
@@ -279,8 +261,8 @@ __device__ __noinline__ void chol_rs(double* H, double* x, int n, int lane) {
 // exactly like chol_rs<32> (row per lane in registers, columns published in shared memory, batched broadcast loads); the e = n - 32 border
 // rows ride along DISTRIBUTED over the lanes (lane j keeps B[q][j]): at step k lane k publishes its now final entries, every lane j > k
 // applies the same rank-1 update to its border entries with its own U[j][k].  The e x e Schur complement C - L21 D L21' and the border
-// right-hand side are warp sums; the small system is solved redundantly by every lane.  Replaces the shuffle-based chol_reg32b below
-// (two 32-double register arrays, 800 spill instructions).
+// right-hand side are warp sums; the small system is solved redundantly by every lane.  Chosen over a shuffle-based bordered Cholesky,
+// which needed two 32-double register arrays (800 spill instructions).
 template <int E>
 __device__ __noinline__ void chol_rs32b(double* H, double* x, int n, int lane) {
   SHARED_PTR(H); SHARED_PTR(x);
@@ -357,128 +339,16 @@ __device__ __noinline__ void chol_rs32b(double* H, double* x, int n, int lane) {
   __syncwarp();
 }
 
-// Bordered register Cholesky for 32 < n <= 32+E: H = [A B'; B C] with A the leading 32x32 block.  A = L11 L11' is factored in
-// registers exactly like chol_reg<32>; the rows of B ride along as extra right-hand sides of the forward substitution
-// (L21 = B L11^-T), the E x E Schur complement C - L21 L21' is reduced with warp sums and factored redundantly by every lane.
-template <int E>
-__device__ __noinline__ void chol_reg32b(const double* H, int n, double* x, int lane) {
-  SHARED_PTR(H); SHARED_PTR(x);
-  const int e = n - 32;
-  double r[32], c[32], bq[E];
-  #pragma unroll
-  for (int j = 0; j < 32; j++) { r[j] = j <= lane ? H[TRI(lane, j)] : 0.0; c[j] = 0.0; }
-  #pragma unroll
-  for (int q = 0; q < E; q++) bq[q] = q < e ? H[TRI(32+q, lane)] : 0.0;
-  double b = x[lane], dinv = 1.0;
-  #pragma unroll
-  for (int k = 0; k < 32; k++) {
-    double inv = rsqrt(fmax(__shfl_sync(FULL, r[k], k), MYO_MINVAL));
-    if (lane == k) dinv = inv;
-    r[k] *= inv;
-    #pragma unroll
-    for (int j = k+1; j < 32; j++) { double ljk = __shfl_sync(FULL, r[k], j); if (lane == k) c[j] = ljk; r[j] = fma(-r[k], ljk, r[j]); } }
-  #pragma unroll
-  for (int k = 0; k < 32; k++) { double yk = __shfl_sync(FULL, b*dinv, k); b = lane == k ? yk : (lane > k ? fma(-r[k], yk, b) : b);
-    #pragma unroll
-    for (int q = 0; q < E; q++) { double yq = __shfl_sync(FULL, bq[q]*dinv, k); bq[q] = lane == k ? yq : (lane > k ? fma(-r[k], yq, bq[q]) : bq[q]); } }
-  // b = y1[lane], bq[q] = L21[q][lane]; Schur complement (identity-padded beyond e) and its right-hand side
-  double S[E][E], y2[E];
-  #pragma unroll
-  for (int q = 0; q < E; q++) {
-    #pragma unroll
-    for (int p = 0; p <= q; p++) { double v = warp_sum(bq[q]*bq[p]); S[q][p] = ((q < e && p < e) ? H[TRI(32+q, 32+p)] : (q == p ? 1.0 : 0.0)) - v; }
-    y2[q] = (q < e ? x[32+q] : 0.0) - warp_sum(bq[q]*b); }
-  #pragma unroll
-  for (int k = 0; k < E; k++) { S[k][k] = sqrt(fmax(S[k][k], MYO_MINVAL)); double ik = 1.0/S[k][k];
-    #pragma unroll
-    for (int i = k+1; i < E; i++) S[i][k] *= ik;
-    #pragma unroll
-    for (int i = k+1; i < E; i++) {
-      #pragma unroll
-      for (int j = k+1; j <= i; j++) S[i][j] -= S[i][k]*S[j][k]; } }
-  #pragma unroll
-  for (int k = 0; k < E; k++) { y2[k] /= S[k][k];
-    #pragma unroll
-    for (int i = k+1; i < E; i++) y2[i] -= S[i][k]*y2[k]; }
-  #pragma unroll
-  for (int k = E-1; k >= 0; k--) { y2[k] /= S[k][k];
-    #pragma unroll
-    for (int i = 0; i < k; i++) y2[i] -= S[k][i]*y2[k]; }
-  // x1 = L11^-T (y1 - L21' x2)
-  #pragma unroll
-  for (int q = 0; q < E; q++) b = fma(-bq[q], y2[q], b);
-  #pragma unroll
-  for (int k = 31; k >= 0; k--) { double xk = __shfl_sync(FULL, b*dinv, k); b = lane == k ? xk : fma(-c[k], xk, b); }
-  __syncwarp();
-  x[lane] = b;
-  #pragma unroll
-  for (int q = 0; q < E; q++) if (lane == q && q < e) x[32+q] = y2[q];
-  __syncwarp();
-}
-
-// The same L D L' with a ROLLED elimination loop: after column k is eliminated every lane shifts its row registers left by one (the shift is
-// folded into the destination of the update FMA), so the pivot column is r[0] at EVERY step and the loop body has static register
-// indices.  Why it matters: the unrolled variant above is ~2 500 straight-line instructions (40 KB) that every call streams from L2 at the
-// rate the SM's instruction fetch sustains for uncached code (tools/ubench/ubench_icache.cu), so a solve inside the step kernel
-// is slower than one whose code is warm (tools/ubench/ubench_chol.cu).  The rolled body (~100 instructions) stays in the
-// instruction cache; it pays with FMAs on columns that are already finished (NMAX - 1 per step instead of n - 1 - k).
-// It was measured slower than the unrolled variant, in isolation and inside the step kernel: the clamped address chain and the dead-column
-// FMAs cost more than the instruction fetch they save.  Kept as an experiment behind MYO_CHOL_ROLLED; the unrolled variant is the product path.
-// H: packed lower triangle, n rows (no padding needed: reads past the last row are clamped onto it and only feed dead slots); destroyed.
-template <int NMAX>
-__device__ __noinline__ void chol_rot(double* H, double* x, int n, int lane) {
-  SHARED_PTR(H); SHARED_PTR(x);
-  const bool own = lane < n; const int rowadr = own ? TRI(lane, 0) : 0;
-  double r[NMAX];
-  #pragma unroll
-  for (int j = 0; j < NMAX; j++) r[j] = (own && j <= lane) ? H[rowadr + j] : 0.0;
-  double b = own ? x[lane] : 0.0, invd_own = 1.0;
-  __syncwarp();
-  #pragma unroll 1
-  for (int k = 0; k < n; k++) {
-    if (own && lane >= k) H[rowadr + k] = r[0];      // column k, unscaled (U[i][k] = L[i][k] d_k); lane k: the pivot d_k
-    if (lane == k) x[k] = b;                         // z_k of the forward substitution is final
-    __syncwarp();
-    double col[NMAX-1];
-    { int row = k + 1 < n ? k + 1 : n - 1, adr = TRI(row, k);      // H[row][k], row = k+1 .. (clamped to n-1)
-      #pragma unroll
-      for (int j = 0; j < NMAX-1; j++) { col[j] = H[adr]; const bool more = row + 1 < n; adr += more ? row + 1 : 0; row += more ? 1 : 0; } }
-    const double dk = H[TRI(k,k)], zk = x[k];
-    asm volatile("" ::: "memory");
-    const double invd = m_rcp(fmax(dk, MYO_MINVAL));
-    if (lane == k) invd_own = invd;
-    const double t = r[0]*invd;                      // L[lane][k] on lanes > k
-    b = lane > k ? fma(-t, zk, b) : b;
-    #pragma unroll
-    for (int j = 0; j < NMAX-1; j++) r[j] = fma(-t, col[j], r[j+1]);      // eliminate AND shift: column k+1 becomes r[0]
-    r[NMAX-1] = 0.0;
-  }
-  // backward substitution: u_i = z_i - sum_{k>i} U[k][i] x_k ; x_i = u_i / d_i
-  #pragma unroll 1
-  for (int k = n-1; k >= 0; k--) { const double xk = __shfl_sync(FULL, b*invd_own, k), hk = (own && lane < k) ? H[TRI(k,0) + lane] : 0.0; b = fma(-hk, xk, b); }
-  __syncwarp();
-  if (own) x[lane] = b*invd_own;
-  __syncwarp();
-}
-
-// padded order of the dense solver for an n x n system (kept for the layout of H and of the solver vectors; the rolled solver needs no padding)
+// padded order of the dense solver for an n x n system (the order of the chol_rs instance that solves it; H and the solver vectors are laid out for it)
 __host__ __device__ __forceinline__ int chol_pad(int n) { return n > 32 ? n : (n <= 8 ? 8 : (n == 23 || n == 29 ? n : (n + 3) & ~3)); }
 // x <- H^-1 x for a dense SPD H (packed lower triangle in shared memory); H is destroyed
 __device__ __forceinline__ void chol_dense(double* H, int n, double* x, int lane) {
   if (n > 36) { chol_factor_rows(H, n, lane); chol_solve(H, n, x, lane); return; }
-#ifdef MYO_CHOL_SHFL32B
-  if (n > 32) { chol_reg32b<4>(H, n, x, lane); return; }
-#else
   if (n > 32) { switch (n) { case 33: chol_rs32b<1>(H, x, n, lane); break; case 34: chol_rs32b<2>(H, x, n, lane); break; case 35: chol_rs32b<3>(H, x, n, lane); break; default: chol_rs32b<4>(H, x, n, lane); break; } return; }
-#endif
-#ifndef MYO_CHOL_ROLLED
   switch (chol_pad(n)) {
     case 8: chol_rs<8>(H, x, n, lane); break;   case 12: chol_rs<12>(H, x, n, lane); break; case 16: chol_rs<16>(H, x, n, lane); break;
     case 20: chol_rs<20>(H, x, n, lane); break; case 24: chol_rs<24>(H, x, n, lane); break; case 28: chol_rs<28>(H, x, n, lane); break;
     case 23: chol_rs<23>(H, x, n, lane); break; case 29: chol_rs<29>(H, x, n, lane); break; default: chol_rs<32>(H, x, n, lane); break; }
-#else
-  if (n <= 16) chol_rot<16>(H, x, n, lane); else if (n <= 24) chol_rot<24>(H, x, n, lane); else chol_rot<32>(H, x, n, lane);
-#endif
 }
 
 // H <- M (+ diag_scale * damping on the diagonal), dense packed lower triangle padded with identity rows up to chol_pad(nv)
@@ -582,37 +452,8 @@ __device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, dou
       if (d2 >= 0) { S_H[d1 > d2 ? TRI(d1,d2) : TRI(d2,d1)] += De*j2; S_H[TRI(d2,d2)] += De*j2*j2; } }
     __syncwarp();
     for (int pass = 0; pass < 2; pass++) { for (int r = w.lane; r < nlimrow; r += 32) { int dsc = S_lrow[r]; if (((dsc >> 8) & 1) == pass && S_jar[m.neq+r] < 0) { int d = dsc & 0xff; S_H[TRI(d,d)] += S_D[m.neq+r]; } } __syncwarp(); }
-    // contacts: J' W J.  (The gather form that pays for the gradient does not pay here: with one H entry per lane nearly every contact
-    // hits SOME lane and the warp runs the hit path 9 x ncon times.)  Two contacts at a time, one per half-warp, 16 lanes over the lower
-    // triangle of the contact's block: a finger-finger block has 36 entries -- two passes of 32 lanes with 4 busy in the second, now
-    // three passes of 16 for TWO contacts.  The two halves may touch the same H entry, so their read-modify-writes take turns
-    // (half 0 first: a fixed order).  It did not beat the one-contact loop below: the two ordered updates and the wider
-    // predication eat the saved pass.  Kept as an experiment behind -DMYO_H_PAIRED.
-#ifdef MYO_H_PAIRED
-    for (int c0 = 0; c0 < ncon; c0 += 2) { const int half = w.lane >> 4, hl = w.lane & 15, c = c0 + half;
-      bool ok = c < ncon; int nr = 0, rb = 0; double W[6] = {0,0,0,0,0,0};  // nn n1 n2 11 12 22
-      if (ok) { const int rn = S_crown[c]; nr = CNR(rn); rb = CROW(rn); ok = nr != 0; }
-      const idx_t* q = pr + (ok ? PPAIR_ISTRIDE*S_cpair[c] : 0);
-      if (ok) {
-        if (nr == 1) { if (S_jar[rb] < 0) W[0] = S_D[S_DCON(c)]; }
-        else { const double Dv = S_D[S_DCON(c)];
-          double a0 = S_jar[rb] < 0 ? Dv : 0, a1 = S_jar[rb+1] < 0 ? Dv : 0, a2 = S_jar[rb+2] < 0 ? Dv : 0, a3 = S_jar[rb+3] < 0 ? Dv : 0;
-          W[0] = a0+a1+a2+a3; W[1] = a0-a1; W[2] = a2-a3; W[3] = a0+a1; W[5] = a2+a3; }
-        ok = W[0] != 0; }
-      const int np = ok ? q[4] : 0, ntri = (np*(np+1)) >> 1; const int other = __shfl_xor_sync(FULL, ntri, 16), nmax = ntri > other ? ntri : other;
-      const JacRef J = S_jac(ok ? c : 0);
-      for (int t = hl; t - hl < nmax; t += 16) {       // (warp-uniform trip count: the warp syncs below sit inside the loop)
-        const bool v = t < ntri; double val = 0; int idx = 0;
-        if (v) { int ei, ej;
-          if (np <= 8) { ei = (t >= 1) + (t >= 3) + (t >= 6) + (t >= 10) + (t >= 15) + (t >= 21) + (t >= 28); ej = t - ((ei*(ei+1)) >> 1); } else tri_index(t, ei, ej);
-          const JacRef ja = J + 3*ei, jb = J + 3*ej; const double a[3] = {ja[0], ja[1], ja[2]}, b[3] = {jb[0], jb[1], jb[2]};
-          double wa0 = W[0]*a[0]+W[1]*a[1]+W[2]*a[2], wa1 = W[1]*a[0]+W[3]*a[1], wa2 = W[2]*a[0]+W[5]*a[2];
-          int di = path[q[3]+ei] >> 1, dj = path[q[3]+ej] >> 1; idx = TRI(di,dj); val = wa0*b[0]+wa1*b[1]+wa2*b[2]; }
-        if (v && half == 0) S_H[idx] += val;
-        __syncwarp();
-        if (v && half == 1) S_H[idx] += val;
-        __syncwarp(); } }
-#else
+    // contacts: J' W J, one contact at a time, the lanes over the lower triangle of its block.  (The gather form that pays for the
+    // gradient does not pay here: with one H entry per lane nearly every contact hits SOME lane and the warp runs the hit path 9 x ncon times.)
     for (int c = 0; c < ncon; c++) { const int rn = S_crown[c], nr = CNR(rn), rb = CROW(rn); if (!nr) continue; const idx_t* q = pr + PPAIR_ISTRIDE*S_cpair[c]; double W[6] = {0,0,0,0,0,0};  // nn n1 n2 11 12 22
       if (nr == 1) { if (S_jar[rb] < 0) W[0] = S_D[S_DCON(c)]; }
       else { const double Dv = S_D[S_DCON(c)];
@@ -625,7 +466,6 @@ __device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, dou
           double wa0 = W[0]*a[0]+W[1]*a[1]+W[2]*a[2], wa1 = W[1]*a[0]+W[3]*a[1], wa2 = W[2]*a[0]+W[5]*a[2];
           int di = path[q[3]+ei] >> 1, dj = path[q[3]+ej] >> 1; S_H[TRI(di,dj)] += wa0*b[0]+wa1*b[1]+wa2*b[2]; } }
       __syncwarp(); }
-#endif
     LAP(9)
     } }
     if (cta_sync) __syncthreads();

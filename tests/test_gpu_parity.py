@@ -347,7 +347,7 @@ def test_reach_task_golden_reset_and_time_switch():
 
 def test_dense_solver_all_sizes():
     """The dense SPD solver of the Newton / integrator phases against numpy for every n it dispatches on: register Cholesky (n <= 32,
-    four unrolled sizes), bordered register Cholesky (33..36), shared-memory rows fallback (> 36) and the shared-memory variant (mode 0)."""
+    four unrolled sizes), bordered register Cholesky (33..36) and shared-memory rows fallback (> 36)."""
     from myosuite_b200 import abi
     rng = np.random.default_rng(5)
     for n in list(range(1, 41)) + [48]:
@@ -357,9 +357,8 @@ def test_dense_solver_all_sizes():
         il = np.tril_indices(n)
         Hp = np.stack([H[k][il] for k in range(count)])
         ref = np.stack([np.linalg.solve(H[k], b[k]) for k in range(count)])
-        for mode in (1, 0):
-            x = abi.debug_chol_solve(Hp, b, mode=mode)
-            np.testing.assert_allclose(x, ref, rtol=1e-9, atol=1e-11 * np.abs(ref).max(), err_msg="n=%d mode=%d" % (n, mode))
+        x = abi.debug_chol_solve(Hp, b)
+        np.testing.assert_allclose(x, ref, rtol=1e-9, atol=1e-11 * np.abs(ref).max(), err_msg="n=%d" % n)
 
 
 # ----------------------------------------------------------------------------- mid-episode states, the hold model, regime and overflow rates

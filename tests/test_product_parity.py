@@ -44,7 +44,7 @@ CASES = {
     "elbow": ("myoElbowPose1D6MRandom-v0", 4096, {}, {}, dict(use_w14=1, warps_per_cta=14, rounds=3, regroup=0, balanced=0)),
     "torso": ("myoTorsoPoseFixed-v0", 661, {}, {}, dict(use_w14=0, warps_per_cta=3, rounds=2, regroup=1)),   # smallest n with 2 rounds
 }
-LAUNCH_ENV = ("MYO_B200_REGROUP", "MYO_B200_W14", "MYO_B200_WARPS_PER_CTA", "MYO_B200_DEBUG_KERNEL", "MYO_B200_LOADKEY")
+LAUNCH_ENV = ("MYO_B200_REGROUP", "MYO_B200_W14", "MYO_B200_WARPS_PER_CTA")
 REPORT = []
 
 
