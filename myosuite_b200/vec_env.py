@@ -12,7 +12,7 @@ import os
 
 import numpy as np
 
-from . import abi, assets, blob, program
+from . import abi, assets, blob, program, tasks
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _REG = None
@@ -45,32 +45,7 @@ def registered_ids():
 
 
 _MODEL_OF_XML = {v[0]: k for k, v in assets.MODEL_XML.items()}
-
-
-def stand_target_centre(m, tips, init_qpos):
-    """[ntip, 3] world positions the leg stand task samples its targets around.  The reference samples them around the tip sites of
-    a first generate_qpos() draw (walk_v0.py:142-174), then starts the episode from an independent second draw.  That centre is a
-    constant only when no draw moves a tip site: every joint between a tip's body and the world has a range of zero width (the draw
-    clips the one coordinate it touches to that range; the other coordinates of a free or ball joint keep init_qpos).  On the legs
-    the pelvis hangs from the free root, whose range [0, 0] pins x.  Any other structure raises instead of sampling a different
-    distribution."""
-    from . import mjcf
-    q = np.array(init_qpos, dtype=np.float64)
-    for j in range(m.njnt):                         # the first draw, on the coordinates it pins
-        if m.jnt_range[j][0] == m.jnt_range[j][1]:
-            q[m.jnt_qposadr[j]] = m.jnt_range[j][0]
-    kin, centre = mjcf.kinematics(m, q), []
-    for name in tips:
-        sid = m.name2id("site", name)
-        b = int(m.site_bodyid[sid])
-        while b != 0:
-            for j in range(int(m.body_jntadr[b]), int(m.body_jntadr[b]) + int(m.body_jntnum[b])):
-                if m.jnt_range[j][0] != m.jnt_range[j][1]:
-                    raise NotImplementedError("stand task: joint %d moves tip site %r under the randomised reset, so its target centre is not constant" % (j, name))
-            b = int(m.body_parentid[b])
-        b = int(m.site_bodyid[sid])
-        centre.append(kin["xpos"][b] + np.reshape(kin["xmat"][b], (3, 3)) @ m.site_pos[sid])
-    return np.array(centre)
+stand_target_centre = tasks.stand_target_centre          # (importable from here as before)
 
 
 class MyoVecEnv:
@@ -95,94 +70,28 @@ class MyoVecEnv:
         kw.update(overrides)
         self.kwargs = kw
         self._check_kwargs(kw)
-        self.torso = entry is not None and entry.endswith("torso_v0:TorsoEnvV0")        # TorsoEnvV0 = the pose task with a fixed mean-of-range target, far_th = pi, pose_thd 0.25
-        # "stand": walk_v0.py's ReachEnvV0 (myoLegStandRandom), the device's reach task with its own reward shape and randomised joint reset
-        self.task = ("none" if entry is None else "pose" if (entry.endswith("pose_v0:PoseEnvV0") or self.torso) else "walk" if entry.endswith("walk_v0:WalkEnvV0")
-                     else "hold" if "obj_hold_v0:ObjHold" in entry else "reach" if entry.endswith("reach_v0:ReachEnvV0")
-                     else "stand" if entry.endswith("walk_v0:ReachEnvV0") else None)
-        if self.task is None:
-            raise NotImplementedError("device task for %s (%s) is not built yet (pose, torso, walk, hold, reach, stand are; MyoVecEnv.from_model gives physics only)" % (env_id, entry))
-        if kw.get("joint_random_range") is not None and self.task != "stand":
-            raise NotImplementedError("joint_random_range is implemented for the leg stand task (walk_v0.py ReachEnvV0) only")
-        self.hold_random = entry is not None and entry.endswith("ObjHoldRandomEnvV0")
         self.mj_model = m = model if model is not None else assets.load(_MODEL_OF_XML[kw["model_path"]])
         self.muscle_condition = kw.get("muscle_condition", "")
         if self.muscle_condition == "sarcopenia":       # base_v0.py:62-67: gainprm[:,2] *= 0.5 (biasprm untouched)
             import copy
             self.mj_model = m = copy.deepcopy(m)
             m.actuator_gainprm[:, 2] *= 0.5
-        self.frame_skip = int(kw.get("frame_skip", 10))
-        self.dt = m.opt_timestep * self.frame_skip
-        self.n_frames = int(self.dt / m.opt_timestep)      # robot.py:901
         prog, self.prog_info = program.build_program(m)
         self.prog = prog
         self.I, self.D = blob.pack(m, prog)
+        # everything task-specific is computed on the host by tasks.configure; what follows allocates and binds it
+        c = tasks.configure(entry, m, self.prog_info, kw, self.max_episode_steps, auto_reset)
+        self.task, self.torso, self.hold_random, self.cfg = c.task, c.torso, c.hold_random, c.cfg
+        self.frame_skip, self.dt, self.n_frames = c.frame_skip, c.dt, c.n_frames
+        self.init_qpos, self.init_qvel, self.tip_names, self.target_center = c.init_qpos, c.init_qvel, c.tip_names, c.target_center
+        self.fatigue_reset_vec, self.reward_cfg = c.fatigue_reset_vec, c.reward_cfg
         # row_storage: "p48" (product: contact Jacobian rows held as the upper 48 bits of the f64 value -- 36 mantissa bits -- in shared memory,
         # 14 env-warps per SM on the hand) or "f64" (verification build of the same source, abi.lib("f64rows"): plain doubles, fewer warps)
         self.row_storage = kw.get("row_storage", "p48")
         if self.row_storage not in ("p48", "f64"):
             raise ValueError("row_storage must be 'p48' or 'f64'")
         self.dev_model = abi.DeviceModel(self.I, self.D, variant="f64rows" if self.row_storage == "f64" else None)
-        cfg = abi.MyoTaskCfg()
-        cfg.task = {"none": abi.TASK_NONE, "pose": abi.TASK_POSE, "walk": abi.TASK_WALK, "hold": abi.TASK_HOLD, "reach": abi.TASK_REACH, "stand": abi.TASK_REACH}[self.task]
-        cfg.frame_skip = self.n_frames
-        cfg.max_episode_steps = int(self.max_episode_steps or 0)
-        cfg.normalize_act = int(bool(kw.get("normalize_act", True)))
-        cfg.muscle_condition = abi.COND_FATIGUE if self.muscle_condition == "fatigue" else abi.COND_NONE
-        # fatigue state at reset (base_v0.py:120-128 -> fatigue.py:82-99)
-        self.fatigue_reset_vec = None if kw.get("fatigue_reset_vec") is None else np.asarray(kw["fatigue_reset_vec"], dtype=np.float64).ravel()
-        if self.fatigue_reset_vec is not None and len(self.fatigue_reset_vec) != m.na:
-            raise AssertionError("Invalid length of initial/reset fatigue vector (expected %d, but obtained %d)" % (m.na, len(self.fatigue_reset_vec)))      # fatigue.py:91
-        cfg.fatigue_reset = 1 if kw.get("fatigue_reset_random") else (2 if self.fatigue_reset_vec is not None else 0)
-        cfg.auto_reset = int(bool(auto_reset))
-        cfg.reset_random = int(kw.get("reset_type", "init") == "random")
-        cfg.pose_thd = float(kw.get("pose_thd", 0.25 if self.torso else 0.35))         # pose_v0.py:43 / torso_v0.py:52
-        if self.torso:
-            cfg.task_d[0] = float(np.pi)                                                # far_th (torso_v0.py:104)
-        init_qpos, init_qvel = np.asarray(m.qpos0, dtype=np.float64).copy(), np.zeros(m.nv)
-        if self.task in ("pose", "none"):
-            w = kw.get("weighted_reward_keys", {"pose": 1.0, "bonus": 4.0, "act_reg": 1.0, "penalty": 50})     # pose_v0.py:18-23
-            for i, k in enumerate(("pose", "bonus", "act_reg", "penalty")):
-                cfg.weights[i] = w[k]
-        elif self.task == "walk":
-            w = kw.get("weighted_reward_keys", {"vel_reward": 5.0, "done": -100, "cyclic_hip": -10, "ref_rot": 10.0, "joint_angle_rew": 5.0})   # walk_v0.py:205-211
-            for i, k in enumerate(("vel_reward", "done", "cyclic_hip", "ref_rot", "joint_angle_rew")):
-                cfg.weights[i] = w[k]
-            self._setup_walk(m, kw, cfg, prog_info=None)
-            rt = kw.get("reset_type", "init")                                                      # walk_v0.py:344-352
-            if rt == "random":       # keyframe 2 or 3 + N(0, 0.02) noise, drawn in the kernel (walk_v0.py:321-337): two rows
-                init_qpos, init_qvel = np.stack([m.key_qpos[2], m.key_qpos[3]]), np.stack([m.key_qvel[2], m.key_qvel[3]])
-            else:
-                key = 2 if rt == "init" else 0
-                init_qpos, init_qvel = m.key_qpos[key].copy(), m.key_qvel[key].copy()
-        elif self.task == "hold":
-            w = kw.get("weighted_reward_keys", {"goal_dist": 100.0, "bonus": 4.0, "penalty": 10})     # obj_hold_v0.py:17-21
-            for i, k in enumerate(("goal_dist", "bonus", "penalty")):
-                cfg.weights[i] = w[k]
-            init_qpos[:-7] = 0.0; init_qpos[0] = -1.5                                                  # obj_hold_v0.py:61-62
-            cfg.reset_random = int(self.hold_random)
-        elif self.task in ("reach", "stand"):
-            w = kw.get("weighted_reward_keys", {"reach": 1.0, "bonus": 4.0, "penalty": 50} if self.task == "reach"      # reach_v0.py:18-22
-                       else {"reach": 1.0, "bonus": 4.0, "penalty": 50, "act_reg": 1})                                     # walk_v0.py:18-24
-            for i, k in enumerate(("reach", "bonus", "act_reg", "penalty")):
-                cfg.weights[i] = w.get(k, 0.0)
-            if self.task == "stand":     # walk_v0.py:65-66: init_qpos / init_qvel = keyframe 0
-                init_qpos, init_qvel = m.key_qpos[0].copy(), m.key_qvel[0].copy()
-        cfg.solver_tolerance = float(kw.get("solver_tolerance", 0.0))
-        cfg.maxcon = int(kw.get("maxcon", 0))
-        cfg.barrier_mode = int(kw.get("barrier_mode", 0))
-        cfg.reserved_i = int(kw.get("lockstep_groups", 0))
-        cfg.reserved[0] = float(bool(kw.get("profile_waits", False)))
-        cfg.reaf_dst = cfg.reaf_src = -1
-        if self.muscle_condition == "reafferentation":   # base_v0.py:78-79,104-108
-            cfg.reaf_dst, cfg.reaf_src = m.name2id("actuator", "EPL"), m.name2id("actuator", "EIP")
-        if self.task == "hold":
-            self._setup_hold(m, cfg)
-        if self.task in ("reach", "stand"):
-            self._setup_reach(m, kw, cfg)
-        if self.task == "stand":
-            self._setup_stand(m, kw, cfg, init_qpos)
-        self.cfg = cfg
+        cfg = self.cfg
         self.device_index = int(device)
         self.device = torch.device("cuda", self.device_index)
         self.batch = abi.Batch(self.dev_model, self.device_index, self.num_envs, cfg)
@@ -193,48 +102,35 @@ class MyoVecEnv:
         self.full_obs_dim = self.obs_dim = max(self.batch.obs_dim, 1); self.act_dim = m.nu
         # custom obs_keys (env_base.py:110,190,458 obsdict2obsvec over `obs_keys`; base_v0.py:33-37 appends "act"): the kernel always writes the
         # task's full default layout into t["obs_full"]; t["obs"] is the gather of the requested keys' columns, refreshed after every launch
+        lay = c.layout
+        self.obs_keys = [k_ for k_, _ in lay]
         self._obs_cols = None
-        if kw.get("obs_keys") is not None and self.task != "none":
-            from . import gym_api
+        if kw.get("obs_keys") is not None and lay:
             keys = list(kw["obs_keys"])
             if m.na > 0 and "act" not in keys:
                 keys.append("act")
-            lay, off, o = gym_api.obs_layout(self.task, m.nq, m.nv, m.na, len(getattr(self, "tip_names", ()))), {}, 0
+            off, o = {}, 0
             for k_, w_ in lay:
                 off[k_] = (o, w_); o += w_
             missing = [k_ for k_ in keys if k_ not in off]
             if missing:
-                raise KeyError("obs_keys not available from this task's obs_dict: %s (available: %s)" % (missing, [k_ for k_, _ in lay]))
-            self.obs_keys = keys
-            if keys != [k_ for k_, _ in lay]:
+                raise KeyError("obs_keys not available from this task's obs_dict: %s (available: %s)" % (missing, self.obs_keys))
+            if keys != self.obs_keys:
                 cols = np.concatenate([np.arange(off[k_][0], off[k_][0] + off[k_][1]) for k_ in keys])
                 self._obs_cols, self._obs_cols_np = torch.as_tensor(cols, dtype=torch.int64, device=self.device), cols
                 self.obs_dim = int(len(cols))
+            self.obs_keys = keys
         t = dict(action=z(n, m.nu, dtype=f32), qpos=z(n, m.nq), qvel=z(n, m.nv), act=z(n, max(m.na, 1)), qacc_warmstart=z(n, m.nv),
                  time=z(n), target=z(n, m.nq), step_count=z(n, dtype=torch.int32), episode_count=z(n, dtype=torch.int64),
                  obs=z(n, self.full_obs_dim, dtype=f32), reward=z(n, dtype=f32), done=z(n, dtype=torch.uint8), truncated=z(n, dtype=torch.uint8),
                  ep_return=z(n, dtype=f32), last_return=z(n, dtype=f32), overflow=z(n, dtype=torch.int32))
         t["qpos"][:] = torch.as_tensor(m.qpos0, device=dv)
-        # target ranges per qpos (pose_v0.py:60-70); "fixed" targets collapse the range
-        tr = np.zeros((m.nq, 2))
-        if kw.get("target_jnt_range"):
-            for jn, (lo, hi) in kw["target_jnt_range"].items():
-                qa = m.jnt_qposadr[m.name2id("joint", jn)]
-                tr[qa] = (0.5 * (lo + hi),) * 2 if self.torso else (lo, hi)     # TorsoEnvV0 never resamples: target = mean of the range (torso_v0.py:66-68)
-        elif kw.get("target_jnt_value") is not None:
-            v = np.asarray(kw["target_jnt_value"], dtype=np.float64)
-            tr[:, 0] = tr[:, 1] = v
-        elif self.task in ("reach", "stand"):       # rows 3k..3k+2: span of target site k (reach_v0.py:163-170); `target` rows hold the sampled site positions
-            for k, span in enumerate(kw["target_reach_range"].values()):         # stand: around the constant tip position of the first draw (walk_v0.py:142-150)
-                c = self.target_center[k] if self.task == "stand" else 0.0
-                tr[3 * k:3 * k + 3, 0], tr[3 * k:3 * k + 3, 1] = c + np.asarray(span[0], dtype=np.float64), c + np.asarray(span[1], dtype=np.float64)
-        t["target_range"] = torch.as_tensor(tr, device=dv).contiguous()
-        t["init_qpos"] = torch.as_tensor(init_qpos, device=dv).contiguous()
-        t["init_qvel"] = torch.as_tensor(init_qvel, device=dv).contiguous()
-        self.init_qpos, self.init_qvel = init_qpos, init_qvel
-        if self.task == "hold":
+        t["target_range"] = torch.as_tensor(c.target_range, device=dv).contiguous()
+        t["init_qpos"] = torch.as_tensor(self.init_qpos, device=dv).contiguous()
+        t["init_qvel"] = torch.as_tensor(self.init_qvel, device=dv).contiguous()
+        if c.env_prm is not None:
             t["env_prm"] = z(n, 8)
-            t["env_prm"][:, :6] = torch.as_tensor(np.array([cfg.task_d[6 + i] for i in range(6)]), device=dv)
+            t["env_prm"][:, :6] = torch.as_tensor(c.env_prm, device=dv)
         if cfg.muscle_condition == abi.COND_FATIGUE:
             t["fatigue"] = z(n, 3, m.nu)
             t["fatigue"][:, 1, :] = 1.0
@@ -279,71 +175,6 @@ class MyoVecEnv:
             bad.append("weight_bodyname / weight_range")
         if bad:
             raise NotImplementedError("reference kwargs accepted by the reference but not by this backend: " + "; ".join(bad))
-
-    # ---------------------------------------------------------------- task parameter blocks (indices into the kernel's dynamic-body list)
-    def _dyn(self, body_name):
-        return self.prog_info["dyn_body_ids"].index(self.mj_model.name2id("body", body_name))
-
-    def _setup_walk(self, m, kw, cfg, prog_info=None):
-        """WalkEnvV0 constants (walk_v0.py:235-266,358-494, registry myobase/__init__.py:443-458)."""
-        from . import mjmath as mm
-        root, torso = m.name2id("body", "root"), m.name2id("body", "torso")
-        q, b = np.array([1.0, 0, 0, 0]), torso
-        while b != root:                                   # torso xquat = root quat (x) constant chain offset (no joints in between)
-            if m.body_jntnum[b] != 0:
-                raise NotImplementedError("torso must be rigidly attached to the free root body")
-            q = mm.quat_mul(m.body_quat[b], q); b = int(m.body_parentid[b])
-        ti = [self._dyn("root"), self._dyn("talus_l"), self._dyn("talus_r"), self._dyn("pelvis")]
-        ti += [int(m.jnt_qposadr[m.name2id("joint", j)]) for j in ("hip_flexion_l", "hip_flexion_r", "hip_adduction_l", "hip_adduction_r", "hip_rotation_l", "hip_rotation_r")]
-        for i, v in enumerate(ti):
-            cfg.task_i[i] = v
-        target_rot = kw.get("target_rot") if kw.get("target_rot") is not None else m.key_qpos[0][3:7]      # init_qpos = key_qpos[0] (walk_v0.py:258)
-        td = list(q) + [kw.get("min_height", 0.8), kw.get("max_rot", 0.8), kw.get("hip_period", 100), kw.get("target_x_vel", 0.0), kw.get("target_y_vel", 1.2)] + \
-            list(target_rot) + [float(np.sum(m.body_mass))]
-        for i, v in enumerate(td):
-            cfg.task_d[i] = float(v)
-
-    def _setup_reach(self, m, kw, cfg):
-        """ReachEnvV0 constants (reach_v0.py:52-67): tip sites (body + offset), world-fixed target sites, far_th."""
-        tips = list(kw["target_reach_range"].keys())
-        if 3 * len(tips) > m.nq or len(tips) > 7:
-            raise NotImplementedError("reach task: at most 7 tips and 3*ntip <= nq")
-        cfg.task_i[0] = len(tips)
-        dyn = self.prog_info["dyn_body_ids"]
-        for k, name in enumerate(tips):
-            sid, tid = m.name2id("site", name), m.name2id("site", name + "_target")
-            if int(m.site_bodyid[tid]) != 0:
-                raise NotImplementedError("reach targets must be world-fixed sites")
-            b = int(m.site_bodyid[sid])
-            cfg.task_i[1 + k] = dyn.index(b) if b in dyn else -1
-            for c in range(3):
-                cfg.task_d[3 * k + c] = float(m.site_pos[sid][c])
-        cfg.task_d[3 * len(tips)] = float(kw.get("far_th", 0.35))
-        self.tip_names = tips
-
-    STAND_SHAPE = (10.0, 10.0, 100.0, 0.05)      # walk_v0.py:104-140: reach = 10 - d - 10 |qvel dt|, act_reg = -100 |act|/na, near_th = 0.05 ntip
-
-    def _setup_stand(self, m, kw, cfg, init_qpos):
-        """walk_v0.py ReachEnvV0 (walk_v0.py:49-79,104-186): reward shape, randomised joint reset, target centre (stand_target_centre)."""
-        lo, hi = (float(x) for x in kw.get("joint_random_range", (0.0, 0.0)))
-        if not hi > lo:
-            raise NotImplementedError("stand task without joint randomisation: the reference then samples the target around the previous episode's last state")
-        for i, v in enumerate(self.STAND_SHAPE):
-            cfg.reach_shape[i] = v
-        cfg.joint_random[0], cfg.joint_random[1] = lo, hi
-        self.target_center = stand_target_centre(m, self.tip_names, init_qpos)
-
-    def _setup_hold(self, m, cfg):
-        """ObjHold constants (obj_hold_v0.py:46-62,126-145)."""
-        from . import mjcf
-        obj_body, sid, gid = m.name2id("body", "object"), m.name2id("site", "object"), m.name2id("geom", "object")
-        pg = {v: k for k, v in self.prog_info["geom_model_ids"].items()}[gid]
-        cfg.task_i[0], cfg.task_i[1] = self._dyn("object"), pg
-        kin = mjcf.kinematics(m, m.qpos0)
-        obj_init = kin["xpos"][obj_body] + kin["xmat"][obj_body] @ m.site_pos[sid]                    # object_init_pos (obj_hold_v0.py:52)
-        goal = m.site_pos[m.name2id("site", "goal")]
-        for i in range(3):
-            cfg.task_d[i] = m.site_pos[sid][i]; cfg.task_d[3 + i] = obj_init[i]; cfg.task_d[6 + i] = goal[i]; cfg.task_d[9 + i] = m.geom_size[gid][i]
 
     # ---------------------------------------------------------------- gym-style API (batched)
     @property
@@ -435,10 +266,8 @@ class MyoVecEnv:
 
     def task_info(self):
         """`rwd_sparse` / `solved` of the current observations (the reference's info dict, env_base.py:585-616), derived lazily from obs."""
-        from . import task_info
         m = self.mj_model
-        return task_info.info_from_obs(self.task, self.t["obs_full"], m.nq, m.nv, m.na, pose_thd=float(self.cfg.pose_thd),
-                                       ntip=len(getattr(self, "tip_names", ())) or None)
+        return tasks.info_from_obs(self.task, self.t["obs_full"], m.nq, m.nv, m.na, pose_thd=float(self.cfg.pose_thd), ntip=len(self.tip_names) or None)
 
     def refresh_obs(self):
         """obs / reward / done of the current state (the reference's env.forward(), env_base.py:393-432)."""
@@ -495,27 +324,14 @@ class MyoEnv:
         self.input_seed = seed
         m = v.mj_model
         self.action_space, self.observation_space = gym_api.make_spaces(m.nu, v.obs_dim, bool(v.kwargs.get("normalize_act", True)), m.actuator_ctrlrange)
-        self._ntip = len(getattr(v, "tip_names", ()))
-        self.obs_keys = list(getattr(v, "obs_keys", None) or [k for k, _ in gym_api.obs_layout(v.task, m.nq, m.nv, m.na, self._ntip)])
-        self.rwd_keys_wt = dict(v.kwargs.get("weighted_reward_keys") or gym_api.DEFAULT_WEIGHTS[v.task])
+        self._ntip = len(v.tip_names)
+        self.obs_keys = list(v.obs_keys)
+        self.rwd_keys_wt = dict(v.kwargs.get("weighted_reward_keys") or tasks.DEFAULT_WEIGHTS[v.task])
+        self._task_cfg = v.reward_cfg                     # host reward constants (tasks.configure)
         self.rwd_mode = "dense"
         self.obs_dict, self.rwd_dict, self.proprio_dict, self.visual_dict = {}, {}, {}, {}
         self._reseed = True
-        self._task_cfg = self._make_task_cfg()
         self.reset()
-
-    # ---- task constants for the host-side reward dict
-    def _make_task_cfg(self):
-        v, m, kw = self.vec, self.vec.mj_model, self.vec.kwargs
-        cfg = {"pose_thd": float(v.cfg.pose_thd), "dt": v.dt, "ntip": self._ntip, "far_th": float(kw.get("far_th", 0.35))}
-        if v.torso:
-            cfg["pose_far_th"] = float(np.pi)
-        if v.task == "walk":
-            cfg.update(target_x_vel=kw.get("target_x_vel", 0.0), target_y_vel=kw.get("target_y_vel", 1.2), min_height=kw.get("min_height", 0.8), max_rot=kw.get("max_rot", 0.8),
-                       target_rot=np.asarray(kw.get("target_rot") if kw.get("target_rot") is not None else m.key_qpos[0][3:7], dtype=np.float64))
-            for j in ("hip_flexion_l", "hip_flexion_r", "hip_adduction_l", "hip_adduction_r", "hip_rotation_l", "hip_rotation_r"):
-                cfg["q_" + j] = int(m.jnt_qposadr[m.name2id("joint", j)])
-        return cfg
 
     # ---- seeding (env_base.py:119-123)
     def seed(self, seed=None):
@@ -564,13 +380,11 @@ class MyoEnv:
     def get_obs_dict(self, *sim_args):
         """obs_dict of the current observation.  (The reference signature takes (mj_model, mj_data); the state lives on the device here, so
         any arguments are ignored.)"""
-        from . import gym_api
         m = self.mj_model
-        return gym_api.obs_dict_from_vec(self.vec.task, self._last["obs_full"], np.array([self._last["time"]]), m.nq, m.nv, m.na, self._ntip)
+        return tasks.obs_dict_from_vec(self.vec.task, self._last["obs_full"], np.array([self._last["time"]]), m.nq, m.nv, m.na, self._ntip)
 
     def get_reward_dict(self, obs_dict):
-        from . import gym_api
-        r = gym_api.reward_dict(self.vec.task, obs_dict, self.rwd_keys_wt, self._task_cfg)
+        r = tasks.reward_dict(self.vec.task, obs_dict, self.rwd_keys_wt, self._task_cfg)
         if float(np.squeeze(obs_dict["time"])) == self._last["time"]:
             r["dense"] = np.float64(self._last["reward"])        # the device's f64 reward (the host recomputation only sees the f32 observation)
         return r
@@ -588,9 +402,8 @@ class MyoEnv:
         return self.forward()[0]
 
     def _key_widths(self):
-        from . import gym_api
         m = self.mj_model
-        w = dict(gym_api.obs_layout(self.vec.task, m.nq, m.nv, m.na, self._ntip))
+        w = dict(tasks.obs_layout(self.vec.task, m.nq, m.nv, m.na, self._ntip))
         return [(k, w[k]) for k in self.obs_keys]
 
     def obsvec2obsdict(self, obsvec):
@@ -678,7 +491,7 @@ def register_gym():
     for eid in registered_ids():
         try:
             steps, _, entry = env_spec(eid)
-            if not any(entry.endswith(x) for x in ("pose_v0:PoseEnvV0", "walk_v0:WalkEnvV0", "reach_v0:ReachEnvV0", "torso_v0:TorsoEnvV0", "walk_v0:ReachEnvV0")) and "obj_hold_v0:ObjHold" not in entry:
+            if tasks.task_of(entry) is None:
                 continue
             g.register(id=eid, entry_point="myosuite_b200.vec_env:MyoEnv", max_episode_steps=steps, kwargs={"env_id": eid})
             done.append(eid)

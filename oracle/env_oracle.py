@@ -121,9 +121,13 @@ def hold_obs_reward(m, o, dt, goal_pos):
     return obs, dict(goal_dist=-d, done=drop, dense=dense)
 
 
-def reach_obs_reward(m, o, dt, tips, targets, time, far_th=0.35, weights=None):
-    """reach_v0.py:98-160: obs = [qpos, qvel*dt, tip_pos, target - tip_pos, act] (f32); reach / bonus / penalty terms.
-    tips: site names; targets: [ntip, 3] world positions of the target sites; time: mjData.time of the observed state."""
+def reach_obs_reward(m, o, dt, tips, targets, time, far_th=0.35, shape=(0.0, 0.0, 0.0, 0.0), weights=None):
+    """reach_v0.py:98-160: obs = [qpos, qvel*dt, tip_pos, target - tip_pos, act] (f32) and every reward term.
+    tips: site names; targets: [ntip, 3] world positions of the target sites; time: mjData.time of the observed state.
+    shape: the kernel's cfg.reach_shape (c_off, c_vel, c_act, near per tip): reach = c_off - d - c_vel |qvel dt|, act_reg = -c_act |act|/na,
+    bonus thresholds near ntip and 2 near ntip.  All zeros means the reach_v0 rule (0, 0, 1, 0.0125); the leg stand task
+    (walk_v0.py:104-140 ReachEnvV0) is (10, 10, 100, 0.05).  The velocity norm is taken only when c_vel is non-zero, as in the kernel."""
+    c_off, c_vel, c_act, near1 = shape if any(shape) else (0.0, 0.0, 1.0, 0.0125)
     weights = weights or {"reach": 1.0, "bonus": 4.0, "penalty": 50}
     qpos, qvel, act = o.f("qpos"), o.f("qvel"), o.f("act")
     sx = o.f("site_xpos").reshape(-1, 3)
@@ -131,9 +135,11 @@ def reach_obs_reward(m, o, dt, tips, targets, time, far_th=0.35, weights=None):
     err = np.asarray(targets, dtype=np.float64).ravel() - tip
     obs = np.concatenate([qpos, qvel * dt, tip, err, act]).astype(np.float32)
     d = np.linalg.norm(err)
+    v = np.linalg.norm(qvel * dt) if c_vel else 0.0
     act_mag = np.linalg.norm(act) / m.na if m.na else 0.0
     far = far_th * len(tips) if time > 2 * dt else np.inf
-    near = len(tips) * 0.0125
-    terms = dict(reach=-d, bonus=1.0 * (d < 2 * near) + 1.0 * (d < near), act_reg=-act_mag, penalty=-1.0 * (d > far))
-    dense = sum(wt * terms[k] for k, wt in weights.items())
-    return obs, dict(reach=-d, done=bool(d > far), solved=bool(d < near), dense=dense)
+    near = len(tips) * near1
+    r = dict(reach=c_off - d - c_vel * v, bonus=1.0 * (d < 2 * near) + 1.0 * (d < near), act_reg=-c_act * act_mag, penalty=-1.0 * (d > far),
+             sparse=-d, solved=bool(d < near), done=bool(d > far))
+    r["dense"] = sum(wt * r[k] for k, wt in weights.items())
+    return obs, r

@@ -1,10 +1,9 @@
 """Host reference of the simulator's random resets: Philox4x32-10 in numpy, the per-(seed, env, episode, lane) stream key of
 `philox_init`, the 53-bit uniform of `philox_uniform`, and the order in which each lane of `env_reset` consumes its stream
 (myosuite_b200/csrc/myo_b200.cu).  Test infrastructure: tests/test_rng_resets.py pins the generator to the Random123 known-answer
-vectors and the device resets to `replay_reset`."""
+vectors and the device resets to `replay_reset`; `replay_env` / `compare_reset` hold a batch's reset state to the replay (there and
+in the in-kernel auto-resets of tests/test_product_parity.py)."""
 import numpy as np
-
-from stand_oracle import stand_reset_qpos
 
 M32 = 0xFFFFFFFF
 PHILOX_M0, PHILOX_M1 = 0xD2511F53, 0xCD9E8D57          # round multipliers
@@ -61,6 +60,17 @@ def uniforms(seed, env, episode, lane, count, rounds=10):
         o = philox4x32(c, key, rounds)
         out += [uniform53(o[..., 0], o[..., 1]), uniform53(o[..., 2], o[..., 3])]
     return np.stack(out[:count], axis=-1)
+
+
+def stand_reset_qpos(m, init_qpos, u, joint_random_range=(-0.2, 0.2)):
+    """ReachEnvV0.generate_qpos (walk_v0.py:152-167) on given uniforms u ~ U[0, 1), one per joint in joint order: the first qpos
+    coordinate of every joint += U(lo, hi) (numpy's low + (high - low) u), clipped to jnt_range whether or not the joint is limited."""
+    lo, hi = joint_random_range
+    adr = m.jnt_qposadr
+    q = np.array(init_qpos, dtype=np.float64, copy=True)
+    q[adr] += lo + (hi - lo) * np.asarray(u, dtype=np.float64)
+    q[adr] = np.clip(q[adr], m.jnt_range[:, 0], m.jnt_range[:, 1])
+    return q
 
 
 class _LaneDraws:
@@ -141,3 +151,60 @@ def replay_reset(m, task, seed, env, episode, init_qpos, init_qvel=None, target_
             f[:, 0, i], f[:, 1, i], f[:, 2, i] = nf * ap, nf * (1 - ap), 1 - nf
         out["fatigue"] = f
     return out
+
+
+# ------------------------------------------------------------------------------------------------ a batch's resets against the replay
+EPS = np.finfo(np.float64).eps
+
+
+def replay_env(env, seed, episode, envs=None):
+    """replay_reset of the MyoVecEnv batch `env`'s envs `envs` (local indices, all by default) at episode counts `episode`."""
+    from myosuite_b200 import abi
+    cfg = env.cfg
+    envs = np.arange(env.num_envs) if envs is None else np.asarray(envs)
+    return replay_reset(env.mj_model, env.task, seed, env.env_offset + envs, episode, env.init_qpos, env.init_qvel,
+                        target_range=env.t["target_range"].cpu().numpy(), reset_random=bool(cfg.reset_random),
+                        joint_random=(cfg.joint_random[0], cfg.joint_random[1]), ntip=len(env.tip_names),
+                        hold_d=list(cfg.task_d)[:12], fatigue_random=cfg.muscle_condition == abi.COND_FATIGUE and cfg.fatigue_reset == 1)
+
+
+def _within(got, want, tol, label):
+    excess = np.abs(got - want) - tol
+    assert np.all(excess <= 0), "%s: %d entries off, worst by %.3g beyond %.3g at %s" % (
+        label, int(np.sum(excess > 0)), excess.max(), np.broadcast_to(tol, excess.shape).flat[np.argmax(excess)], np.unravel_index(np.argmax(excess), excess.shape))
+
+
+def _span_tol(lo, hi):
+    """lo + u (hi - lo), with or without an FMA: within 4 eps max(|lo|, |hi|) of numpy's rounding."""
+    return 4 * EPS * np.maximum(np.abs(lo), np.abs(hi))
+
+
+def compare_reset(env, S, R, label, rows=slice(None)):
+    """Device state S of the envs `rows` against replay R (already restricted to those envs): bit for bit where the kernel's expression
+    admits no contraction (fatigue state, stand joint offsets, walk keyframe row, untouched init_qpos), else to a few ulps."""
+    m, cfg, task = env.mj_model, env.cfg, env.task
+    tr = env.t["target_range"].cpu().numpy()
+    if "fatigue" in R:
+        np.testing.assert_array_equal(S["fatigue"][rows], R["fatigue"], err_msg=label + ": fatigue state")
+    if "key" in R:                                            # walk's random reset
+        qv = S["qvel"][rows]
+        key = np.where(np.all(qv == env.init_qvel[1], axis=1), 1, np.where(np.all(qv == env.init_qvel[0], axis=1), 0, -1))
+        np.testing.assert_array_equal(key, R["key"], err_msg=label + ": walk keyframe row")
+        _within(S["qpos"][rows], R["qpos"], 1e-15, label + ": walk qpos")
+    elif task == "pose" and cfg.reset_random:
+        free = m.jnt_type == 0
+        adr = m.jnt_qposadr[~free]
+        _within(S["qpos"][rows][:, adr], R["qpos"][:, adr], _span_tol(m.jnt_range[~free, 0], m.jnt_range[~free, 1]), label + ": pose qpos")
+    else:                                                     # stand offsets (numpy's rounding, no contraction) or untouched init_qpos
+        np.testing.assert_array_equal(S["qpos"][rows], R["qpos"], err_msg=label + ": qpos")
+    if "target" in R:
+        cols = m.jnt_qposadr[m.jnt_type != 0] if task == "pose" else np.arange(3 * int(cfg.task_i[0]))
+        _within(S["target"][rows][:, cols], R["target"][:, cols], _span_tol(tr[cols, 0], tr[cols, 1]), label + ": target")
+    if "env_prm" in R:
+        got = S["env_prm"][rows][:, :6]
+        if cfg.reset_random:
+            obj = np.array(cfg.task_d[3:6])
+            lo, hi = np.concatenate([obj - 0.03, [0.02] * 3]), np.concatenate([obj + 0.03, [0.03] * 3])
+            _within(got, R["env_prm"], _span_tol(lo, hi), label + ": hold goal / size")
+        else:
+            np.testing.assert_array_equal(got, R["env_prm"], err_msg=label + ": hold fixed goal / size")

@@ -1,24 +1,25 @@
 """The leg stand task, myoLegStandRandom-v0 and its Sarc / Fati variants (the ReachEnvV0 of walk_v0.py on the legs model).
 
-CPU: registry, the host obs_dict / rwd_dict, the CPU reference of the task (tests/stand_oracle.py) and the host-computed target centre
-against tests/golden/stand.npz, which the reference's own methods produced (tests/golden/make_golden_stand.py).
-GPU: the kernel's obs / reward / done on the golden states, the distribution of the randomised reset, the product step kernel against the
-oracle at the benchmark shape (first steps after a reset and in-kernel auto-resets included) and the gym contract."""
+CPU: registry, the host obs_dict / rwd_dict / info, the oracle's reach rule with the stand shape (env_oracle.reach_obs_reward), the reset
+rule (philox_ref.stand_reset_qpos) and the host-computed target centre against tests/golden/stand.npz, which the reference's own methods
+produced (tests/golden/make_golden_stand.py).
+GPU: the kernel's obs / reward / done on the golden states, the distribution of the randomised reset and the gym contract.  The product
+step kernel is checked against the oracle at the benchmark shape in tests/test_product_parity.py (cases stand, stand_fatigue)."""
 import copy
 import os
 import pickle
-import time
 
 import numpy as np
 import pytest
 
-from myosuite_b200 import gym_api, vec_env
-from stand_oracle import STAND_WEIGHTS, stand_obs_reward, stand_reset_qpos
+from myosuite_b200 import gym_api, tasks, vec_env
+from philox_ref import stand_reset_qpos
 
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 STAND = "myoLegStandRandom-v0"
 IDS = (STAND, "myoSarcLegStandRandom-v0", "myoFatiLegStandRandom-v0")
 NQ, NV, NA, DT = 35, 34, 80, 0.01
+STAND_WEIGHTS = {"reach": 1.0, "bonus": 4.0, "penalty": 50, "act_reg": 1}        # walk_v0.py:18-24
 
 
 @pytest.fixture(scope="module")
@@ -64,7 +65,7 @@ def _f64_obs_dict(models, Z):
     return dict({k: np.array(x) for k, x in d.items()}, time=Z["obs_time"])
 
 
-def test_host_dicts_vs_reference_golden(models, Z):
+def test_host_dicts_and_info_vs_reference_golden(models, Z):
     # the obs_dict is a view of the observation vector
     od = gym_api.obs_dict_from_vec("stand", Z["obs"], Z["obs_time"], NQ, NV, NA, ntip=1)
     assert list(od) == ["time", "qpos", "qvel", "tip_pos", "reach_err", "act"]
@@ -86,16 +87,17 @@ def test_host_dicts_vs_reference_golden(models, Z):
     for th in (0.05, 0.1):
         assert np.any(d < th) and np.any(d > th)
     assert np.any(armed & (d > 0.44)) and np.any(armed & (d < 0.44)) and np.any(~armed & (d > 0.44)) and np.any(~armed)
-    from myosuite_b200 import task_info
-    inf = task_info.info_from_obs("stand", Z["obs"], NQ, NV, NA, ntip=1)
+    inf = tasks.info_from_obs("stand", Z["obs"], NQ, NV, NA, ntip=1)
     assert np.array_equal(inf["solved"], Z["obs_solved"].astype(bool))
 
 
 def test_oracle_stand_obs_reward_vs_reference_golden(models, Z):
+    """The oracle's reach rule with the kernel's stand shape (cfg.reach_shape) against the reference's own stand reward."""
+    from oracle import env_oracle
     m = models["myolegs"]; o = _oracle(m)
     for i, (q, v, a, tg, tm) in enumerate(zip(Z["obs_qpos"], Z["obs_qvel"], Z["obs_act"], Z["obs_targets"], Z["obs_time"])):
         _observe(o, m, q, v, a)
-        obs, r = stand_obs_reward(m, o, DT, ["pelvis"], tg[None], tm, far_th=0.44)
+        obs, r = env_oracle.reach_obs_reward(m, o, DT, ["pelvis"], tg[None], tm, far_th=0.44, shape=tasks.STAND_SHAPE, weights=STAND_WEIGHTS)
         np.testing.assert_array_equal(obs, Z["obs"][i])
         for k in ("reach", "bonus", "act_reg", "penalty", "sparse", "dense"):
             assert r[k] == pytest.approx(Z["obs_" + k][i], rel=1e-12, abs=1e-12), (i, k)
@@ -232,162 +234,3 @@ def test_stand_gym_contract(env_id):
     if "Fati" in env_id:
         assert "fatigue" in env1.get_env_state()
 
-
-# ---- the product step kernel against the oracle at the benchmark shape
-STAND_CASES = {
-    "stand": (STAND, 2048, dict(use_w14=0, warps_per_cta=6, rounds=3, regroup=1)),
-    "stand_fatigue": ("myoFatiLegStandRandom-v0", 2048, dict(use_w14=0, warps_per_cta=6, rounds=3, regroup=1)),
-}
-N_FIRST = 48              # envs reset just before the checked step: it is their first step, from a state whose joint couplings are broken
-REPORT = []
-
-
-@pytest.fixture(scope="module")
-def report():
-    yield
-    if REPORT:
-        print("\nleg stand, product kernel vs oracle:")
-        for line in REPORT:
-            print("  " + line)
-
-
-def _stand_task_obs(env, o, tnow, target):
-    """obs, dense reward, done of the oracle's current state, and the distance of d to the nearest threshold it is compared with."""
-    m, far_th = env.mj_model, float(env.kwargs["far_th"])
-    o.set(ctrl=np.zeros(m.nu)); o.forward()
-    obs, r = stand_obs_reward(m, o, env.dt, env.tip_names, target[:3].reshape(1, 3), tnow, far_th=far_th)
-    d = -r["sparse"]
-    ths = [0.05, 0.1] + ([far_th] if tnow > 2 * env.dt else [])
-    return obs, r["dense"], r["done"], min(abs(d - t) for t in ths)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("case", list(STAND_CASES))
-def test_stand_product_step_vs_oracle(case, monkeypatch, report):
-    """test_product_parity.py's replay on the stand task: launch shape, slot map on every step, a quarter of the envs forced to the
-    TimeLimit (in-kernel auto-resets), plus envs reset right before the checked step, so that the step from a freshly randomised state
-    (couplings violated) is held to the mid-episode bounds too."""
-    import torch
-    from oracle import env_oracle
-    from parity_helpers import _in_regime, relerr
-    from test_product_parity import (ACT_ATOL, FATIGUE_RTOL, LAUNCH_ENV, MAX_SKIP_REGIME, N_RESET, QACC_REL, QPOS_ATOL, QVEL_REL, SEED,
-                                     THRESHOLD_MARGIN, WARM, Oracles, check_map, load_state, perm_or_none, select, slot_table)
-    eid, n, expect = STAND_CASES[case]
-    for k in LAUNCH_ENV:
-        monkeypatch.delenv(k, raising=False)
-    t0 = time.time()
-    env = vec_env.MyoVecEnv(eid, n, seed=SEED)
-    m = env.mj_model
-    info = env.batch.launch_info()
-    assert {k: info[k] for k in expect} == expect, info
-    env.reset(seed=SEED)
-    g = torch.Generator(device="cpu").manual_seed(SEED)
-    for _ in range(WARM):
-        env.step((torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device))
-        check_map(slot_table(info, n, perm_or_none(env, info)), n)
-    rng = np.random.default_rng(SEED)
-    trunc_set = rng.choice(n, n // 4, replace=False)
-    first_set = rng.choice(np.setdiff1d(np.arange(n), trunc_set), N_FIRST, replace=False)
-    mask = np.zeros(n, np.uint8); mask[first_set] = 1
-    env.reset(mask=torch.as_tensor(mask, device=env.device))
-    S0 = env.get_env_state()
-    sc = S0["step_count"].copy(); sc[trunc_set] = env.max_episode_steps - 1
-    env.set_env_state({"step_count": sc})
-    S = env.get_env_state()
-    assert np.all(S["step_count"][first_set] == 0) and np.all(S["time"][first_set] == 0) and np.all(S["qacc_warmstart"][first_set] == 0)
-    ov0 = env.t["overflow"].cpu().numpy().copy()
-    a = (torch.rand(n, m.nu, generator=g) * 2 - 1).numpy().astype(np.float32)
-    oracles = Oracles(env)
-
-    obs, rew, done, trunc, info_d = env.step(torch.as_tensor(a, device=env.device))
-    torch.cuda.synchronize()
-    obs, rew, done, trunc = (x.cpu().numpy().copy() for x in (obs, rew, done, trunc))
-    last_ret, ov = info_d["last_return"].cpu().numpy().copy(), env.t["overflow"].cpu().numpy().copy()
-    N = env.get_env_state()
-    T = slot_table(info, n, perm_or_none(env, info))
-    check_map(T, n)
-    assert np.all(trunc[trunc_set])
-    chosen = select(T, rng, [], rng.choice(trunc_set, N_RESET, replace=False))
-    for e in first_set:
-        chosen.setdefault(int(e), set()).add("first-step")
-    where = {int(e): (r, w, c) for (r, w, c), e in np.ndenumerate(T) if e >= 0}
-    worst = {k: 0.0 for k in ("qpos", "qvel", "qacc", "obs", "reward", "qpos_first", "qvel_first", "qacc_first")}
-    cnt = dict(checked=0, phys=0, first=0, reset=0, threshold=0, overflow=0, regime=0)
-    tr = env.t["target_range"].cpu().numpy()
-    k0 = m.key_qpos[0]
-
-    def check(e, why):
-        msg = "%s env %d (round, warp, cta) %s, checked as %s" % (case, e, where[e], sorted(why))
-        if ov0[e] or ov[e]:
-            cnt["overflow"] += 1
-            return
-        o = oracles.get(); load_state(o, env, S, e)
-        fat = None
-        if "fatigue" in S:
-            fat = env_oracle.Fatigue(m.nu, dt=env.dt, tauact=m.actuator_dynprm[:, 0], taudeact=m.actuator_dynprm[:, 1])
-            fat.MA, fat.MR, fat.MF = (S["fatigue"][e, k].copy() for k in range(3))
-        ctrl = env_oracle.action_to_ctrl(a[e].astype(np.float64), bool(env.cfg.normalize_act))
-        o.set(ctrl=fat.compute_act(ctrl)[0].copy() if fat is not None else ctrl)
-        in_regime = True
-        for _ in range(env.n_frames):
-            o.step(1); in_regime = in_regime and _in_regime(o, m)
-        if not in_regime:
-            cnt["regime"] += 1
-            return
-        tnow = float(S["time"][e])
-        for _ in range(env.n_frames):
-            tnow += m.opt_timestep
-        qpos, qvel, act, qacc = (o.f(k).copy() for k in ("qpos", "qvel", "act", "qacc"))
-        x_obs, x_rw, x_done, margin = _stand_task_obs(env, o, tnow, S["target"][e])
-        x_trunc = int(S["step_count"][e]) + 1 >= env.max_episode_steps
-        if margin > THRESHOLD_MARGIN:
-            worst["reward"] = max(worst["reward"], abs(float(rew[e]) - x_rw))
-            assert rew[e] == pytest.approx(x_rw, rel=1e-5, abs=1e-5), msg
-            assert bool(done[e]) == bool(x_done), msg
-        else:
-            cnt["threshold"] += 1
-        assert bool(trunc[e]) == x_trunc, msg
-        R = np.float32(S["ep_return"][e]) + rew[e]
-        if done[e] or trunc[e]:
-            assert last_ret[e] == R, msg
-            cnt["reset"] += 1
-            q = N["qpos"][e]
-            assert np.all(N["act"][e] == 0) and np.all(N["qacc_warmstart"][e] == 0) and N["time"][e] == 0 and np.all(N["qvel"][e] == 0), msg
-            assert N["step_count"][e] == 0 and N["episode_count"][e] == S["episode_count"][e] + 1 and N["ep_return"][e] == 0, msg
-            assert q[0] == 0 and np.all(q[1:7] == k0[1:7]), msg
-            adr = m.jnt_qposadr[1:]
-            assert np.all(q[adr] >= m.jnt_range[1:, 0]) and np.all(q[adr] <= m.jnt_range[1:, 1]) and np.all(np.abs(q[adr] - k0[adr]) <= 0.2 + 1e-12), msg
-            assert np.all(N["target"][e][:3] >= tr[:3, 0]) and np.all(N["target"][e][:3] <= tr[:3, 1]), msg
-            if "fatigue" in N:
-                assert np.all(N["fatigue"][e, 0] == 0) and np.all(N["fatigue"][e, 1] == 1) and np.all(N["fatigue"][e, 2] == 0), msg
-            o = oracles.get(); load_state(o, env, N, e)
-            np.testing.assert_allclose(obs[e], _stand_task_obs(env, o, 0.0, N["target"][e])[0], rtol=2e-6, atol=2e-6, err_msg=msg)
-        else:
-            first = "first-step" in why
-            cnt["phys"] += 1; cnt["first"] += first
-            sfx = "_first" if first else ""
-            worst["qpos" + sfx] = max(worst["qpos" + sfx], float(np.abs(N["qpos"][e] - qpos).max()))
-            worst["qvel" + sfx] = max(worst["qvel" + sfx], relerr(N["qvel"][e], qvel))
-            worst["qacc" + sfx] = max(worst["qacc" + sfx], relerr(N["qacc_warmstart"][e], qacc))
-            np.testing.assert_allclose(N["qpos"][e], qpos, rtol=0, atol=QPOS_ATOL, err_msg=msg)
-            assert relerr(N["qvel"][e], qvel) < QVEL_REL, msg
-            assert relerr(N["qacc_warmstart"][e], qacc) < QACC_REL, msg
-            np.testing.assert_allclose(N["act"][e, :m.na], act, rtol=0, atol=ACT_ATOL, err_msg=msg)
-            if fat is not None:
-                np.testing.assert_allclose(N["fatigue"][e], np.stack([fat.MA, fat.MR, fat.MF]), rtol=FATIGUE_RTOL, atol=1e-15, err_msg=msg)
-            assert N["time"][e] == tnow and N["step_count"][e] == S["step_count"][e] + 1 and N["ep_return"][e] == R, msg
-            worst["obs"] = max(worst["obs"], float(np.abs(obs[e] - x_obs).max()))
-            np.testing.assert_allclose(obs[e], x_obs, rtol=2e-6, atol=2e-6, err_msg=msg)
-        cnt["checked"] += 1
-
-    for e in sorted(chosen):
-        check(e, chosen[e])
-    REPORT.append("%-14s %-26s n %4d  %s  warps %d  grid %d  rounds %d  checked %d of %d (physics %d, of them first steps after a reset %d; "
-                  "auto-reset %d; skipped: deep penetration %d, contact overflow %d; near a threshold %d)  worst: qpos %.1e qvel %.1e qacc %.1e "
-                  "(first steps: qpos %.1e qvel %.1e qacc %.1e)  obs %.1e  reward %.1e  [%.1f s]"
-                  % (case, eid, n, "w14" if info["use_w14"] else "k320", info["warps_per_cta"], info["grid"], info["rounds"], cnt["checked"], len(chosen),
-                     cnt["phys"], cnt["first"], cnt["reset"], cnt["regime"], cnt["overflow"], cnt["threshold"], worst["qpos"], worst["qvel"], worst["qacc"],
-                     worst["qpos_first"], worst["qvel_first"], worst["qacc_first"], worst["obs"], worst["reward"], time.time() - t0))
-    print(REPORT[-1])
-    assert cnt["reset"] >= N_RESET and cnt["first"] >= N_FIRST // 2 and cnt["phys"] >= 32
-    assert cnt["regime"] <= MAX_SKIP_REGIME * len(chosen) and cnt["overflow"] <= 3

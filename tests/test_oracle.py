@@ -442,22 +442,3 @@ def test_statistical_drop_in_vs_reference_npg_logs():
     e = chk.run("myoElbowPose1D6MRandom-v0", 480, seed=1)
     assert abs(e["mean"] - 63.0) < 45 and abs(e["std"] - 190) < 25 and abs(e["success_pct"] - 54.5) < 15, e
 
-
-def test_task_info_from_obs_matches_reference_goldens():
-    """rwd_sparse / solved derived from the observation vector (myosuite_b200/task_info.py) vs the reference's own reward dicts."""
-    from myosuite_b200 import task_info
-    for tag, thd, nq, na in (("elbow", 0.175, 1, 6), ("hand", 0.7, 23, 39)):
-        obs = G["pose_%s_obs" % tag]
-        inf = task_info.info_from_obs("pose", obs, nq, nq, na, pose_thd=thd)
-        np.testing.assert_allclose(inf["rwd_sparse"], G["pose_%s_rwd_sparse" % tag], rtol=2e-6, atol=2e-6)
-        ok = np.abs(-inf["rwd_sparse"] - thd) > 1e-5                                     # (f32 obs: skip cases on the threshold)
-        np.testing.assert_array_equal(inf["solved"][ok], G["pose_%s_rwd_solved" % tag].astype(bool)[ok])
-    inf = task_info.info_from_obs("reach", T["reach_obs"], 23, 23, 39, ntip=5)
-    np.testing.assert_array_equal(inf["solved"], T["reach_solved"].astype(bool))
-    import torch
-    inf_t = task_info.info_from_obs("reach", torch.as_tensor(T["reach_obs"]), 23, 23, 39, ntip=5)
-    np.testing.assert_allclose(inf_t["rwd_sparse"].numpy(), inf["rwd_sparse"], rtol=1e-12)
-    d = np.linalg.norm(T["hold_obs"][:, 49:52].astype(np.float64), axis=1)
-    inf = task_info.info_from_obs("hold", T["hold_obs"], 30, 29, 39)
-    np.testing.assert_allclose(inf["rwd_sparse"], -d) and np.array_equal(inf["solved"], d < 0.010)
-    assert task_info.info_from_obs("walk", T["walk_obs"], 35, 34, 80) is None

@@ -8,12 +8,15 @@ a snapshot of the full env state (warm start, time, fatigue and per-env object s
 
 The envs are chosen from the slot -> env map the step ran with (the load-sorted permutation, or the fixed map of env_kernel_body) so
 that every (round, warp slot) pair is checked in at least two CTAs, together with the last slot, the neighbours of idle slots, the
-most contact-heavy envs of a pre-sample, envs that auto-reset on this step and a random sample."""
+most contact-heavy envs of a pre-sample, envs that auto-reset on this step and a random sample.  The leg stand cases also reset some
+envs right before the checked step: their step starts from the randomised reset state, whose joint couplings are broken, and is held to
+the mid-episode bounds too."""
 import time
 
 import numpy as np
 import pytest
 
+import philox_ref as P
 from parity_helpers import _in_regime, relerr
 
 pytestmark = pytest.mark.gpu
@@ -43,7 +46,10 @@ CASES = {
     "reach": ("myoHandReachRandom-v0", 4096, {}, {}, dict(use_w14=1, warps_per_cta=11, rounds=3, regroup=1)),
     "elbow": ("myoElbowPose1D6MRandom-v0", 4096, {}, {}, dict(use_w14=1, warps_per_cta=14, rounds=3, regroup=0, balanced=0)),
     "torso": ("myoTorsoPoseFixed-v0", 661, {}, {}, dict(use_w14=0, warps_per_cta=3, rounds=2, regroup=1)),   # smallest n with 2 rounds
+    "stand": ("myoLegStandRandom-v0", 2048, {}, {}, dict(use_w14=0, warps_per_cta=6, rounds=3, regroup=1)),
+    "stand_fatigue": ("myoFatiLegStandRandom-v0", 2048, {}, {}, dict(use_w14=0, warps_per_cta=6, rounds=3, regroup=1)),
 }
+N_FIRST = {"stand": 48, "stand_fatigue": 48}      # envs reset right before the checked step (0 for the other cases)
 LAUNCH_ENV = ("MYO_B200_REGROUP", "MYO_B200_W14", "MYO_B200_WARPS_PER_CTA")
 REPORT = []
 
@@ -129,10 +135,13 @@ def task_obs(env, o, steps, tnow, target, prm):
     if env.task == "hold":
         obs, r = env_oracle.hold_obs_reward(m, o, dt, prm[:3])
         return obs, r["dense"], r["done"], min(abs(-r["goal_dist"] - t) for t in (0.010, 0.020, 0.300))
-    ntip, far_th = len(env.tip_names), float(env.kwargs.get("far_th", 0.35))
-    obs, r = env_oracle.reach_obs_reward(m, o, dt, env.tip_names, target[:3 * ntip].reshape(ntip, 3), tnow, far_th=far_th)
-    ths = [ntip * 0.0125, 2 * ntip * 0.0125] + ([far_th * ntip] if tnow > 2 * dt else [])
-    return obs, r["dense"], r["done"], min(abs(-r["reach"] - t) for t in ths)
+    from test_leg_stand import STAND_WEIGHTS
+    ntip, far_th, shape = len(env.tip_names), float(env.kwargs.get("far_th", 0.35)), tuple(env.cfg.reach_shape)
+    obs, r = env_oracle.reach_obs_reward(m, o, dt, env.tip_names, target[:3 * ntip].reshape(ntip, 3), tnow, far_th=far_th, shape=shape,
+                                         weights=STAND_WEIGHTS if env.task == "stand" else None)
+    near = ntip * (shape[3] if any(shape) else 0.0125)
+    ths = [near, 2 * near] + ([far_th * ntip] if tnow > 2 * dt else [])
+    return obs, r["dense"], r["done"], min(abs(-r["sparse"] - t) for t in ths)
 
 
 def select(T, rng, contact_top, reset_envs):
@@ -176,6 +185,7 @@ def test_product_step_vs_oracle(case, monkeypatch):
     from myosuite_b200 import vec_env
     from oracle import env_oracle
     eid, n, lib_env, kw, expect = CASES[case]
+    n_first = N_FIRST.get(case, 0)
     for k in LAUNCH_ENV:
         monkeypatch.delenv(k, raising=False)
     for k, v in lib_env.items():
@@ -196,12 +206,18 @@ def test_product_step_vs_oracle(case, monkeypatch):
         env.step((torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device))
         check_map(slot_table(info, n, perm_or_none(env, info)), n)
     rng = np.random.default_rng(SEED)
-    S0 = env.get_env_state()
     trunc_set = rng.choice(n, n // 4, replace=False)
+    first_set = []
+    if n_first:          # their checked step is the first of an episode
+        first_set = rng.choice(np.setdiff1d(np.arange(n), trunc_set), n_first, replace=False)
+        mask = np.zeros(n, np.uint8); mask[first_set] = 1
+        env.reset(mask=torch.as_tensor(mask, device=env.device))
+    S0 = env.get_env_state()
     sc = S0["step_count"].copy(); sc[trunc_set] = env.max_episode_steps - 1
     env.set_env_state({"step_count": sc})
     S = env.get_env_state()
     assert np.array_equal(S["qacc_warmstart"], S0["qacc_warmstart"]) and np.array_equal(S["qpos"], S0["qpos"])
+    assert np.all(S["step_count"][first_set] == 0) and np.all(S["time"][first_set] == 0) and np.all(S["qacc_warmstart"][first_set] == 0)
     ov0 = env.t["overflow"].cpu().numpy().copy()
     a = (torch.rand(n, m.nu, generator=g) * 2 - 1).numpy().astype(np.float32)
 
@@ -224,10 +240,12 @@ def test_product_step_vs_oracle(case, monkeypatch):
     resets = np.nonzero(done | trunc)[0]
     assert np.all(trunc[trunc_set]) and len(resets) >= n // 4
     chosen = select(T, rng, contact_top, rng.choice(trunc_set, N_RESET, replace=False))
+    for e in first_set:
+        chosen.setdefault(int(e), set()).add("first-step")
 
     where = {int(e): (r, w, c) for (r, w, c), e in np.ndenumerate(T) if e >= 0}
-    worst = dict(qpos=0.0, qvel=0.0, qacc=0.0, obs=0.0, reward=0.0)
-    cnt = dict(checked=0, phys=0, reset=0, threshold=0, overflow=0, regime=0)
+    worst = dict(qpos=0.0, qvel=0.0, qacc=0.0, obs=0.0, reward=0.0, qpos_first=0.0, qvel_first=0.0, qacc_first=0.0)
+    cnt = dict(checked=0, phys=0, first=0, reset=0, threshold=0, overflow=0, regime=0)
     covered = {}
     rtol, atol = OBS_TOL.get(env.task, (2e-6, 2e-6)); rw_tol = RWD_TOL.get(env.task, 1e-5)
 
@@ -273,31 +291,25 @@ def test_product_step_vs_oracle(case, monkeypatch):
             # ---- the stored state is a fresh reset ...
             assert np.all(N["act"][e] == 0) and np.all(N["qacc_warmstart"][e] == 0) and N["time"][e] == 0, msg
             assert N["step_count"][e] == 0 and N["episode_count"][e] == S["episode_count"][e] + 1 and N["ep_return"][e] == 0, msg
-            if env.task == "pose" and env.cfg.reset_random:
-                jr = m.jnt_range[m.jnt_type != 0]; qa = m.jnt_qposadr[m.jnt_type != 0]
-                assert np.all(N["qpos"][e][qa] >= jr[:, 0]) and np.all(N["qpos"][e][qa] <= jr[:, 1]), msg
-            else:                                                   # (no case runs the walk task's random keyframe reset)
-                assert np.array_equal(N["qpos"][e], np.reshape(env.init_qpos, (-1, m.nq))[0]), msg
+            # (no case runs the walk task's random keyframe reset)
             assert np.array_equal(N["qvel"][e], np.reshape(env.init_qvel, (-1, m.nv))[0]), msg
-            tr = env.t["target_range"].cpu().numpy()
-            if env.task in ("pose", "reach"):
-                assert np.all(N["target"][e] >= tr[:, 0]) and np.all(N["target"][e] <= tr[:, 1]), msg
+            # qpos, target, per-env object: the draws of the stream of the episode count the env had before the step
+            P.compare_reset(env, N, P.replay_env(env, env.seed_value, S["episode_count"][[e]], [e]), msg, rows=[e])
             if "fatigue" in N:
                 assert env.cfg.fatigue_reset == 0
                 assert np.all(N["fatigue"][e, 0] == 0) and np.all(N["fatigue"][e, 1] == 1) and np.all(N["fatigue"][e, 2] == 0), msg
-            if env.task == "hold":
-                p = N["env_prm"][e]; obj0 = np.array([env.cfg.task_d[3 + i] for i in range(3)])
-                assert np.all(np.abs(p[:3] - obj0) <= 0.03 + 1e-12) and np.all(p[3:6] >= 0.02) and np.all(p[3:6] <= 0.03), msg
             # ... and its obs is the obs of that state
             o = oracles.get(N["env_prm"][e] if "env_prm" in N else None); load_state(o, env, N, e)
             r_obs = task_obs(env, o, 0, 0.0, N["target"][e], N["env_prm"][e] if "env_prm" in N else None)[0]
             np.testing.assert_allclose(obs[e], r_obs, rtol=rtol, atol=atol, err_msg=msg)
         else:
             # ---- physics and state of a step that did not end the episode: the mid-episode tolerances on every such env
-            cnt["phys"] += 1
-            worst["qpos"] = max(worst["qpos"], float(np.abs(N["qpos"][e] - qpos).max()))
-            worst["qvel"] = max(worst["qvel"], relerr(N["qvel"][e], qvel))
-            worst["qacc"] = max(worst["qacc"], relerr(N["qacc_warmstart"][e], qacc))
+            first = "first-step" in why                     # a step from a fresh reset state: the same bounds, its own worst case
+            cnt["phys"] += 1; cnt["first"] += first
+            sfx = "_first" if first else ""
+            worst["qpos" + sfx] = max(worst["qpos" + sfx], float(np.abs(N["qpos"][e] - qpos).max()))
+            worst["qvel" + sfx] = max(worst["qvel" + sfx], relerr(N["qvel"][e], qvel))
+            worst["qacc" + sfx] = max(worst["qacc" + sfx], relerr(N["qacc_warmstart"][e], qacc))
             np.testing.assert_allclose(N["qpos"][e], qpos, rtol=0, atol=QPOS_ATOL, err_msg=msg)
             assert relerr(N["qvel"][e], qvel) < QVEL_REL, msg
             assert relerr(N["qacc_warmstart"][e], qacc) < QACC_REL, msg           # the stored warm start is the last substep's qacc
@@ -329,16 +341,18 @@ def test_product_step_vs_oracle(case, monkeypatch):
                 chosen[int(T[r, w, c])] = {"cover-replacement"}; replaced += 1
                 check(int(T[r, w, c]), chosen[int(T[r, w, c])])
     full = sum(len(covered.get(k, ())) >= min(2, v) for k, v in live.items())
+    first_rep = ("  first steps after a reset %d: qpos %.1e  qvel %.1e  qacc %.1e" % (cnt["first"], worst["qpos_first"], worst["qvel_first"], worst["qacc_first"])
+                 if n_first else "")
     REPORT.append("%-12s %-26s n %4d  %s  warps %2d  grid %3d  rounds %d  %s  checked %3d of %3d (physics %3d, auto-reset %2d; skipped: deep penetration %d, "
                   "contact overflow %d; reward/done near a threshold %d)  (round, slot) pairs checked in 2 CTAs %d/%d (%d replacements)  "
-                  "worst: qpos %.1e  qvel %.1e  qacc %.1e  obs %.1e  reward %.1e  [%.1f s]"
+                  "worst: qpos %.1e  qvel %.1e  qacc %.1e  obs %.1e  reward %.1e%s  [%.1f s]"
                   % (case, eid, n, "w14" if info["use_w14"] else "k320", nw, info["grid"], R, "regroup" if info["regroup"] else ("balanced" if info["balanced"] else "contiguous"),
                      cnt["checked"], len(chosen), cnt["phys"], cnt["reset"], cnt["regime"], cnt["overflow"], cnt["threshold"], full, len(live), replaced,
-                     worst["qpos"], worst["qvel"], worst["qacc"], worst["obs"], worst["reward"], time.time() - t0))
+                     worst["qpos"], worst["qvel"], worst["qacc"], worst["obs"], worst["reward"], first_rep, time.time() - t0))
     print(REPORT[-1])
     assert cnt["reset"] >= N_RESET
     assert full == len(live), "(round, slot) pairs not checked in two CTAs"
-    assert cnt["phys"] >= 32
+    assert cnt["phys"] >= 32 and cnt["first"] >= n_first // 2
     # envs outside the parity claim stay rare: deep ellipsoid penetration on ~6 % of the env-steps of a random-action rollout (regime test),
     # more among the contact-heavy picks here; contact overflow ~1e-5 of env-steps
     assert cnt["regime"] <= MAX_SKIP_REGIME * len(chosen) and cnt["overflow"] <= 3

@@ -11,7 +11,6 @@ import pytest
 
 import philox_ref as P
 
-EPS = np.finfo(np.float64).eps
 
 
 # ------------------------------------------------------------------------------------------------ CPU
@@ -121,56 +120,6 @@ def _env(case, n=N):
     return _ENVS[case, n]
 
 
-def _replay(env, seed, episode):
-    from myosuite_b200 import abi
-    cfg = env.cfg
-    return P.replay_reset(env.mj_model, env.task, seed, env.env_offset + np.arange(env.num_envs), episode, env.init_qpos, env.init_qvel,
-                          target_range=env.t["target_range"].cpu().numpy(), reset_random=bool(cfg.reset_random),
-                          joint_random=(cfg.joint_random[0], cfg.joint_random[1]), ntip=int(cfg.task_i[0]) if env.task in ("reach", "stand") else 0,
-                          hold_d=list(cfg.task_d)[:12], fatigue_random=cfg.muscle_condition == abi.COND_FATIGUE and cfg.fatigue_reset == 1)
-
-
-def _within(got, want, tol, label):
-    excess = np.abs(got - want) - tol
-    assert np.all(excess <= 0), "%s: %d entries off, worst by %.3g beyond %.3g at %s" % (
-        label, int(np.sum(excess > 0)), excess.max(), np.broadcast_to(tol, excess.shape).flat[np.argmax(excess)], np.unravel_index(np.argmax(excess), excess.shape))
-
-
-def _span_tol(lo, hi):
-    """lo + u (hi - lo), with or without an FMA: within 4 eps max(|lo|, |hi|) of numpy's rounding."""
-    return 4 * EPS * np.maximum(np.abs(lo), np.abs(hi))
-
-
-def _compare(env, S, R, label, rows=slice(None)):
-    """Device state S of the envs `rows` against replay R (already restricted to those envs)."""
-    m, cfg, task = env.mj_model, env.cfg, env.task
-    tr = env.t["target_range"].cpu().numpy()
-    if "fatigue" in R:
-        np.testing.assert_array_equal(S["fatigue"][rows], R["fatigue"], err_msg=label + ": fatigue state")
-    if task == "walk":
-        qv = S["qvel"][rows]
-        key = np.where(np.all(qv == env.init_qvel[1], axis=1), 1, np.where(np.all(qv == env.init_qvel[0], axis=1), 0, -1))
-        np.testing.assert_array_equal(key, R["key"], err_msg=label + ": walk keyframe row")
-        _within(S["qpos"][rows], R["qpos"], 1e-15, label + ": walk qpos")
-    elif task == "pose" and cfg.reset_random:
-        free = m.jnt_type == 0
-        adr = m.jnt_qposadr[~free]
-        _within(S["qpos"][rows][:, adr], R["qpos"][:, adr], _span_tol(m.jnt_range[~free, 0], m.jnt_range[~free, 1]), label + ": pose qpos")
-    else:                                                     # stand offsets (numpy's rounding, no contraction) or untouched init_qpos
-        np.testing.assert_array_equal(S["qpos"][rows], R["qpos"], err_msg=label + ": qpos")
-    if "target" in R:
-        cols = m.jnt_qposadr[m.jnt_type != 0] if task == "pose" else np.arange(3 * int(cfg.task_i[0]))
-        _within(S["target"][rows][:, cols], R["target"][:, cols], _span_tol(tr[cols, 0], tr[cols, 1]), label + ": target")
-    if "env_prm" in R:
-        got = S["env_prm"][rows][:, :6]
-        if cfg.reset_random:
-            obj = np.array(cfg.task_d[3:6])
-            lo, hi = np.concatenate([obj - 0.03, [0.02] * 3]), np.concatenate([obj + 0.03, [0.03] * 3])
-            _within(got, R["env_prm"], _span_tol(lo, hi), label + ": hold goal / size")
-        else:
-            np.testing.assert_array_equal(got, R["env_prm"], err_msg=label + ": hold fixed goal / size")
-
-
 def _reset_and_compare(env, label, seed=None, episode=None):
     """reset(seed) (episode counters rewound to 0) or, with seed None, a reset at the current episode counts (set to `episode` first)."""
     import torch
@@ -185,8 +134,8 @@ def _reset_and_compare(env, label, seed=None, episode=None):
     torch.cuda.synchronize()
     S = env.get_env_state()
     np.testing.assert_array_equal(S["episode_count"], ep + 1)
-    R = _replay(env, env.seed_value, ep)
-    _compare(env, S, R, "%s seed %d env_offset %d" % (label, env.seed_value, env.env_offset))
+    R = P.replay_env(env, env.seed_value, ep)
+    P.compare_reset(env, S, R, "%s seed %d env_offset %d" % (label, env.seed_value, env.env_offset))
     return S, R
 
 
@@ -243,9 +192,9 @@ def test_auto_reset_matches_replay():
     assert np.all(reset[forced])
     np.testing.assert_array_equal(S["episode_count"][reset], S0["episode_count"][reset] + 1)
     np.testing.assert_array_equal(S["step_count"][reset], 0)
-    R = _replay(env, 7, S0["episode_count"])
+    R = P.replay_env(env, 7, S0["episode_count"])
     R = {k: v[reset] for k, v in R.items()}
-    _compare(env, S, R, "auto-reset", rows=reset)
+    P.compare_reset(env, S, R, "auto-reset", rows=reset)
 
 
 @pytest.mark.gpu
