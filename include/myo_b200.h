@@ -111,10 +111,15 @@ typedef struct {
   long long* tap_phase_cycles; /* [n, 20] SM-clock cycles per phase over the call (profiling aid; 8-11 solver parts, 12,13: max ncon / nefc, 14,15: Newton iterations / dense ones, 16: cooperative collision, 17: load..substeps) */
   const double* fatigue_reset_vec; /* [nu] nullable unless cfg.fatigue_reset == 2: the reference's fatigue_reset_vec (base_v0.py:29,48; fatigue.py:90-94) */
   int32_t* overflow;         /* [n] nullable: sticky flag, set when a substep of this env dropped contacts (more than maxcon, or more ellipsoid candidates than the list holds); cleared by the env's reset */
+  /* Since version 2.  The observation of the state an episode ended in, written by myo_batch_step for the envs whose done or truncated
+   * it sets, before the auto-reset (if on) overwrites their obs row; without auto-reset it equals obs.  The rows of the other envs are
+   * not written, and reset / observe / forward-debug never write it.  A row is valid exactly where done | truncated of the same step is set. */
+  float* final_obs;          /* [n, obs_dim] out, nullable (needs obs) */
 } myo_buffers;
 
 const char* myo_last_error(void);
-int myo_version(void);
+int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
+                                smaller struct, so callers check that this matches the version of the header they were compiled against */
 
 /* Model from the packed blob produced by myosuite_b200.blob.pack (host arrays; copied).
  * Replaces: MjSpec.from_file(path).compile() + the model upload.  */

@@ -18,6 +18,7 @@ c_i32, c_i64, c_u64, c_f64, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_uint
 TASK_NONE, TASK_POSE, TASK_WALK, TASK_HOLD, TASK_REACH = 0, 1, 2, 3, 4
 RESET_ENV_LIMIT = 1 << 47           # MYO_RESET_ENV_LIMIT: global env ids below it key distinct reset streams
 COND_NONE, COND_FATIGUE = 0, 2
+ABI_VERSION = 2                     # myo_version() of the header this binding mirrors (MyoBuffers ends with final_obs since 2)
 
 
 class MyoDims(ctypes.Structure):
@@ -35,7 +36,7 @@ class MyoTaskCfg(ctypes.Structure):
 BUFFER_FIELDS = ["action", "qpos", "qvel", "act", "qacc_warmstart", "time", "fatigue", "target", "target_range", "init_qpos", "init_qvel", "env_prm",
                  "step_count", "episode_count", "obs", "reward", "done", "truncated", "ep_return", "last_return",
                  "tap_qacc", "tap_actuator_force", "tap_ten_length", "tap_qfrc_smooth", "tap_ncon", "tap_contact_pair",
-                 "tap_contact_dist", "tap_moment", "tap_qM", "tap_phase_cycles", "fatigue_reset_vec", "overflow"]
+                 "tap_contact_dist", "tap_moment", "tap_qM", "tap_phase_cycles", "fatigue_reset_vec", "overflow", "final_obs"]
 
 
 class MyoBuffers(ctypes.Structure):
@@ -99,6 +100,8 @@ def _bind(L):
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     L.myo_batch_launch_info.argtypes = [c_vp, c_vp, ctypes.c_int]
     L.myo_batch_debug_perm.argtypes = [c_vp, c_vp, ctypes.c_int]
+    if L.myo_version() != ABI_VERSION:
+        raise MyoError("%s has ABI version %d, this binding needs %d: rebuild it (python -m myosuite_b200.build)" % (L._name, L.myo_version(), ABI_VERSION))
     return L
 
 

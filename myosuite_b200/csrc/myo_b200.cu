@@ -369,6 +369,11 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
             if (b.step_count) b.step_count[env] = sc; if (b.time) b.time[env] = tnow;
             if (b.ep_return) { float R = b.ep_return[env] + (float)rw; b.ep_return[env] = R; if ((done || trunc) && b.last_return) b.last_return[env] = R; } }
           __syncwarp();
+          // the observation of the state the episode ended in, kept before the auto-reset overwrites obs (the __syncwarp above and the one
+          // closing task_observe make every lane's obs stores visible; the one below orders these reads before the reset's obs stores)
+          if ((done || trunc) && b.final_obs) { const size_t r = (size_t)env*a.obs_dim;
+            for (int i = w.lane; i < a.obs_dim; i += 32) b.final_obs[r+i] = b.obs[r+i];
+            __syncwarp(); }
           if ((done || trunc) && a.cfg.auto_reset) { env_reset(m, w, a, env); task_observe(m, w, a, env, 0, 0.0); if (w.lane == 0 && b.overflow) b.overflow[env] = 0; }
         } else if (w.lane == 0 && b.time) b.time[env] = tnow;
       }
@@ -418,7 +423,7 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
-extern "C" int myo_version(void) { return 1; }
+extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
 
 extern "C" int myo_model_from_blob(const int32_t* I, int64_t nI, const double* D, int64_t nD, myo_model** out) {
   if (!I || !out || nI < MYO_BLOB_HDR + MYO_NDIM + 3*MYO_NSEC) return fail("myo_model_from_blob: bad arguments");
@@ -621,6 +626,7 @@ extern "C" int myo_batch_bind(myo_batch* b, const myo_buffers* bufs) {
   if (b->cfg.muscle_condition == MYO_COND_FATIGUE && !bufs->fatigue) return fail("myo_batch_bind: fatigue buffer required for MYO_COND_FATIGUE");
   if (b->cfg.muscle_condition == MYO_COND_FATIGUE && b->cfg.fatigue_reset == 2 && !bufs->fatigue_reset_vec) return fail("myo_batch_bind: fatigue_reset_vec buffer required for fatigue_reset = 2");
   if (b->cfg.task == MYO_TASK_HOLD && !bufs->env_prm) return fail("myo_batch_bind: env_prm buffer required for MYO_TASK_HOLD");
+  if (bufs->final_obs && !bufs->obs) return fail("myo_batch_bind: final_obs is a copy of obs and needs the obs buffer");
   b->bufs = *bufs; b->bound = true; return 0;
 }
 

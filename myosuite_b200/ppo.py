@@ -8,15 +8,20 @@ tensors that never leave HBM, and the networks are plain torch modules trained w
 of this repository, the simulator is).  Defaults follow the reference's MJX PPO configuration.
 
 Time-limit truncation: MyoVecEnv auto-resets inside the step, so the observation after a `done | truncated` step already belongs to the next
-episode; both end the GAE recursion (like SB3 without terminal-observation bootstrapping).
+episode, and both end the GAE recursion.  By default that is all (like SB3 without terminal-observation bootstrapping): a truncated episode
+is valued as if its last state were terminal.  With PPO(..., bootstrap_truncated=True) (`--bootstrap_truncated`) a step that is truncated
+but not terminated adds gamma V(s_T) to its TD target, V evaluated on the state the episode ended in (the step's info["final_obs"]).
 """
 import math
 import time
 
 
-def gae(rewards, values, dones, last_value, gamma, lam):
+def gae(rewards, values, dones, last_value, gamma, lam, boot=None):
     """Generalised advantage estimate.  rewards / values / dones: [T, n] (dones[t] = episode ended BY step t); last_value: [n] = V(obs after
-    the last step).  Returns (advantages [T, n], returns [T, n])."""
+    the last step).  boot: None, or (boot_mask [T, n], final_values [T, n]) to bootstrap episodes cut by the time limit: where boot_mask[t]
+    is set (truncated and not terminated), the TD target of step t gains gamma final_values[t] = gamma V(the state the episode ended in);
+    final_values must be finite (zero, say) where the mask is clear.  The recursion still stops at dones[t].  Returns (advantages [T, n],
+    returns [T, n])."""
     import torch
     T = rewards.shape[0]
     adv = torch.zeros_like(rewards)
@@ -24,6 +29,8 @@ def gae(rewards, values, dones, last_value, gamma, lam):
     for t in range(T - 1, -1, -1):
         live = 1.0 - dones[t].to(rewards.dtype)
         delta = rewards[t] + gamma * nxt * live - values[t]
+        if boot is not None:
+            delta = delta + gamma * (boot[0][t].to(rewards.dtype) * boot[1][t])
         run = delta + gamma * lam * live * run
         adv[t] = run
         nxt = values[t]
@@ -64,7 +71,7 @@ def _mlp(torch, sizes, out_gain):
 
 class PPO:
     def __init__(self, env, hidden=(64, 64, 64), lr=3e-4, gamma=0.97, lam=0.95, clip=0.3, entropy=1e-3, vf_coef=0.5, max_grad_norm=1.0,
-                 unroll=10, epochs=8, minibatches=32, init_log_std=-0.5, normalize_obs=True, seed=0):
+                 unroll=10, epochs=8, minibatches=32, init_log_std=-0.5, normalize_obs=True, seed=0, bootstrap_truncated=False):
         import torch
         if not env.cfg.auto_reset:
             raise ValueError("PPO needs MyoVecEnv(..., auto_reset=True)")
@@ -73,6 +80,7 @@ class PPO:
         self.gen = torch.Generator(device=self.dev).manual_seed(seed)
         self.gamma, self.lam, self.clip, self.entropy, self.vf_coef, self.max_grad_norm = gamma, lam, clip, entropy, vf_coef, max_grad_norm
         self.unroll, self.epochs, self.minibatches = int(unroll), int(epochs), int(minibatches)
+        self.bootstrap_truncated = bool(bootstrap_truncated)
         od, ad = env.obs_dim, env.act_dim
         self.pi = _mlp(torch, (od, *hidden, ad), 0.01).to(self.dev)
         self.vf = _mlp(torch, (od, *hidden, 1), 1.0).to(self.dev)
@@ -105,13 +113,18 @@ class PPO:
         torch, env, T, n = self.torch, self.env, self.unroll, self.env.num_envs
         O = torch.zeros(T, n, env.obs_dim, device=self.dev); A = torch.zeros(T, n, env.act_dim, device=self.dev)
         R = torch.zeros(T, n, device=self.dev); D = torch.zeros(T, n, dtype=torch.bool, device=self.dev)
+        if self.bootstrap_truncated:          # truncated-not-terminated mask and the observations those episodes ended in
+            B = torch.zeros(T, n, dtype=torch.bool, device=self.dev); FO = torch.zeros(T, n, env.obs_dim, device=self.dev)
         with torch.no_grad():
             for t in range(T):
                 O[t] = self.obs
                 mean = self.pi(self._n(self.obs))
                 A[t] = mean + self.log_std.exp() * torch.randn(mean.shape, device=self.dev, generator=self.gen)
-                obs, rew, done, trunc, _ = env.step(A[t].clamp(-1.0, 1.0))          # the env clips like the reference's action space does
+                obs, rew, done, trunc, info = env.step(A[t].clamp(-1.0, 1.0))          # the env clips like the reference's action space does
                 R[t], D[t] = rew, done.bool() | trunc.bool()
+                if self.bootstrap_truncated:
+                    B[t] = trunc.bool() & ~done.bool()
+                    FO[t] = info["final_obs"]          # (rows outside done | truncated are stale or NaN; masked out below)
                 self.obs = obs
                 self.ep_ret += rew
                 if bool(D[t].any()):
@@ -123,7 +136,10 @@ class PPO:
             V = self.vf(No).squeeze(-1)
             logp = self._logp(self.pi(No), A)
             last_v = self.vf(self._n(self.obs)).squeeze(-1)
-            adv, ret = gae(R, V, D, last_v, self.gamma, self.lam)
+            boot = None
+            if self.bootstrap_truncated:          # V of the final states, normalised like the unroll's observations
+                boot = (B, torch.where(B, self.vf(self._n(FO)).squeeze(-1), 0.0))
+            adv, ret = gae(R, V, D, last_v, self.gamma, self.lam, boot)
         self.total_steps += T * n
         return dict(obs=No.reshape(T * n, -1), act=A.reshape(T * n, -1), logp=logp.reshape(-1), adv=adv.reshape(-1), ret=ret.reshape(-1), rew=R)
 
@@ -175,8 +191,9 @@ if __name__ == "__main__":      # python -m myosuite_b200.ppo --env myoElbowPose
     ap = argparse.ArgumentParser()
     ap.add_argument("--env", default="myoElbowPose1D6MRandom-v0"); ap.add_argument("--num_envs", type=int, default=8192)
     ap.add_argument("--num_timesteps", type=int, default=5_000_000); ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--bootstrap_truncated", action="store_true", help="bootstrap time-limit truncations with V(final observation)")
     a = ap.parse_args()
-    agent = PPO(vec_env.MyoVecEnv(a.env, a.num_envs, seed=a.seed), seed=a.seed)
+    agent = PPO(vec_env.MyoVecEnv(a.env, a.num_envs, seed=a.seed), seed=a.seed, bootstrap_truncated=a.bootstrap_truncated)
     t0 = time.perf_counter()
     h = agent.train(a.num_timesteps, log=lambda r: print({k: (round(v, 4) if isinstance(v, float) else v) for k, v in r.items()}))
     print("PPO training for %d total steps on %d envs took %.2f s (%.0f env-steps/s incl. updates)" % (h[-1]["steps"], a.num_envs, time.perf_counter() - t0, h[-1]["steps_per_s"]))

@@ -136,6 +136,8 @@ class MyoVecEnv:
             t["fatigue"][:, 1, :] = 1.0
             if self.fatigue_reset_vec is not None:
                 t["fatigue_reset_vec"] = torch.as_tensor(self.fatigue_reset_vec, device=dv).contiguous()
+        if cfg.task != abi.TASK_NONE:          # the observation each ended episode ended in (written by the step kernel; NaN until an env first ends)
+            t["final_obs"] = torch.full((n, self.full_obs_dim), float("nan"), dtype=f32, device=dv)
         if taps:
             t.update(tap_qacc=z(n, m.nv), tap_actuator_force=z(n, m.nu), tap_ten_length=z(n, m.nu), tap_qfrc_smooth=z(n, m.nv),
                      tap_ncon=z(n, 4, dtype=torch.int32), tap_contact_pair=z(n, max(self.dims.maxcon, 1), dtype=torch.int32),
@@ -144,8 +146,11 @@ class MyoVecEnv:
         self.t = t
         self.batch.bind(**t)
         t["obs_full"] = t["obs"]                                  # what the kernel writes (bound above); t["obs"] is what callers see
+        if "final_obs" in t:
+            t["final_obs_full"] = t["final_obs"]                  # likewise for final_obs
         if self._obs_cols is not None:
             t["obs"] = z(n, self.obs_dim, dtype=f32)
+            t["final_obs"] = torch.full((n, self.obs_dim), float("nan"), dtype=f32, device=dv)
         self._h_action = None
 
     def _sync_obs(self):
@@ -205,7 +210,12 @@ class MyoVecEnv:
         return self.torch.cuda.current_stream(self.device).cuda_stream
 
     def step(self, action):
-        """action: float32 CUDA tensor [num_envs, nu] (values as the reference's action_space: [-1, 1])."""
+        """action: float32 CUDA tensor [num_envs, nu] (values as the reference's action_space: [-1, 1]).
+
+        info["final_obs"] [num_envs, obs_dim] (the layout of obs) holds the observation of the state each episode that ended on this step
+        ended in: with auto-reset, obs already belongs to the next episode.  A row is valid exactly where done | truncated of the same
+        step is set; other rows keep what an earlier step wrote (NaN before an env first ends).  The tensor is reused by every step.
+        None for the physics-only batch."""
         a = self.t["action"]
         if action.data_ptr() != a.data_ptr():
             if tuple(action.shape) != tuple(a.shape):
@@ -214,7 +224,10 @@ class MyoVecEnv:
         self.batch.step(stream=self._stream())
         self._sync_obs()
         t = self.t
-        return t["obs"], t["reward"], t["done"], t["truncated"], {"last_return": t["last_return"], "time": t["time"], "overflow": t["overflow"]}
+        if self._obs_cols is not None:
+            self.torch.index_select(t["final_obs_full"], 1, self._obs_cols, out=t["final_obs"])
+        return t["obs"], t["reward"], t["done"], t["truncated"], {"last_return": t["last_return"], "time": t["time"], "overflow": t["overflow"],
+                                                                  "final_obs": t.get("final_obs")}
 
     def step_host(self, action_cpu_pinned):
         """End-to-end call with HOST buffers: H2D action copy, step, D2H of reward/done (the e2e bench path)."""
@@ -268,6 +281,14 @@ class MyoVecEnv:
         """`rwd_sparse` / `solved` of the current observations (the reference's info dict, env_base.py:585-616), derived lazily from obs."""
         m = self.mj_model
         return tasks.info_from_obs(self.task, self.t["obs_full"], m.nq, m.nv, m.na, pose_thd=float(self.cfg.pose_thd), ntip=len(self.tip_names) or None)
+
+    def final_task_info(self):
+        """`rwd_sparse` / `solved` of the states the episodes ended in (task_info of info["final_obs"]): valid in the rows where done |
+        truncated of the last step is set.  None for tasks without a distance-type success signal (walk), like task_info."""
+        if "final_obs_full" not in self.t:
+            return None
+        m = self.mj_model
+        return tasks.info_from_obs(self.task, self.t["final_obs_full"], m.nq, m.nv, m.na, pose_thd=float(self.cfg.pose_thd), ntip=len(self.tip_names) or None)
 
     def refresh_obs(self):
         """obs / reward / done of the current state (the reference's env.forward(), env_base.py:393-432)."""
