@@ -671,8 +671,9 @@ __device__ __forceinline__ void store_contact(const DevModel& m, double* con, id
   double y0 = 0, y1 = 0, y2 = 0;
   if (o.has_y) { y0 = o.yx; y1 = o.yy; y2 = o.yz; }
   if (y0*y0+y1*y1+y2*y2 < 0.25) { y0 = 0; y1 = 0; y2 = 0; if (c.ny < 0.5 && c.ny > -0.5) y1 = 1; else y2 = 1; }
-  double dd = c.nx*y0+c.ny*y1+c.nz*y2; y0 -= dd*c.nx; y1 -= dd*c.ny; y2 -= dd*c.nz; double n = m_rcp(m_sqrt(y0*y0+y1*y1+y2*y2));
-  f[3] = y0*n; f[4] = y1*n; f[5] = y2*n;
+  double dd = c.nx*y0+c.ny*y1+c.nz*y2; y0 -= dd*c.nx; y1 -= dd*c.ny; y2 -= dd*c.nz; const double yn = m_sqrt(y0*y0+y1*y1+y2*y2);
+  // a hint along the normal (a capsule standing upright on a plane) leaves nothing to normalise: (1, 0, 0), as mju_normalize3 does
+  if (yn < MYO_MINVAL) { f[3] = 1; f[4] = 0; f[5] = 0; } else { const double n = m_rcp(yn); f[3] = y0*n; f[4] = y1*n; f[5] = y2*n; }
   icon[ci] = (idx_t)p; }
 
 // Contacts are found by the analytic colliders first ([0, na)), then by the iterative ellipsoid colliders ([na, ncon)), each run in model pair
