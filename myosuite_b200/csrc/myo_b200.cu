@@ -481,6 +481,7 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   ext = imax(ext, c1);
   d.kcand = d.npair - d.npair_an; d.ngc = P[PD_NGC];
   d.s_gpose = afterK; d.s_clist = afterK + al2(6*d.ngc); ext = imax(ext, d.s_clist + al2((d.kcand + 1)/2));
+  ext = imax(ext, d.s_gpose + al2(2*d.njnt));      // the hinge sines / cosines of the kinematics phase (phase_kinematics)
   const int extNonSolve = ext;
   int t = head;
   d.s_conJ = t; t += al2(imax((3*d.maxpath*mc*JAC_BYTES + 7)/8, (mc + 1)/2)); d.s_efD = t; t += al2(d.neq + d.nlimrow + mc); d.s_eqJ = t; t += al2(d.neq);      /* (the Jacobian region doubles as the int rank keys of the contact ordering) */

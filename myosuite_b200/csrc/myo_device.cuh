@@ -144,8 +144,9 @@ __device__ void phase_kinematics(const DevModel& m, const Warp w) {
   const double* jpos = CD(jnt_pos); const double* jaxis = CD(jnt_axis); const double* qpos0 = CD(qpos0);
   double* xpos = SCR(s_xpos); double* xmat = SCR(s_xmat);
   // sin / cos of every hinge angle in ONE lane-parallel pass (the level loop below would otherwise run the sincos code once per tree level with
-  // a handful of lanes active).  Parked in the head of the Hessian region, which is idle until the constraint phase (the tail holds the warm start).
-  double* sc = SCR(s_H);
+  // a handful of lanes active).  Parked in the collision geom-pose region right after the body poses: idle until collision, and it cannot
+  // overlap xpos / xmat, which the level loop writes while later levels still read their sines (the Hessian region can start inside them).
+  double* sc = SCR(s_gpose);
   for (int j = w.lane; j < m.njnt; j += 32) { const int t = jtype[j]; if (t != 0 && t != 2) { double s_, c_; sincos(W_(qpos)[jq[j]] - qpos0[jq[j]], &s_, &c_); sc[2*j] = s_; sc[2*j+1] = c_; } }
   __syncwarp();
   for (int L = 0; L < m.nlevel; L++) {
