@@ -46,7 +46,14 @@ class MyoBuffers(ctypes.Structure):
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
-           "myo_batch_launch_info", "myo_batch_debug_perm"]
+           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout"]
+
+# myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
+LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
+LAYOUT_SCRATCH = ("xpos", "xmat", "U", "PL", "mom", "tlen", "tvel", "tfrc", "cin", "crb", "bf", "conJ", "efD", "efA", "eqJ", "icon", "con", "clist",
+                  "gpose", "efR", "efV", "va", "vg", "vp", "vMa", "vMp", "H", "Hs", "LD", "Dinv")
+LAYOUT_SCALARS = ("head", "afterK", "extNonSolve", "solveEnd", "arefInH", "qwsInH", "n_per_warp", "maxcon", "maxefc")
+LAYOUT_N = 2 * len(LAYOUT_PERSISTENT) + 2 * len(LAYOUT_SCRATCH) + len(LAYOUT_SCALARS)
 
 
 class MyoError(RuntimeError):
@@ -84,6 +91,7 @@ def _bind(L):
     L.myo_last_error.restype = ctypes.c_char_p
     L.myo_model_from_blob.argtypes = [c_vp, c_i64, c_vp, c_i64, ctypes.POINTER(c_vp)]
     L.myo_model_dims.argtypes = [c_vp, ctypes.POINTER(MyoTaskCfg), ctypes.POINTER(MyoDims)]
+    L.myo_model_layout.argtypes = [c_vp, ctypes.POINTER(MyoTaskCfg), c_vp, ctypes.c_int]
     L.myo_model_destroy.argtypes = [c_vp]
     L.myo_model_destroy.restype = None
     L.myo_batch_create.argtypes = [c_vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(MyoTaskCfg), ctypes.POINTER(c_vp)]
@@ -125,6 +133,18 @@ class DeviceModel:
         d = MyoDims()
         _check(self.L.myo_model_dims(self.handle, ctypes.byref(cfg) if cfg is not None else None, ctypes.byref(d)), self.L)
         return d
+
+    def layout(self, cfg=None):
+        """Shared-memory layout of one env's slice (myo_model_layout; no device needed), in doubles from the slice start:
+        {"o": {persistent region: offset}, "o_size": {...}, "s": {scratch region: offset}, "s_size": {...}, and the scalars}."""
+        v = np.zeros(LAYOUT_N, dtype=np.int32)
+        _check(self.L.myo_model_layout(self.handle, ctypes.byref(cfg) if cfg is not None else None, v.ctypes.data, v.size), self.L)
+        v = [int(x) for x in v]
+        npr, nsc = len(LAYOUT_PERSISTENT), len(LAYOUT_SCRATCH)
+        out = {"o": dict(zip(LAYOUT_PERSISTENT, v[:npr])), "o_size": dict(zip(LAYOUT_PERSISTENT, v[npr:2 * npr])),
+               "s": dict(zip(LAYOUT_SCRATCH, v[2 * npr:2 * npr + nsc])), "s_size": dict(zip(LAYOUT_SCRATCH, v[2 * npr + nsc:2 * npr + 2 * nsc]))}
+        out.update(zip(LAYOUT_SCALARS, v[2 * npr + 2 * nsc:]))
+        return out
 
     def __del__(self):
         if getattr(self, "handle", None):

@@ -378,9 +378,11 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
         } else if (w.lane == 0 && b.time) b.time[env] = tnow;
       }
       __syncwarp();
-      // ---- store state
+      // ---- store state.  A forward pass without substeps runs the solve but not the integrator, so the warm start was not rewritten, and
+      // where it lives in the Hessian tail (fill_devmodel) the solve has overwritten it: the caller's warm start stays as it was.
+      const bool store_qws = !(DBG && a.mode == 1 && !integrate);
       for (int i = w.lane; i < m.nq; i += 32) b.qpos[(size_t)env*m.nq+i] = W_(qpos)[i];
-      for (int i = w.lane; i < m.nv; i += 32) { b.qvel[(size_t)env*m.nv+i] = W_(qvel)[i]; b.qacc_warmstart[(size_t)env*m.nv+i] = W_(qws)[i]; }
+      for (int i = w.lane; i < m.nv; i += 32) { b.qvel[(size_t)env*m.nv+i] = W_(qvel)[i]; if (store_qws) b.qacc_warmstart[(size_t)env*m.nv+i] = W_(qws)[i]; }
       for (int i = w.lane; i < m.na; i += 32) b.act[(size_t)env*m.na+i] = W_(act)[i];
       __syncwarp();
     }
@@ -437,8 +439,15 @@ extern "C" void myo_model_destroy(myo_model* m) { delete m; }
 
 static int al2(int x) { return (x + 1) & ~1; }
 static int imax(int a, int b) { return a > b ? a : b; }
-static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel& d) {
+// What fill_devmodel decided beyond the DevModel offsets (myo_model_layout): the size reserved for every persistent and scratch region
+// (slot orders of include/myo_b200.h) and the boundaries and flags of the scratch scheme, the latter relative to the scratch start.
+enum { LP_qpos, LP_qvel, LP_act, LP_qws, LP_dax, LP_dan, LP_qM, LP_fsm, LP_eprm, LP_wz, LP_cnt, LP_scr, LP_N };
+enum { LS_xpos, LS_xmat, LS_U, LS_PL, LS_mom, LS_tlen, LS_tvel, LS_tfrc, LS_cin, LS_crb, LS_bf, LS_conJ, LS_efD, LS_efA, LS_eqJ,
+       LS_icon, LS_con, LS_clist, LS_gpose, LS_efR, LS_efV, LS_va, LS_vg, LS_vp, LS_vMa, LS_vMp, LS_H, LS_Hs, LS_LD, LS_Dinv, LS_N };
+struct Layout { int32_t psz[LP_N], ssz[LS_N], head, afterK, extNonSolve, solveEnd, arefInH, qwsInH; };
+static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel& d, Layout* lay = nullptr) {
   const int32_t* I = mm->I.data(); const double* D = mm->D.data(); memset(&d, 0, sizeof(d));
+  Layout L_; Layout& L = lay ? *lay : L_; memset(&L, 0, sizeof(L));
   const int32_t* hoff = MYO_ISEC(I, MYO_SEC_HOT_off);
   for (int s = 0; s < MYO_NSEC; s++) d.hoff[s] = hoff[s];
   d.nI16w = MYO_SEC_LEN(I, MYO_SEC_HOT_I16); d.nD = hoff[MYO_NSEC] >= 0 ? hoff[MYO_NSEC] : MYO_SEC_LEN(I, MYO_SEC_HOT_D);      // doubles staged to shared memory (the cold tables behind them stay in HBM)
@@ -452,12 +461,12 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   d.ovr_geom = (cfg && cfg->task == MYO_TASK_HOLD) ? cfg->task_i[1] : -1;
   int mc = cfg && cfg->maxcon > 0 ? cfg->maxcon : 32; if (mc > 64) mc = 64; if (mc > 2*d.npair) mc = 2*d.npair; /* (the contact-order merge handles up to 64) */ d.maxcon = mc; d.nlimrow = P[PD_NLIMROW] > 0 ? P[PD_NLIMROW] : 2*d.nlim; d.maxefc = d.neq + d.nlimrow + 4*mc;
   int o = 0;
-  #define TAKE(field, n) d.field = o; o += al2(n)
+  #define TAKE(field, n) d.o_##field = o; L.psz[LP_##field] = al2(n); o += al2(n)
   // persistent per-env arrays.  ctrl is NOT here: it is written once per control step to a library-owned global row and re-read by the actuation
   // phase of every substep (an L2 hit); the solver's warm start lives in the tail of the Hessian region when that tail is provably idle (below).
-  TAKE(o_qpos, d.nq); TAKE(o_qvel, d.nv); TAKE(o_act, d.na); TAKE(o_dax, 3*d.nv); TAKE(o_dan, 3*d.nv); TAKE(o_qM, d.nM); TAKE(o_fsm, d.nv);
-  d.neprm = (cfg && cfg->task == MYO_TASK_HOLD) ? 8 : 0; TAKE(o_eprm, d.neprm); d.nwz = P[PD_NWE_SPH_IN] + P[PD_NWE_CYL_IN]; TAKE(o_wz, d.nwz); TAKE(o_cnt, CNT_N/2);
-  d.nvp = chol_pad(d.nv);
+  TAKE(qpos, d.nq); TAKE(qvel, d.nv); TAKE(act, d.na); TAKE(dax, 3*d.nv); TAKE(dan, 3*d.nv); TAKE(qM, d.nM); TAKE(fsm, d.nv);
+  d.neprm = (cfg && cfg->task == MYO_TASK_HOLD) ? 8 : 0; TAKE(eprm, d.neprm); d.nwz = P[PD_NWE_SPH_IN] + P[PD_NWE_CYL_IN]; TAKE(wz, d.nwz); TAKE(cnt, CNT_N/2);
+  d.nvp = chol_pad(d.nv); L.psz[LP_qws] = al2(d.nv);
   const int o_qws_persistent = o;          // (claimed only if the warm start cannot alias the Hessian tail)
   // ---- scratch, time-multiplexed by stage (offsets from d.o_scr, fixed up at the end).  Lifetimes:
   //   head: icon (contact / row integer records), con (contact records)     collision .. constraints ; in the solve the con region holds jar, jv
@@ -469,26 +478,30 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   const int icon = al2(mc + (mc + 1)/2 + (2*(mc + d.nlimrow + 4) + d.maxefc + 7)/8);       // cmask u64[mc] | crown i32[mc] | cpair i16[mc] | lrow i16[nlimrow+4] | drow u8[maxefc]
   const int rows = al2(d.maxefc), conReg = imax(al2(CON_STRIDE*mc), 2*rows), K = al2(3*d.nbd) + al2(9*d.nbd);
   d.s_icon = 0; d.s_con = icon; d.s_efR = icon; d.s_efV = icon + rows; const int head = icon + conReg;
-  d.s_xpos = head; d.s_xmat = head + al2(3*d.nbd); const int afterK = head + K;
+  L.ssz[LS_icon] = icon; L.ssz[LS_con] = conReg; L.ssz[LS_efR] = rows; L.ssz[LS_efV] = rows;
+  d.s_xpos = head; d.s_xmat = head + al2(3*d.nbd); const int afterK = head + K; L.ssz[LS_xpos] = al2(3*d.nbd); L.ssz[LS_xmat] = al2(9*d.nbd);
   int c0, c1, ext;      // two cursors: inside [0, head) and after K
-  #define PLACE(field, n) { const int n_ = al2(n); if (c0 + n_ <= head) { d.field = c0; c0 += n_; } else { d.field = c1; c1 += n_; } }
+  #define PLACE(field, n) { const int n_ = al2(n); L.ssz[LS_##field] = n_; if (c0 + n_ <= head) { d.s_##field = c0; c0 += n_; } else { d.s_##field = c1; c1 += n_; } }
   c0 = 0; c1 = afterK;
-  PLACE(s_mom, d.nnz); PLACE(s_tlen, d.nta); PLACE(s_tvel, d.nta); PLACE(s_tfrc, d.nta); { const int nsA = d.tg_sp[1], nsB = d.nsp - nsA, nwA = d.tg_we[1], nwB = d.nwe - nwA;      // one tendon group at a time lives in U / PL
-    PLACE(s_PL, imax(nsA + nwA, nsB + nwB)); PLACE(s_U, 3*imax(nsA + 2*nwA, nsB + 2*nwB)); }
+  PLACE(mom, d.nnz); PLACE(tlen, d.nta); PLACE(tvel, d.nta); PLACE(tfrc, d.nta); { const int nsA = d.tg_sp[1], nsB = d.nsp - nsA, nwA = d.tg_we[1], nwB = d.nwe - nwA;      // one tendon group at a time lives in U / PL
+    PLACE(PL, imax(nsA + nwA, nsB + nwB)); PLACE(U, 3*imax(nsA + 2*nwA, nsB + 2*nwB)); }
   ext = c1;
   c0 = 0; c1 = afterK;
-  PLACE(s_cin, 10*d.nbd); PLACE(s_crb, 10*d.nbd); PLACE(s_bf, 6*d.nbd);
+  PLACE(cin, 10*d.nbd); PLACE(crb, 10*d.nbd); PLACE(bf, 6*d.nbd);
   ext = imax(ext, c1);
   d.kcand = d.npair - d.npair_an; d.ngc = P[PD_NGC];
-  d.s_gpose = afterK; d.s_clist = afterK + al2(6*d.ngc); ext = imax(ext, d.s_clist + al2((d.kcand + 1)/2));
+  d.s_gpose = afterK; d.s_clist = afterK + al2(6*d.ngc); ext = imax(ext, d.s_clist + al2((d.kcand + 1)/2)); L.ssz[LS_gpose] = al2(6*d.ngc); L.ssz[LS_clist] = al2((d.kcand + 1)/2);
   ext = imax(ext, d.s_gpose + al2(2*d.njnt));      // the hinge sines / cosines of the kinematics phase (phase_kinematics)
   const int extNonSolve = ext;
   int t = head;
-  d.s_conJ = t; t += al2(imax((3*d.maxpath*mc*JAC_BYTES + 7)/8, (mc + 1)/2)); d.s_efD = t; t += al2(d.neq + d.nlimrow + mc); d.s_eqJ = t; t += al2(d.neq);      /* (the Jacobian region doubles as the int rank keys of the contact ordering) */
+  L.ssz[LS_conJ] = al2(imax((3*d.maxpath*mc*JAC_BYTES + 7)/8, (mc + 1)/2)); L.ssz[LS_efD] = al2(d.neq + d.nlimrow + mc); L.ssz[LS_eqJ] = al2(d.neq);
+  d.s_conJ = t; t += L.ssz[LS_conJ]; d.s_efD = t; t += L.ssz[LS_efD]; d.s_eqJ = t; t += L.ssz[LS_eqJ];      /* (the Jacobian region doubles as the int rank keys of the contact ordering) */
   d.s_va = t; t += al2(d.nvp); d.s_vg = t; d.s_vp = t; t += al2(d.nvp); d.s_vMa = t; t += al2(d.nvp); d.s_vMp = t; t += al2(d.nvp);
+  L.ssz[LS_va] = L.ssz[LS_vg] = L.ssz[LS_vp] = L.ssz[LS_vMa] = L.ssz[LS_vMp] = al2(d.nvp);
   const int hsize = imax(al2(d.nvp*(d.nvp+1)/2), 2*al2(d.nM) + al2(d.nv)); const bool arefInH = rows <= hsize;
   d.s_efA = t; if (!arefInH) t += rows;      /* aref (constraints -> start of the solve) lives in the Hessian region when it fits: H is first written after its last read */
   d.s_H = t; d.s_Hs = t; d.s_LD = t + al2(d.nM); d.s_Dinv = t + 2*al2(d.nM); if (arefInH) d.s_efA = t; t += hsize;
+  L.ssz[LS_efA] = rows; L.ssz[LS_H] = hsize; L.ssz[LS_Hs] = L.ssz[LS_LD] = al2(d.nM); L.ssz[LS_Dinv] = hsize - 2*al2(d.nM);
   // warm start in the last nv slots of the Hessian region: read once at the start of the solve (before any write to H), rewritten at the end
   // of the integrator (after the last read of H).  Requires that no other stage reaches that far and that aref (head of H) does not overlap it.
   int qws = t - al2(d.nv);
@@ -496,6 +509,7 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   ext = imax(ext, t);
   int scratch = ext;
   if (qwsInH) { d.o_scr = o; d.o_qws = o + qws; } else { d.o_qws = o_qws_persistent; o += al2(d.nv); d.o_scr = o; }
+  L.psz[LP_scr] = scratch; L.head = head; L.afterK = afterK; L.extNonSolve = extNonSolve; L.solveEnd = t; L.arefInH = arefInH; L.qwsInH = qwsInH;
   #undef PLACE
   #undef TAKE
   // scratch offsets are used relative to the warp base
@@ -509,6 +523,23 @@ extern "C" int myo_model_dims(const myo_model* m, const myo_task_cfg* cfg, myo_d
   if (!m || !out) return fail("myo_model_dims: null"); DevModel d; fill_devmodel(m, cfg, d); const int32_t* I = m->I.data();
   memset(out, 0, sizeof(*out)); out->nq = d.nq; out->nv = d.nv; out->nu = d.nu; out->na = d.na; out->nbody = MYO_DIM(I, MYO_DIM_nbody); out->njnt = d.njnt; out->ntendon = MYO_DIM(I, MYO_DIM_ntendon);
   out->nM = d.nM; out->npair = d.npair; out->nta = d.nta; out->maxcon = d.maxcon; out->maxefc = d.maxefc; out->smem_bytes_per_env = d.n_per_warp*8; out->reserved[0] = d.nnz; out->reserved[1] = d.nD*8 + ((d.nI16w + 1)/2)*8; return 0;
+}
+
+extern "C" int myo_model_layout(const myo_model* m, const myo_task_cfg* cfg, int32_t* out, int cap) {
+  if (!m || !out || cap < 1) return fail("myo_model_layout: bad arguments");
+  DevModel d; Layout L; fill_devmodel(m, cfg, d, &L);
+  const int32_t po[LP_N] = {d.o_qpos, d.o_qvel, d.o_act, d.o_qws, d.o_dax, d.o_dan, d.o_qM, d.o_fsm, d.o_eprm, d.o_wz, d.o_cnt, d.o_scr};
+  const int32_t so[LS_N] = {d.s_xpos, d.s_xmat, d.s_U, d.s_PL, d.s_mom, d.s_tlen, d.s_tvel, d.s_tfrc, d.s_cin, d.s_crb, d.s_bf, d.s_conJ, d.s_efD, d.s_efA, d.s_eqJ,
+                            d.s_icon, d.s_con, d.s_clist, d.s_gpose, d.s_efR, d.s_efV, d.s_va, d.s_vg, d.s_vp, d.s_vMa, d.s_vMp, d.s_H, d.s_Hs, d.s_LD, d.s_Dinv};
+  int32_t v[MYO_LAYOUT_N]; int k = 0;
+  for (int i = 0; i < LP_N; i++) v[k++] = po[i];
+  for (int i = 0; i < LP_N; i++) v[k++] = L.psz[i];
+  for (int i = 0; i < LS_N; i++) v[k++] = so[i];
+  for (int i = 0; i < LS_N; i++) v[k++] = L.ssz[i];
+  const int32_t tail[] = {d.o_scr + L.head, d.o_scr + L.afterK, d.o_scr + L.extNonSolve, d.o_scr + L.solveEnd, L.arefInH, L.qwsInH, d.n_per_warp, d.maxcon, d.maxefc};
+  for (int32_t x : tail) v[k++] = x;
+  for (int i = 0; i < cap && i < MYO_LAYOUT_N; i++) out[i] = v[i];
+  return 0;
 }
 
 extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const myo_task_cfg* cfg, myo_batch** out) {
