@@ -117,6 +117,34 @@ typedef struct {
   float* final_obs;          /* [n, obs_dim] out, nullable (needs obs) */
 } myo_buffers;
 
+/* Caller-owned device buffers of a readout of mjData (myo_batch_data), all nullable: only the non-null fields are computed.  Every
+ * value equals MuJoCo's mjData after mj_forward at the env's current (time, qpos, qvel, act) with the per-env overrides (env_prm,
+ * targets) applied and ctrl = the last env step's ctrl (zeros before the first step).  MuJoCo ids and order, f64 unless noted. */
+typedef struct {
+  /* pose group: mj_kinematics (the quaternion chain: xquat carries MuJoCo's sign, xmat = quat2mat(xquat)) */
+  double* xpos;              /* [n, nbody, 3] */
+  double* xquat;             /* [n, nbody, 4] */
+  double* xmat;              /* [n, nbody, 9] */
+  double* site_xpos;         /* [n, nsite, 3] */
+  /* [nsite, 2] in, nullable (every site at its model site_pos): where the local position of each site comes from, as (kind, index):
+   * 0 model site_pos ; 1 target[env, index .. index+2] ; 2 env_prm[env, index .. index+2] ; 3 the world position of site `index` at the
+   * forward kinematics of qpos := target[env] (the pose task's target markers).  Kinds 1-3 fall back to 0 when their buffer is unbound. */
+  const int32_t* site_source;
+  /* actuation group: transmission, velocities, muscle forces */
+  double* actuator_length;   /* [n, nu] */
+  double* actuator_velocity; /* [n, nu] */
+  double* actuator_force;    /* [n, nu] */
+  double* qfrc_actuator;     /* [n, nv] */
+  /* dynamics group: collision and the constraint solve (no integration; the warm start is read, never written) */
+  double* qacc;              /* [n, nv] */
+  int32_t* ncon;             /* [n] */
+  int32_t* contact_geom;     /* [n, maxcon, 2] geom1, geom2 in model pair order, -1 padded */
+  double* contact_dist;      /* [n, maxcon]    0 padded */
+  double* contact_pos;       /* [n, maxcon, 3] */
+  double* contact_frame;     /* [n, maxcon, 9] rows normal, tangent1, tangent2 */
+  double* contact_force;     /* [n, maxcon, 6] mj_contactForce: the pyramid forces decoded into the contact frame, normal first */
+} myo_data_buffers;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -171,6 +199,12 @@ int myo_batch_observe(myo_batch* b, void* stream);
  * verbatim (no sigmoid), writing the tap_* buffers; state is not advanced.  If n_substeps > 0 the
  * state IS advanced by that many mj_step's with the same ctrl (taps hold the last forward). */
 int myo_batch_forward_debug(myo_batch* b, const double* ctrl_dev /* [n, nu] */, int n_substeps, void* stream);
+
+/* Readout of mjData for every env (the fields of myo_data_buffers that are non-null), one launch on `stream`; the state is not
+ * advanced and no bound buffer is written.  The deepest requested group decides how much of the forward pass runs: the pose group
+ * alone needs kinematics, the actuation group adds tendons and muscles, the dynamics group adds collision and the constraint solve.
+ * Replaces reading env.unwrapped.mj_data after reset() / step() (envs/env_base.py:77-92, robot/robot.py:595-607). */
+int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

@@ -43,10 +43,27 @@ class MyoBuffers(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in BUFFER_FIELDS]
 
 
+# myo_data_buffers (include/myo_b200.h): the mjData readout of myo_batch_data, field -> (group, dtype, trailing shape in the model's sizes)
+DATA_FIELDS = ["xpos", "xquat", "xmat", "site_xpos", "site_source", "actuator_length", "actuator_velocity", "actuator_force", "qfrc_actuator",
+               "qacc", "ncon", "contact_geom", "contact_dist", "contact_pos", "contact_frame", "contact_force"]
+DATA_SHAPES = {"xpos": ("pose", "f64", ("nbody", 3)), "xquat": ("pose", "f64", ("nbody", 4)), "xmat": ("pose", "f64", ("nbody", 9)),
+               "site_xpos": ("pose", "f64", ("nsite", 3)),
+               "actuator_length": ("actuation", "f64", ("nu",)), "actuator_velocity": ("actuation", "f64", ("nu",)),
+               "actuator_force": ("actuation", "f64", ("nu",)), "qfrc_actuator": ("actuation", "f64", ("nv",)),
+               "qacc": ("dynamics", "f64", ("nv",)), "ncon": ("dynamics", "i32", ()), "contact_geom": ("dynamics", "i32", ("maxcon", 2)),
+               "contact_dist": ("dynamics", "f64", ("maxcon",)), "contact_pos": ("dynamics", "f64", ("maxcon", 3)),
+               "contact_frame": ("dynamics", "f64", ("maxcon", 9)), "contact_force": ("dynamics", "f64", ("maxcon", 6))}
+SITE_MODEL, SITE_TARGET, SITE_ENV_PRM, SITE_AT_TARGET_POSE = 0, 1, 2, 3       # myo_data_buffers.site_source kinds
+
+
+class MyoDataBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in DATA_FIELDS]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
-           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout"]
+           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -103,6 +120,7 @@ def _bind(L):
     L.myo_batch_step.argtypes = [c_vp, c_vp]
     L.myo_batch_observe.argtypes = [c_vp, c_vp]
     L.myo_batch_forward_debug.argtypes = [c_vp, c_vp, ctypes.c_int, c_vp]
+    L.myo_batch_data.argtypes = [c_vp, ctypes.POINTER(MyoDataBuffers), c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -199,6 +217,19 @@ class Batch:
 
     def forward_debug(self, ctrl, n_substeps=0, stream=None):
         _check(self.L.myo_batch_forward_debug(self.handle, ctrl.data_ptr(), n_substeps, stream), self.L)
+
+    def data(self, stream=None, **tensors):
+        """mjData readout (myo_batch_data) into the given torch CUDA tensors (names of DATA_FIELDS; only these are computed)."""
+        d = MyoDataBuffers()
+        for k, t in tensors.items():
+            if k not in DATA_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_data(self.handle, ctypes.byref(d), stream), self.L)
 
     @property
     def launches(self):

@@ -398,6 +398,163 @@ extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14(const __gri
 // parity taps / forward-debug / profiling counters / tuning knobs
 extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<true, 320>(m, a); }
 
+// ------------------------------------------------------------------ mjData readout (myo_batch_data)
+// One forward pass over the stored state of every env, one env per warp on the balanced map (env = CTA + grid * slot).  Each field is
+// written while the scratch region holding it is live; nothing is stored back (the Newton warm start is read, the inverse-wrap roots
+// start cold).  The body poses are MuJoCo's quaternion chain over every model body (mj_kinematics), so that xquat carries MuJoCo's
+// sign; they come from the model tables in HBM and do not touch shared memory.
+// The model constants into shared memory, as env_kernel_body stages them (bulk async copies, completion on an mbarrier); a copy of that
+// code, so that the step kernels are compiled from unchanged source.  Every thread of the CTA calls it.
+__device__ __forceinline__ void stage_model(const DevModel& m, unsigned long long& mbar) {
+  double* s_d = smem; idx_t* s_i = (idx_t*)(smem + m.nD);
+  const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
+  if (threadIdx.x == 0) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb)); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned bytes_d = (unsigned)m.nD*8u, bytes_i = (unsigned)m.nI16w*4u;
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes_d + bytes_i) : "memory");
+    const unsigned CH = 32768u;   // chunked: every piece 16-byte aligned and a multiple of 16 bytes
+    for (unsigned o = 0; o < bytes_d; o += CH) { unsigned n = bytes_d - o < CH ? bytes_d - o : CH;
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_d + o)), "l"((const char*)m.gD + o), "r"(n), "r"(mb) : "memory"); }
+    for (unsigned o = 0; o < bytes_i; o += CH) { unsigned n = bytes_i - o < CH ? bytes_i - o : CH;
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_i + o)), "l"((const char*)m.gI16 + o), "r"(n), "r"(mb) : "memory"); }
+  }
+  { unsigned done = 0; while (!done) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(mb) : "memory"); }
+}
+
+enum { DATA_NONE = 0, DATA_ACT = 1, DATA_DYN = 2 };      // how far the shared-memory forward pass runs
+struct DataArgs {
+  myo_data_buffers d; myo_buffers b;
+  int n_env, depth, pose, nbody, nsite, nlevel; double tol;
+  const int32_t *lvl, *parent, *jadr, *jnum, *jtype, *jq, *site_body, *pair_geom;   // lvl: level_adr[nlevel + 1], then the bodies in level order
+  const double *bpos, *bquat, *jpos, *jaxis, *qpos0, *site_pos;
+  double* pose_buf;             // [n_env, 2, nbody, 7] library-owned: pos, quat of every body at qpos (slot 0) and at the target row (slot 1)
+};
+
+// mj_kinematics at `qpos` (global row), lanes over the bodies of one tree level at a time: world position and unit quaternion per body
+__device__ void data_kinematics(const DataArgs& a, const double* qpos, double* P, int lane) {
+  for (int L = 0; L < a.nlevel; L++) {
+    for (int k = a.lvl[L] + lane; k < a.lvl[L+1]; k += 32) { const int bd = a.lvl[a.nlevel + 1 + k]; double pos[3] = {0, 0, 0}, quat[4] = {1, 0, 0, 0};
+      if (bd > 0) { const int j0 = a.jadr[bd], nj = a.jnum[bd];
+        if (nj == 1 && a.jtype[j0] == 0) { const double* qp = qpos + a.jq[j0];      // free joint: pose straight from qpos (normalised copy)
+          for (int c = 0; c < 3; c++) pos[c] = qp[c];
+          for (int c = 0; c < 4; c++) quat[c] = qp[3+c];
+          quat_norm(quat);
+        } else { const double* pp = P + 7*a.parent[bd]; double R[9], v[3]; quat2mat(R, pp + 3); mat_vec(v, R, a.bpos + 3*bd);
+          for (int c = 0; c < 3; c++) pos[c] = pp[c] + v[c];
+          quat_mul(quat, pp + 3, a.bquat + 4*bd);
+          for (int j = j0; j < j0 + nj; j++) { const int t = a.jtype[j]; if (t != 2 && t != 3) continue;      // slide, hinge
+            const double* al = a.jaxis + 3*j; double ax[3], anc[3]; quat2mat(R, quat); mat_vec(ax, R, al); mat_vec(v, R, a.jpos + 3*j);
+            for (int c = 0; c < 3; c++) anc[c] = pos[c] + v[c];
+            const double dq = qpos[a.jq[j]] - a.qpos0[a.jq[j]];
+            if (t == 2) { for (int c = 0; c < 3; c++) pos[c] += ax[c]*dq; }
+            else { double s, co, qn[4]; sincos(0.5*dq, &s, &co); const double ql[4] = {co, al[0]*s, al[1]*s, al[2]*s}; quat_mul(qn, quat, ql);
+              for (int c = 0; c < 4; c++) quat[c] = qn[c];
+              quat2mat(R, quat); mat_vec(v, R, a.jpos + 3*j); for (int c = 0; c < 3; c++) pos[c] = anc[c] - v[c]; } } }
+        quat_norm(quat); }
+      double* o = P + 7*bd; for (int c = 0; c < 3; c++) o[c] = pos[c]; for (int c = 0; c < 4; c++) o[3+c] = quat[c]; }
+    __syncwarp(); }
+}
+
+// world position of local point `loc` on body bd of the pose table P
+__device__ __forceinline__ void data_point(const double* P, int bd, const double* loc, double* out) {
+  double R[9]; quat2mat(R, P + 7*bd + 3); mat_vec(out, R, loc); for (int c = 0; c < 3; c++) out[c] += P[7*bd + c]; }
+
+__device__ void data_poses(const DevModel& m, const DataArgs& a, int env, int lane) {
+  const myo_data_buffers& d = a.d; const int nb = a.nbody;
+  double* P = a.pose_buf + (size_t)env*2*nb*7; double* Pt = P + nb*7;
+  data_kinematics(a, a.b.qpos + (size_t)env*m.nq, P, lane);
+  for (int k = lane; k < nb; k += 32) { const double* p = P + 7*k;
+    if (d.xpos) for (int c = 0; c < 3; c++) d.xpos[((size_t)env*nb + k)*3 + c] = p[c];
+    if (d.xquat) for (int c = 0; c < 4; c++) d.xquat[((size_t)env*nb + k)*4 + c] = p[3+c];
+    if (d.xmat) { double R[9]; quat2mat(R, p + 3); for (int c = 0; c < 9; c++) d.xmat[((size_t)env*nb + k)*9 + c] = R[c]; } }
+  if (!d.site_xpos) return;
+  const int32_t* src = d.site_source; bool at_target = false;      // a site placed from the kinematics of the target pose
+  if (src && a.b.target) for (int s = lane; s < a.nsite; s += 32) at_target |= src[2*s] == 3;
+  if (__any_sync(FULL, at_target)) data_kinematics(a, a.b.target + (size_t)env*m.nq, Pt, lane);
+  for (int s = lane; s < a.nsite; s += 32) { const int kind = src ? src[2*s] : 0, ix = src ? src[2*s+1] : 0; double loc[3], out[3];
+    for (int c = 0; c < 3; c++) loc[c] = a.site_pos[3*s + c];
+    if (kind == 1 && a.b.target) { for (int c = 0; c < 3; c++) loc[c] = a.b.target[(size_t)env*m.nq + ix + c]; }
+    else if (kind == 2 && a.b.env_prm) { for (int c = 0; c < 3; c++) loc[c] = a.b.env_prm[(size_t)env*8 + ix + c]; }
+    else if (kind == 3 && a.b.target) data_point(Pt, a.site_body[ix], a.site_pos + 3*ix, loc);
+    data_point(P, a.site_body[s], loc, out);
+    for (int c = 0; c < 3; c++) d.site_xpos[((size_t)env*a.nsite + s)*3 + c] = out[c]; }
+  __syncwarp();
+}
+
+// contact list after constraint assembly (the contact records die in the solve), in model pair order
+__device__ void data_contacts(const DevModel& m, const Warp w, const DataArgs& a, int env) {
+  const myo_data_buffers& d = a.d; const int ncon = WI_(ncon); const size_t r0 = (size_t)env*m.maxcon;
+  for (int c = w.lane; c < m.maxcon; c += 32) { if (c < ncon) continue; const size_t r = r0 + c;
+    if (d.contact_geom) { d.contact_geom[2*r] = -1; d.contact_geom[2*r+1] = -1; }
+    if (d.contact_dist) d.contact_dist[r] = 0;
+    if (d.contact_pos) for (int k = 0; k < 3; k++) d.contact_pos[3*r+k] = 0;
+    if (d.contact_frame) for (int k = 0; k < 9; k++) d.contact_frame[9*r+k] = 0; }
+  for (int c = w.lane; c < ncon; c += 32) { const size_t r = r0 + CRANK(S_crown[c]); const int p = S_cpair[c]; const double* cd = S_con + c*CON_STRIDE;
+    if (d.contact_geom) { d.contact_geom[2*r] = a.pair_geom[2*p]; d.contact_geom[2*r+1] = a.pair_geom[2*p+1]; }
+    if (d.contact_dist) d.contact_dist[r] = cd[0];
+    if (d.contact_pos) for (int k = 0; k < 3; k++) d.contact_pos[3*r+k] = cd[1+k];
+    if (d.contact_frame) { double f[9]; for (int k = 0; k < 6; k++) f[k] = cd[4+k]; cross3(f+6, f, f+3); for (int k = 0; k < 9; k++) d.contact_frame[9*r+k] = f[k]; } }
+  __syncwarp();
+}
+
+// after the Newton solve: qacc, ncon and mj_contactForce of every contact (the forces of its rows, -D jar where jar < 0, decoded from the pyramid)
+__device__ void data_solve(const DevModel& m, const Warp w, const DataArgs& a, int env) {
+  const myo_data_buffers& d = a.d; const int ncon = WI_(ncon); const size_t r0 = (size_t)env*m.maxcon;
+  if (d.qacc) for (int i = w.lane; i < m.nv; i += 32) d.qacc[(size_t)env*m.nv + i] = S_a[i];
+  if (d.ncon && w.lane == 0) d.ncon[env] = ncon;
+  if (d.contact_force) {
+    for (int c = w.lane; c < m.maxcon; c += 32) if (c >= ncon) for (int k = 0; k < 6; k++) d.contact_force[6*(r0 + c) + k] = 0;
+    const idx_t* pr = CI(PPAIR); const double* pd = CD(PPAIR_d);
+    for (int c = w.lane; c < ncon; c += 32) { const int rn = S_crown[c], nr = CNR(rn), rb = CROW(rn); double f[6] = {0, 0, 0, 0, 0, 0};
+      if (nr) { const double Dc = S_D[S_DCON(c)]; double q[4] = {0, 0, 0, 0};
+        for (int k = 0; k < nr; k++) { const double x = S_jar[rb + k]; q[k] = x < 0 ? -Dc*x : 0.0; }
+        if (nr == 1) f[0] = q[0];
+        else { const double* P = pd + pr[PPAIR_ISTRIDE*S_cpair[c] + 6]*PPAIR_STRIDE; f[0] = q[0] + q[1] + q[2] + q[3]; f[1] = (q[0] - q[1])*P[2]; f[2] = (q[2] - q[3])*P[3]; } }
+      for (int k = 0; k < 6; k++) d.contact_force[6*(r0 + CRANK(rn)) + k] = f[k]; } }
+  __syncwarp();
+}
+
+extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DataArgs a) {
+  __shared__ __align__(8) unsigned long long mbar;
+  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  if (a.depth != DATA_NONE) stage_model(m, mbar);
+  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  const myo_data_buffers& d = a.d; const myo_buffers& b = a.b;
+  const int per_cta = (a.n_env + (int)gridDim.x - 1)/(int)gridDim.x;
+  for (int j = wid; j < per_cta; j += nw) {
+    const int env = (int)blockIdx.x + (int)gridDim.x*j;
+    if (env >= a.n_env) break;
+    if (a.pose) data_poses(m, a, env, w.lane);
+    if (a.depth == DATA_NONE) continue;
+    // ---- the stored state into this warp's slice, as the step kernels load it
+    if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
+    for (int i = w.lane; i < m.nq; i += 32) W_(qpos)[i] = b.qpos[(size_t)env*m.nq+i];
+    for (int i = w.lane; i < m.nv; i += 32) { W_(qvel)[i] = b.qvel[(size_t)env*m.nv+i]; W_(qws)[i] = b.qacc_warmstart[(size_t)env*m.nv+i]; }
+    for (int i = w.lane; i < m.na; i += 32) W_(act)[i] = b.act[(size_t)env*m.na+i];
+    if (w.lane < m.neprm) W_(eprm)[w.lane] = b.env_prm ? b.env_prm[(size_t)env*8 + w.lane] : 0.0;
+    for (int i = w.lane; i < m.nwz; i += 32) W_(wz)[i] = -1.0;
+    __syncwarp();
+    phase_kinematics(m, w); phase_tendon_all(m, w);
+    phase_actuation(m, w, false, m.g_ctrl + (size_t)env*m.nu, d.actuator_force ? d.actuator_force + (size_t)env*m.nu : nullptr,
+                    d.actuator_length ? d.actuator_length + (size_t)env*m.nu : nullptr);
+    if (d.actuator_velocity) { const idx_t* at = CI(PA_tendon); const double* __restrict__ PAm = GD(PAM_d); const double* tvel = SCR(s_tvel);
+      for (int i = w.lane; i < m.nu; i += 32) d.actuator_velocity[(size_t)env*m.nu + i] = LDC(PAm + i*PAM_STRIDE + 4)*tvel[at[i]]; }
+    if (d.qfrc_actuator) { const idx_t* cadr = CI(PCOL_adr); const idx_t* col = CI(PCOL); const idx_t* nzt = CI(PNZ_tendon); const double* mom = SCR(s_mom); const double* tfrc = SCR(s_tfrc);
+      for (int i = w.lane; i < m.nv; i += 32) { double s = 0; for (int e = cadr[i]; e < cadr[i+1]; e++) { const int z = col[e]; s += mom[z]*tfrc[nzt[z]]; }
+        d.qfrc_actuator[(size_t)env*m.nv + i] = s; } }
+    __syncwarp();
+    if (a.depth < DATA_DYN) continue;
+    phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w);
+    phase_collision(m, w); phase_constraints(m, w);
+    data_contacts(m, w, a, env);
+    phase_solve(m, w, a.tol, nullptr, true, false);
+    data_solve(m, w, a, env);
+  }
+}
+
 // ================================================================== host side (C-ABI)
 static thread_local std::string g_err;
 static int fail(const std::string& s) { g_err = s; return -1; }
@@ -422,7 +579,9 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
 }
 
 struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
-  int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset; };
+  int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
+  // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
+  int32_t* dRI; double* dRD; double* dPose; DataArgs data; int data_warps, data_grid, data_smem; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -603,7 +762,8 @@ extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const
     n_env, b->use_w14 ? "launch_bounds(448)" : "launch_bounds(320)", b->warps_per_cta, b->grid, b->smem_bytes, b->const_bytes, per, fit, b->dbg_warps, b->dbg_grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
   *out = b; return 0;
 }
-extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); if (b->dLoad) cudaFree(b->dLoad); if (b->dPerm) cudaFree(b->dPerm); delete b; }
+extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); if (b->dLoad) cudaFree(b->dLoad); if (b->dPerm) cudaFree(b->dPerm);
+  if (b->dRI) cudaFree(b->dRI); if (b->dRD) cudaFree(b->dRD); if (b->dPose) cudaFree(b->dPose); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
 // Launch shape of the product kernels' env steps, as launch() and env_kernel_body compute it.  Fields (first min(n, 8) written):
@@ -698,4 +858,63 @@ extern "C" int myo_batch_observe(myo_batch* b, void* stream) {
 extern "C" int myo_batch_forward_debug(myo_batch* b, const double* ctrl, int n_substeps, void* stream) {
   if (!b || !ctrl) return fail("myo_batch_forward_debug: null");
   StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 1; a.dbg_ctrl = ctrl; a.n_substeps = n_substeps; return launch(b, a, stream);
+}
+
+// First readout of a batch: the model tables of mj_kinematics (every body, in tree-level order), the sites and the geoms of every program
+// pair go to HBM; the pose scratch is allocated; the launch shape of myo_data_kernel follows from its own register and thread limits.
+static int data_setup(myo_batch* b) {
+  const int32_t* I = b->model->I.data(); const double* D = b->model->D.data(); DataArgs& a = b->data;
+  const int nb = MYO_DIM(I, MYO_DIM_nbody), nj = MYO_DIM(I, MYO_DIM_njnt), ns = MYO_DIM(I, MYO_DIM_nsite), nq = MYO_DIM(I, MYO_DIM_nq), np = b->dm.npair;
+  const int32_t* parent = MYO_ISEC(I, MYO_SEC_body_parentid); const int32_t* ppair = MYO_ISEC(I, MYO_SEC_PPAIR);
+  std::vector<int> depth(nb, 0); int nlevel = 1;
+  for (int k = 1; k < nb; k++) { depth[k] = depth[parent[k]] + 1; nlevel = imax(nlevel, depth[k] + 1); }      // (parents precede children)
+  std::vector<int32_t> ri(nlevel + 1, 0);
+  for (int k = 0; k < nb; k++) ri[depth[k] + 1]++;
+  for (int L = 0; L < nlevel; L++) ri[L + 1] += ri[L];
+  for (int L = 0; L < nlevel; L++) for (int k = 0; k < nb; k++) if (depth[k] == L) ri.push_back(k);
+  size_t o_parent = ri.size(); ri.insert(ri.end(), parent, parent + nb);
+  size_t o_jadr = ri.size(); ri.insert(ri.end(), MYO_ISEC(I, MYO_SEC_body_jntadr), MYO_ISEC(I, MYO_SEC_body_jntadr) + nb);
+  size_t o_jnum = ri.size(); ri.insert(ri.end(), MYO_ISEC(I, MYO_SEC_body_jntnum), MYO_ISEC(I, MYO_SEC_body_jntnum) + nb);
+  size_t o_jtype = ri.size(); ri.insert(ri.end(), MYO_ISEC(I, MYO_SEC_jnt_type), MYO_ISEC(I, MYO_SEC_jnt_type) + nj);
+  size_t o_jq = ri.size(); ri.insert(ri.end(), MYO_ISEC(I, MYO_SEC_jnt_qposadr), MYO_ISEC(I, MYO_SEC_jnt_qposadr) + nj);
+  size_t o_sb = ri.size(); ri.insert(ri.end(), MYO_ISEC(I, MYO_SEC_site_bodyid), MYO_ISEC(I, MYO_SEC_site_bodyid) + ns);
+  size_t o_pg = ri.size();
+  for (int p = 0; p < np; p++) { const int mp = ppair[PPAIR_ISTRIDE*p + 7]; ri.push_back(MYO_ISEC(I, MYO_SEC_pair_geom1)[mp]); ri.push_back(MYO_ISEC(I, MYO_SEC_pair_geom2)[mp]); }
+  std::vector<double> rd;
+  const int sec[6] = {MYO_SEC_body_pos, MYO_SEC_body_quat, MYO_SEC_jnt_pos, MYO_SEC_jnt_axis, MYO_SEC_qpos0, MYO_SEC_site_pos};
+  const int len[6] = {3*nb, 4*nb, 3*nj, 3*nj, nq, 3*ns}; size_t od[6];
+  for (int s = 0; s < 6; s++) { if (MYO_SEC_LEN(I, sec[s]) != len[s]) return fail("myo_batch_data: model blob section of unexpected size");
+    od[s] = rd.size(); rd.insert(rd.end(), MYO_DSEC(I, D, sec[s]), MYO_DSEC(I, D, sec[s]) + len[s]); }
+  CUDA_OK(cudaMalloc(&b->dRI, ri.size()*4)); CUDA_OK(cudaMemcpy(b->dRI, ri.data(), ri.size()*4, cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMalloc(&b->dRD, imax((int)rd.size(), 1)*8)); CUDA_OK(cudaMemcpy(b->dRD, rd.data(), rd.size()*8, cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMalloc(&b->dPose, (size_t)b->n_env*2*nb*7*8));
+  a.nbody = nb; a.nsite = ns; a.nlevel = nlevel; a.lvl = b->dRI; a.parent = b->dRI + o_parent; a.jadr = b->dRI + o_jadr; a.jnum = b->dRI + o_jnum;
+  a.jtype = b->dRI + o_jtype; a.jq = b->dRI + o_jq; a.site_body = b->dRI + o_sb; a.pair_geom = b->dRI + o_pg;
+  a.bpos = b->dRD + od[0]; a.bquat = b->dRD + od[1]; a.jpos = b->dRD + od[2]; a.jaxis = b->dRD + od[3]; a.qpos0 = b->dRD + od[4]; a.site_pos = b->dRD + od[5];
+  a.pose_buf = b->dPose; a.n_env = b->n_env; a.tol = b->cfg.solver_tolerance > 0 ? b->cfg.solver_tolerance : 1e-10;
+  // launch shape: as many env-warps per CTA as the kernel's thread limit and shared memory allow, balanced env -> CTA map
+  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+  cudaFuncAttributes fa; CUDA_OK(cudaFuncGetAttributes(&fa, myo_data_kernel));
+  const int per = b->dm.n_per_warp*8, fit = ((int)prop.sharedMemPerBlockOptin - b->const_bytes - 64)/per;
+  int wpc = fa.maxThreadsPerBlock/32; if (wpc > fit) wpc = fit; if (wpc > b->n_env) wpc = b->n_env;
+  if (wpc < 1) return fail("myo_batch_data: model working set exceeds shared memory of one CTA");
+  b->data_warps = wpc; b->data_smem = b->const_bytes + wpc*per;
+  CUDA_OK(cudaFuncSetAttribute(myo_data_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, b->data_smem));
+  int c = 1; CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_data_kernel, wpc*32, b->data_smem)); if (c < 1) c = 1;
+  const int need = (b->n_env + wpc - 1)/wpc; b->data_grid = need < prop.multiProcessorCount*c ? need : prop.multiProcessorCount*c;
+  return 0;
+}
+
+extern "C" int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream) {
+  if (!b || !d) return fail("myo_batch_data: null");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  const bool pose = d->xpos || d->xquat || d->xmat || d->site_xpos;
+  const bool act = d->actuator_length || d->actuator_velocity || d->actuator_force || d->qfrc_actuator;
+  const bool dyn = d->qacc || d->ncon || d->contact_geom || d->contact_dist || d->contact_pos || d->contact_frame || d->contact_force;
+  if (!pose && !act && !dyn) return 0;
+  CUDA_OK(cudaSetDevice(b->device));
+  if (!b->dRI) { const int rc = data_setup(b); if (rc) return rc; }
+  DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE);
+  myo_data_kernel<<<b->data_grid, b->data_warps*32, a.depth == DATA_NONE ? 0 : b->data_smem, (cudaStream_t)stream>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

@@ -292,6 +292,24 @@ def _target_range(c, m, kw):
     return tr
 
 
+def site_sources(task, m, kw, tip_names):
+    """int32 [nsite, 2] (kind, index) of the sites whose model site_pos the reference moves per episode (abi.SITE_* kinds, the
+    myo_data_buffers.site_source of the mjData readout), or None when the task moves none:
+      reach / stand  <tip>_target = the target row's 3 values of that tip (reach_v0.py:163-170, walk_v0.py:142-150)
+      hold           goal = env_prm[0:3] (obj_hold_v0.py:126-145)
+      pose           <tip>_target of every viz_site_targets tip = the tip site at the kinematics of the target pose (pose_v0.py:154-170)"""
+    src = np.zeros((m.nsite, 2), dtype=np.int32)
+    if task in ("reach", "stand"):
+        for k, name in enumerate(tip_names):
+            src[m.name2id("site", name + "_target")] = (abi.SITE_TARGET, 3 * k)
+    elif task == "hold":
+        src[m.name2id("site", "goal")] = (abi.SITE_ENV_PRM, 0)
+    elif task == "pose":
+        for name in kw.get("viz_site_targets") or ():
+            src[m.name2id("site", name + "_target")] = (abi.SITE_AT_TARGET_POSE, m.name2id("site", name))
+    return src if np.any(src[:, 0]) else None
+
+
 def configure(entry, m, prog_info, kw, max_episode_steps=0, auto_reset=True):
     """Everything a batch of `entry` (a reference entry point, None for physics only) needs besides the device, from the model `m`, its
     program info (program.build_program) and the env kwargs.  Returns a namespace with

@@ -152,6 +152,10 @@ class MyoVecEnv:
             t["obs"] = z(n, self.obs_dim, dtype=f32)
             t["final_obs"] = torch.full((n, self.obs_dim), float("nan"), dtype=f32, device=dv)
         self._h_action = None
+        # mjData readout (data()): buffers allocated on first request; site_source places the sites the task moves per episode
+        self._data, self.state_version = {}, 0
+        src = tasks.site_sources(self.task, m, kw, self.tip_names)
+        self._site_source = None if src is None else torch.as_tensor(src, device=dv).contiguous()
 
     def _sync_obs(self):
         if self._obs_cols is not None:
@@ -202,6 +206,7 @@ class MyoVecEnv:
             else:
                 self.t["episode_count"][mask.bool()] = 0
         self._reset_mask = mask          # keep alive until the launch has consumed it
+        self.state_version += 1
         self.batch.reset(mask=mask, seed=self.seed_value, env_offset=self.env_offset, stream=self._stream())
         self._sync_obs()
         return self.t["obs"], {}
@@ -222,6 +227,7 @@ class MyoVecEnv:
                 raise ValueError("action must have shape %s, got %s" % (tuple(a.shape), tuple(action.shape)))
             a.copy_(action, non_blocking=True)
         self.batch.step(stream=self._stream())
+        self.state_version += 1
         self._sync_obs()
         t = self.t
         if self._obs_cols is not None:
@@ -234,6 +240,7 @@ class MyoVecEnv:
         torch = self.torch
         self.t["action"].copy_(action_cpu_pinned, non_blocking=True)
         self.batch.step(stream=self._stream())
+        self.state_version += 1
         self._sync_obs()
         if self._h_action is None:
             self._h_reward = torch.empty(self.num_envs, dtype=torch.float32, pin_memory=True)
@@ -253,6 +260,7 @@ class MyoVecEnv:
             if v is not None:
                 self.t[name][:, : np.shape(v)[-1]] = torch.as_tensor(np.asarray(v), dtype=torch.float64, device=self.device)
         self.t["qacc_warmstart"].zero_()
+        self.state_version += 1
 
     STATE_KEYS = ("time", "qpos", "qvel", "act", "qacc_warmstart", "target", "step_count", "episode_count", "ep_return", "fatigue", "env_prm")
 
@@ -293,8 +301,36 @@ class MyoVecEnv:
     def refresh_obs(self):
         """obs / reward / done of the current state (the reference's env.forward(), env_base.py:393-432)."""
         self.batch.observe(stream=self._stream())
+        self.state_version += 1
         self._sync_obs()
         return self.t["obs"], self.t["reward"], self.t["done"]
+
+    DATA_FIELDS = tuple(k for k in abi.DATA_FIELDS if k != "site_source")
+
+    def data(self, *fields):
+        """mjData of every env after mj_forward at its current state (the reference's env.unwrapped.mj_data after reset() / step()):
+        {field: tensor [num_envs, ...]} for the requested fields of DATA_FIELDS (all when none is named), in MuJoCo ids and order.
+        One launch computes only what the deepest requested group needs (pose < actuation < dynamics; myo_batch_data).  The tensors
+        are allocated on first request (NaN / -1 until first written) and reused: a result is valid until the next state change.
+        ctrl is the last step's ctrl (zeros before the first step); after an auto-reset the values describe the new episode's state."""
+        torch = self.torch
+        fields = tuple(fields) or self.DATA_FIELDS
+        bad = [f for f in fields if f not in self.DATA_FIELDS]
+        if bad:
+            raise KeyError("unknown mjData fields %s (available: %s)" % (bad, list(self.DATA_FIELDS)))
+        m, n = self.mj_model, self.num_envs
+        size = dict(nbody=m.nbody, nsite=m.nsite, nu=m.nu, nv=m.nv, maxcon=self.dims.maxcon)
+        for f in fields:
+            if f not in self._data:
+                _, dt, shape = abi.DATA_SHAPES[f]
+                shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in shape)
+                self._data[f] = (torch.full(shape, float("nan"), dtype=torch.float64, device=self.device) if dt == "f64"
+                                 else torch.full(shape, -1, dtype=torch.int32, device=self.device))
+        bufs = {f: self._data[f] for f in fields}
+        if "site_xpos" in bufs:
+            bufs["site_source"] = self._site_source
+        self.batch.data(stream=self._stream(), **bufs)
+        return {f: self._data[f] for f in fields}
 
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
@@ -306,22 +342,78 @@ class MyoVecEnv:
         c = self.torch.as_tensor(np.asarray(ctrl), dtype=self.torch.float64, device=self.device).contiguous()
         self._dbg_ctrl = c
         self.batch.forward_debug(c, n_substeps, stream=self._stream())
+        self.state_version += 1
+
+
+class _Named:
+    """One named element of mj_data, as MuJoCo's data.body(name) / site / actuator / joint accessors return it."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def __repr__(self):
+        return "<%s>" % ", ".join("%s=%r" % kv for kv in self.__dict__.items())
 
 
 class _DataView:
-    """`env.mj_data`-like read access to the single env's state (numpy copies of the device rows)."""
+    """`env.mj_data`-like read access to the single env: qpos, qvel, act, time and every field of the mjData readout (MyoVecEnv.data)
+    as numpy arrays, with MuJoCo's named views body(name), site(name), actuator(name), joint(name) and the contact list.  Lazy: the
+    first access after a state change runs one readout launch and one device-to-host copy; later accesses read the host copy."""
 
     def __init__(self, vec):
-        self._vec = vec
+        self._vec, self._version, self._d = vec, None, None
 
-    def _row(self, k):
-        self._vec.torch.cuda.current_stream(self._vec.device).synchronize()
-        return self._vec.t[k][0].detach().cpu().numpy().copy()
+    def _fetch(self):
+        v = self._vec
+        if self._version != v.state_version:
+            m = v.mj_model
+            out = v.data()
+            parts = [("qpos", v.t["qpos"][0]), ("qvel", v.t["qvel"][0]), ("act", v.t["act"][0, :m.na]), ("time", v.t["time"][:1])]
+            parts += [(f, out[f][0]) for f in v.DATA_FIELDS]
+            flat = v.torch.cat([x.reshape(-1).double() for _, x in parts]).cpu().numpy()
+            d, o = {}, 0
+            for k, x in parts:
+                a = flat[o:o + x.numel()].reshape(tuple(x.shape)); o += x.numel()
+                d[k] = a.astype(np.int32) if x.dtype == v.torch.int32 else a
+            d["time"], d["ncon"] = float(d["time"][0]), int(d["ncon"])
+            self._d, self._version = d, v.state_version
+        return self._d
 
-    qpos = property(lambda self: self._row("qpos"))
-    qvel = property(lambda self: self._row("qvel"))
-    act = property(lambda self: self._row("act")[: self._vec.mj_model.na])
-    time = property(lambda self: float(self._row("time")))
+    def __getattr__(self, k):
+        if k.startswith("_") or k not in ("qpos", "qvel", "act", "time") + self._vec.DATA_FIELDS:
+            raise AttributeError(k)
+        x = self._fetch()[k]
+        return x.copy() if isinstance(x, np.ndarray) else x
+
+    def _id(self, kind, key):
+        return int(key) if isinstance(key, (int, np.integer)) else self._vec.mj_model.name2id(kind, key)
+
+    def body(self, key):
+        i, d = self._id("body", key), self._fetch()
+        return _Named(id=i, xpos=d["xpos"][i].copy(), xquat=d["xquat"][i].copy(), xmat=d["xmat"][i].copy())
+
+    def site(self, key):
+        i = self._id("site", key)
+        return _Named(id=i, xpos=self._fetch()["site_xpos"][i].copy())
+
+    def actuator(self, key):
+        i, d = self._id("actuator", key), self._fetch()
+        return _Named(id=i, length=d["actuator_length"][i:i + 1].copy(), velocity=d["actuator_velocity"][i:i + 1].copy(), force=d["actuator_force"][i:i + 1].copy())
+
+    def joint(self, key):
+        from . import mjcf
+        m, d = self._vec.mj_model, self._fetch()
+        i = self._id("joint", key); t = int(m.jnt_type[i])
+        nq_, nv_ = {mjcf.JNT_FREE: (7, 6), mjcf.JNT_BALL: (4, 3)}.get(t, (1, 1))
+        q, dv = int(m.jnt_qposadr[i]), int(m.jnt_dofadr[i])
+        return _Named(id=i, qpos=d["qpos"][q:q + nq_].copy(), qvel=d["qvel"][dv:dv + nv_].copy(), qacc=d["qacc"][dv:dv + nv_].copy())
+
+    @property
+    def contact(self):
+        """The first ncon contacts (geom1, geom2, dist, pos, frame; arrays over the contacts, like MuJoCo's data.contact)."""
+        d = self._fetch(); n = d["ncon"]
+        return _Named(geom1=d["contact_geom"][:n, 0].copy(), geom2=d["contact_geom"][:n, 1].copy(), dist=d["contact_dist"][:n].copy(),
+                      pos=d["contact_pos"][:n].copy(), frame=d["contact_frame"][:n].copy())
 
 
 class MyoEnv:
