@@ -158,17 +158,19 @@ void myo_model_destroy(myo_model* m);
 /* Shared-memory layout of one env's slice, as the step kernels of a batch created with this model and cfg use it (host only: needs no
  * device).  Writes the first min(cap, MYO_LAYOUT_N) of these int32 values; offsets and sizes are in doubles, offsets from the start of
  * the slice:
- *   [0, 12)   persistent offsets  qpos qvel act qws dax dan qM fsm eprm wz cnt scr   (scr: start of the stage scratch; qws lies inside
- *             the scratch, in the tail of the Hessian region, when the qwsInH flag below is set)
+ *   [0, 12)   persistent offsets, in MYO_LAYOUT_PERSISTENT order (scr: start of the stage scratch; qws lies inside the scratch, in the
+ *             tail of the Hessian region, when the qwsInH flag below is set)
  *   [12, 24)  their reserved sizes, same order (scr: size of the scratch)
- *   [24, 54)  scratch offsets  xpos xmat U PL mom tlen tvel tfrc cin crb bf conJ efD efA eqJ icon con clist gpose efR efV va vg vp vMa vMp
- *             H Hs LD Dinv
+ *   [24, 54)  scratch offsets, in MYO_LAYOUT_SCRATCH order
  *   [54, 84)  their reserved sizes, same order (aliases share storage: con / efR / efV, vg / vp, H / Hs, and efA / H when arefInH)
  *   84 head: end of the contact head (icon records, then contact records)     85 afterK: end of the body poses xpos / xmat behind it
  *   86 extNonSolve: end of the scratch the stages before the constraints use  87 end of the solve stage's regions (the Hessian region)
  *   88 arefInH: aref lives at the head of the Hessian region                  89 qwsInH: the warm start lives in its tail
  *   90 n_per_warp (doubles per env slice)    91 maxcon (cfg's, or 32 when 0, clamped to min(64, 2 npair))    92 maxefc */
 #define MYO_LAYOUT_N 93
+#define MYO_LAYOUT_PERSISTENT(X) X(qpos) X(qvel) X(act) X(qws) X(dax) X(dan) X(qM) X(fsm) X(eprm) X(wz) X(cnt) X(scr)
+#define MYO_LAYOUT_SCRATCH(X) X(xpos) X(xmat) X(U) X(PL) X(mom) X(tlen) X(tvel) X(tfrc) X(cin) X(crb) X(bf) X(conJ) X(efD) X(efA) X(eqJ) \
+  X(icon) X(con) X(clist) X(gpose) X(efR) X(efV) X(va) X(vg) X(vp) X(vMa) X(vMp) X(H) X(Hs) X(LD) X(Dinv)
 int myo_model_layout(const myo_model* m, const myo_task_cfg* cfg_or_null, int32_t* out, int cap);
 
 /* Batch of n_env envs of one model on one device. */

@@ -16,7 +16,7 @@ struct StepArgs {
   myo_buffers b; myo_task_cfg cfg;
   int n_env, obs_dim, mode;     // mode 0: env step ; 1: debug forward (ctrl verbatim, optional substeps) ; 2: reset only
   int n_substeps;               // mode 1
-  int balanced;                 // env -> CTA map: 1 = e % grid (equal env counts per CTA, big models), 0 = contiguous groups of warps (small models: neighbouring rows share cache lines)
+  int balanced;                 // slot -> env map without perm (slot_env): 1 = e % grid (big models), 0 = contiguous groups of warps (small models)
   const double* dbg_ctrl;       // mode 1
   const uint8_t* reset_mask;    // mode 2 (nullable)
   int* load;                    // mode 0, product kernels (nullable): per-env load key written at the end of the step (mean contacts + Newton iterations per substep)
@@ -27,6 +27,14 @@ struct StepArgs {
   double tol, dt;
 };
 static const int LOAD_WN = 2, LOAD_WI = 3;      // the load key's weights (StepArgs.load_wn / load_wi) for the product kernels' env steps
+
+// Slot -> env map without load sorting (slot j0 + wid of a CTA: warp wid of the round starting at j0).  Balanced: env e on CTA e % grid, so
+// no CTA runs a full extra round while the others idle (4096 envs on 132 SMs at 11 warps: rounds of 11, 11, 9 or 10 everywhere instead of
+// 11, 11, 11 on four fifths of the SMs).  Contiguous: each round of a CTA takes nw consecutive envs (neighbouring rows share cache lines).
+// SLOTS_PER_CTA is a macro so that the step kernels read gridDim.x inside each branch: as a function argument the read moves ahead of the
+// branch and their register allocation changes.
+#define SLOTS_PER_CTA(balanced, n_env, grid, nw) ((balanced) ? ((n_env) + (grid) - 1)/(grid) : (((n_env) + (nw) - 1)/(nw) + (grid) - 1)/(grid)*(nw))
+__host__ __device__ __forceinline__ int slot_env(int balanced, int cta, int grid, int nw, int j0, int wid) { return balanced ? cta + grid*(j0 + wid) : (cta + grid*(j0/nw))*nw + wid; }
 
 // ------------------------------------------------------------------ Philox4x32-10 (counter-based RNG, one stream per (seed, env, episode))
 struct Philox { uint32_t c0, c1, c2, c3, k0, k1, o0, o1, o2, o3; int have; };   // scalars only: indexed arrays would live in local memory
@@ -241,6 +249,38 @@ __device__ __noinline__ RwDone task_observe(const DevModel& m, const Warp w, con
 __device__ __forceinline__ void group_sync(int ngroups, int gid, int gthreads) {
   if (ngroups <= 1) __syncthreads(); else asm volatile("bar.sync %0, %1;" :: "r"(1 + gid), "r"(gthreads) : "memory"); }
 
+// The model constants into shared memory: bulk async copies (TMA), completion on an mbarrier.  Every thread of the CTA runs it.  A macro,
+// not a function: one more call site in env_kernel_body changes the order in which its callees are inlined, and with it the step
+// kernels' stack layout and machine code.
+#define STAGE_MODEL(m, mbar) { \
+  double* s_d = smem; idx_t* s_i = (idx_t*)(smem + m.nD); \
+  const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar); \
+  if (threadIdx.x == 0) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb)); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); } \
+  __syncthreads(); \
+  if (threadIdx.x == 0) { \
+    const unsigned bytes_d = (unsigned)m.nD*8u, bytes_i = (unsigned)m.nI16w*4u; \
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes_d + bytes_i) : "memory"); \
+    const unsigned CH = 32768u;   /* chunked: every piece 16-byte aligned and a multiple of 16 bytes */ \
+    for (unsigned o = 0; o < bytes_d; o += CH) { unsigned n = bytes_d - o < CH ? bytes_d - o : CH; \
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" \
+                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_d + o)), "l"((const char*)m.gD + o), "r"(n), "r"(mb) : "memory"); } \
+    for (unsigned o = 0; o < bytes_i; o += CH) { unsigned n = bytes_i - o < CH ? bytes_i - o : CH; \
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" \
+                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_i + o)), "l"((const char*)m.gI16 + o), "r"(n), "r"(mb) : "memory"); } \
+  } \
+  { unsigned done = 0; while (!done) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(mb) : "memory"); } \
+}
+
+// The stored state of `env` into this warp's slice (coalesced: one env's row per warp).  The inverse-wrap roots start cold.
+__device__ __forceinline__ void load_env_state(const DevModel& m, const Warp w, const myo_buffers& b, int env) {
+  for (int i = w.lane; i < m.nq; i += 32) W_(qpos)[i] = b.qpos[(size_t)env*m.nq+i];
+  for (int i = w.lane; i < m.nv; i += 32) { W_(qvel)[i] = b.qvel[(size_t)env*m.nv+i]; W_(qws)[i] = b.qacc_warmstart[(size_t)env*m.nv+i]; }
+  for (int i = w.lane; i < m.na; i += 32) W_(act)[i] = b.act[(size_t)env*m.na+i];
+  if (w.lane < m.neprm) W_(eprm)[w.lane] = b.env_prm ? b.env_prm[(size_t)env*8 + w.lane] : 0.0;     // per-env model overrides (hold task only)
+  for (int i = w.lane; i < m.nwz; i += 32) W_(wz)[i] = -1.0;     // cold start of the inverse-wrap roots at the first substep
+  __syncwarp();
+}
+
 // ------------------------------------------------------------------ the kernel
 // DBG = false: the product step / reset / observe kernel (modes 0, 2, 3): no parity taps, no cycle counters, fixed barrier scheme.
 // DBG = true: everything -- forward-debug mode (1), parity taps, per-phase cycle counters, the barrier / lockstep-group tuning knobs.
@@ -249,24 +289,7 @@ template <bool DBG, int MAXT>
 __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArgs& a) {
   __shared__ __align__(8) unsigned long long mbar;
   const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  // ---- stage the model constants into shared memory: bulk async copies (TMA), completion on an mbarrier
-  double* s_d = smem; idx_t* s_i = (idx_t*)(smem + m.nD);
-  const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-  if (threadIdx.x == 0) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb)); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned bytes_d = (unsigned)m.nD*8u, bytes_i = (unsigned)m.nI16w*4u;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes_d + bytes_i) : "memory");
-    const unsigned CH = 32768u;   // chunked: every piece 16-byte aligned and a multiple of 16 bytes
-    for (unsigned o = 0; o < bytes_d; o += CH) { unsigned n = bytes_d - o < CH ? bytes_d - o : CH;
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_d + o)), "l"((const char*)m.gD + o), "r"(n), "r"(mb) : "memory"); }
-    for (unsigned o = 0; o < bytes_i; o += CH) { unsigned n = bytes_i - o < CH ? bytes_i - o : CH;
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_i + o)), "l"((const char*)m.gI16 + o), "r"(n), "r"(mb) : "memory"); }
-  }
-  { unsigned done = 0; while (!done) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(mb) : "memory"); }
-
+  STAGE_MODEL(m, mbar)
   const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
   if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
   __syncwarp();
@@ -276,23 +299,15 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
   const int nsub = a.mode == 0 ? a.cfg.frame_skip : ((DBG && a.mode == 1) ? (a.n_substeps > 0 ? a.n_substeps : 1) : 0);
   const bool integrate = a.mode == 0 || (DBG && a.mode == 1 && a.n_substeps > 0);
   const bool prof = DBG && b.tap_phase_cycles != nullptr;
-  // env e belongs to CTA e % gridDim.x: every CTA gets floor or ceil of n_env / gridDim.x envs, so no CTA runs a full extra round
-  // while the others idle (4096 envs on 132 SMs at 11 warps: rounds of 11, 11, 9 or 10 everywhere instead of 11, 11, 11 on four fifths of the SMs)
   // With a.perm (big models, env steps of the product kernels) the slot -> env map is the load-sorted one: the envs of a round carry
   // similar contact loads, so the lockstep barriers wait for a slowest env that is close to the average one.
   const bool regrouped = !DBG && a.perm != nullptr;
-  const int per_cta = regrouped ? a.perm_rounds*nw : (a.balanced ? (a.n_env + (int)gridDim.x - 1)/(int)gridDim.x : ((a.n_env + nw - 1)/nw + (int)gridDim.x - 1)/(int)gridDim.x*nw);
+  const int per_cta = regrouped ? a.perm_rounds*nw : SLOTS_PER_CTA(a.balanced, a.n_env, (int)gridDim.x, nw);
   for (int j0 = 0; j0 < per_cta; j0 += nw) {
-    const int env = regrouped ? a.perm[(int)blockIdx.x + (int)gridDim.x*(j0 + wid)] : (a.balanced ? (int)blockIdx.x + (int)gridDim.x*(j0 + wid) : ((int)blockIdx.x + (int)gridDim.x*(j0/nw))*nw + wid);
+    const int env = regrouped ? a.perm[(int)blockIdx.x + (int)gridDim.x*(j0 + wid)] : slot_env(a.balanced, (int)blockIdx.x, (int)gridDim.x, nw, j0, wid);
     const bool live = (j0 + wid) < per_cta && env >= 0 && env < a.n_env; const long long tstep_ = prof ? clock64() : 0; int load_acc = 0;
     if (live) {
-      // ---- load state (coalesced: one env's row per warp)
-      for (int i = w.lane; i < m.nq; i += 32) W_(qpos)[i] = b.qpos[(size_t)env*m.nq+i];
-      for (int i = w.lane; i < m.nv; i += 32) { W_(qvel)[i] = b.qvel[(size_t)env*m.nv+i]; W_(qws)[i] = b.qacc_warmstart[(size_t)env*m.nv+i]; }
-      for (int i = w.lane; i < m.na; i += 32) W_(act)[i] = b.act[(size_t)env*m.na+i];
-      if (w.lane < m.neprm) W_(eprm)[w.lane] = b.env_prm ? b.env_prm[(size_t)env*8 + w.lane] : 0.0;     // per-env model overrides (hold task only)
-      for (int i = w.lane; i < m.nwz; i += 32) W_(wz)[i] = -1.0;     // cold start of the inverse-wrap roots at the first substep
-      __syncwarp();
+      load_env_state(m, w, b, env);
       if (a.mode == 2) {
         if (!a.reset_mask || a.reset_mask[env]) { env_reset(m, w, a, env);
           task_observe(m, w, a, env, 0, 0.0);
@@ -403,27 +418,6 @@ extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __gri
 // written while the scratch region holding it is live; nothing is stored back (the Newton warm start is read, the inverse-wrap roots
 // start cold).  The body poses are MuJoCo's quaternion chain over every model body (mj_kinematics), so that xquat carries MuJoCo's
 // sign; they come from the model tables in HBM and do not touch shared memory.
-// The model constants into shared memory, as env_kernel_body stages them (bulk async copies, completion on an mbarrier); a copy of that
-// code, so that the step kernels are compiled from unchanged source.  Every thread of the CTA calls it.
-__device__ __forceinline__ void stage_model(const DevModel& m, unsigned long long& mbar) {
-  double* s_d = smem; idx_t* s_i = (idx_t*)(smem + m.nD);
-  const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-  if (threadIdx.x == 0) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb)); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned bytes_d = (unsigned)m.nD*8u, bytes_i = (unsigned)m.nI16w*4u;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes_d + bytes_i) : "memory");
-    const unsigned CH = 32768u;   // chunked: every piece 16-byte aligned and a multiple of 16 bytes
-    for (unsigned o = 0; o < bytes_d; o += CH) { unsigned n = bytes_d - o < CH ? bytes_d - o : CH;
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_d + o)), "l"((const char*)m.gD + o), "r"(n), "r"(mb) : "memory"); }
-    for (unsigned o = 0; o < bytes_i; o += CH) { unsigned n = bytes_i - o < CH ? bytes_i - o : CH;
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   :: "r"((unsigned)__cvta_generic_to_shared((char*)s_i + o)), "l"((const char*)m.gI16 + o), "r"(n), "r"(mb) : "memory"); }
-  }
-  { unsigned done = 0; while (!done) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(mb) : "memory"); }
-}
-
 enum { DATA_NONE = 0, DATA_ACT = 1, DATA_DYN = 2 };      // how far the shared-memory forward pass runs
 struct DataArgs {
   myo_data_buffers d; myo_buffers b;
@@ -520,23 +514,17 @@ __device__ void data_solve(const DevModel& m, const Warp w, const DataArgs& a, i
 extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DataArgs a) {
   __shared__ __align__(8) unsigned long long mbar;
   const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (a.depth != DATA_NONE) stage_model(m, mbar);
+  if (a.depth != DATA_NONE) STAGE_MODEL(m, mbar)
   const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
   const myo_data_buffers& d = a.d; const myo_buffers& b = a.b;
-  const int per_cta = (a.n_env + (int)gridDim.x - 1)/(int)gridDim.x;
+  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
   for (int j = wid; j < per_cta; j += nw) {
-    const int env = (int)blockIdx.x + (int)gridDim.x*j;
+    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
     if (env >= a.n_env) break;
     if (a.pose) data_poses(m, a, env, w.lane);
     if (a.depth == DATA_NONE) continue;
-    // ---- the stored state into this warp's slice, as the step kernels load it
     if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
-    for (int i = w.lane; i < m.nq; i += 32) W_(qpos)[i] = b.qpos[(size_t)env*m.nq+i];
-    for (int i = w.lane; i < m.nv; i += 32) { W_(qvel)[i] = b.qvel[(size_t)env*m.nv+i]; W_(qws)[i] = b.qacc_warmstart[(size_t)env*m.nv+i]; }
-    for (int i = w.lane; i < m.na; i += 32) W_(act)[i] = b.act[(size_t)env*m.na+i];
-    if (w.lane < m.neprm) W_(eprm)[w.lane] = b.env_prm ? b.env_prm[(size_t)env*8 + w.lane] : 0.0;
-    for (int i = w.lane; i < m.nwz; i += 32) W_(wz)[i] = -1.0;
-    __syncwarp();
+    load_env_state(m, w, b, env);
     phase_kinematics(m, w); phase_tendon_all(m, w);
     phase_actuation(m, w, false, m.g_ctrl + (size_t)env*m.nu, d.actuator_force ? d.actuator_force + (size_t)env*m.nu : nullptr,
                     d.actuator_length ? d.actuator_length + (size_t)env*m.nu : nullptr);
@@ -578,10 +566,12 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
     perm[c + grid*(r*nw + u)] = e; }
 }
 
-struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
-  int warps_per_cta, grid, smem_bytes, obs_dim; int dbg_warps, dbg_grid, dbg_smem; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
+struct LaunchShape { int warps, smem, grid; };      // env-warps per CTA, dynamic shared memory (bytes), CTAs
+// Zero-initialised by myo_batch_create (new myo_batch()), so that myo_batch_destroy can free a partly built batch.
+struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
+  LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
-  int32_t* dRI; double* dRD; double* dPose; DataArgs data; int data_warps, data_grid, data_smem; };
+  int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -600,9 +590,12 @@ static int al2(int x) { return (x + 1) & ~1; }
 static int imax(int a, int b) { return a > b ? a : b; }
 // What fill_devmodel decided beyond the DevModel offsets (myo_model_layout): the size reserved for every persistent and scratch region
 // (slot orders of include/myo_b200.h) and the boundaries and flags of the scratch scheme, the latter relative to the scratch start.
-enum { LP_qpos, LP_qvel, LP_act, LP_qws, LP_dax, LP_dan, LP_qM, LP_fsm, LP_eprm, LP_wz, LP_cnt, LP_scr, LP_N };
-enum { LS_xpos, LS_xmat, LS_U, LS_PL, LS_mom, LS_tlen, LS_tvel, LS_tfrc, LS_cin, LS_crb, LS_bf, LS_conJ, LS_efD, LS_efA, LS_eqJ,
-       LS_icon, LS_con, LS_clist, LS_gpose, LS_efR, LS_efV, LS_va, LS_vg, LS_vp, LS_vMa, LS_vMp, LS_H, LS_Hs, LS_LD, LS_Dinv, LS_N };
+#define LP_ENUM(n) LP_##n,
+#define LS_ENUM(n) LS_##n,
+enum { MYO_LAYOUT_PERSISTENT(LP_ENUM) LP_N };
+enum { MYO_LAYOUT_SCRATCH(LS_ENUM) LS_N };
+#undef LP_ENUM
+#undef LS_ENUM
 struct Layout { int32_t psz[LP_N], ssz[LS_N], head, afterK, extNonSolve, solveEnd, arefInH, qwsInH; };
 static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel& d, Layout* lay = nullptr) {
   const int32_t* I = mm->I.data(); const double* D = mm->D.data(); memset(&d, 0, sizeof(d));
@@ -672,9 +665,9 @@ static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel
   #undef PLACE
   #undef TAKE
   // scratch offsets are used relative to the warp base
-  { int32_t* f[] = {&d.s_xpos, &d.s_xmat, &d.s_U, &d.s_PL, &d.s_mom, &d.s_tlen, &d.s_tvel, &d.s_tfrc, &d.s_cin, &d.s_crb, &d.s_bf, &d.s_conJ, &d.s_efD, &d.s_efA, &d.s_eqJ,
-                    &d.s_icon, &d.s_con, &d.s_clist, &d.s_gpose, &d.s_efR, &d.s_efV, &d.s_va, &d.s_vg, &d.s_vp, &d.s_vMa, &d.s_vMp, &d.s_H, &d.s_Hs, &d.s_LD, &d.s_Dinv};
-    for (int32_t* q : f) *q += d.o_scr; }
+  #define TO_WARP(n) d.s_##n += d.o_scr;
+  MYO_LAYOUT_SCRATCH(TO_WARP)
+  #undef TO_WARP
   d.n_per_warp = d.o_scr + scratch;
 }
 
@@ -687,17 +680,84 @@ extern "C" int myo_model_dims(const myo_model* m, const myo_task_cfg* cfg, myo_d
 extern "C" int myo_model_layout(const myo_model* m, const myo_task_cfg* cfg, int32_t* out, int cap) {
   if (!m || !out || cap < 1) return fail("myo_model_layout: bad arguments");
   DevModel d; Layout L; fill_devmodel(m, cfg, d, &L);
-  const int32_t po[LP_N] = {d.o_qpos, d.o_qvel, d.o_act, d.o_qws, d.o_dax, d.o_dan, d.o_qM, d.o_fsm, d.o_eprm, d.o_wz, d.o_cnt, d.o_scr};
-  const int32_t so[LS_N] = {d.s_xpos, d.s_xmat, d.s_U, d.s_PL, d.s_mom, d.s_tlen, d.s_tvel, d.s_tfrc, d.s_cin, d.s_crb, d.s_bf, d.s_conJ, d.s_efD, d.s_efA, d.s_eqJ,
-                            d.s_icon, d.s_con, d.s_clist, d.s_gpose, d.s_efR, d.s_efV, d.s_va, d.s_vg, d.s_vp, d.s_vMa, d.s_vMp, d.s_H, d.s_Hs, d.s_LD, d.s_Dinv};
+  #define P_OFF(n) d.o_##n,
+  #define S_OFF(n) d.s_##n,
+  const int32_t po[LP_N] = {MYO_LAYOUT_PERSISTENT(P_OFF)};
+  const int32_t so[LS_N] = {MYO_LAYOUT_SCRATCH(S_OFF)};
+  #undef P_OFF
+  #undef S_OFF
   int32_t v[MYO_LAYOUT_N]; int k = 0;
   for (int i = 0; i < LP_N; i++) v[k++] = po[i];
   for (int i = 0; i < LP_N; i++) v[k++] = L.psz[i];
   for (int i = 0; i < LS_N; i++) v[k++] = so[i];
   for (int i = 0; i < LS_N; i++) v[k++] = L.ssz[i];
   const int32_t tail[] = {d.o_scr + L.head, d.o_scr + L.afterK, d.o_scr + L.extNonSolve, d.o_scr + L.solveEnd, L.arefInH, L.qwsInH, d.n_per_warp, d.maxcon, d.maxefc};
+  static_assert(2*LP_N + 2*LS_N + sizeof(tail)/sizeof(tail[0]) == MYO_LAYOUT_N, "MYO_LAYOUT_N counts the region lists of include/myo_b200.h");
   for (int32_t x : tail) v[k++] = x;
   for (int i = 0; i < cap && i < MYO_LAYOUT_N; i++) out[i] = v[i];
+  return 0;
+}
+
+static int warps_that_fit(const cudaDeviceProp& prop, int per_env_bytes, int const_bytes) { return ((int)prop.sharedMemPerBlockOptin - const_bytes - 64)/per_env_bytes; }
+// Launch shape of kernel `fn`: as many env-warps per CTA as its thread limit and shared memory allow, at most one per env.  min_rounds (one
+// CTA per SM): the batch takes ceil(n_env / (SMs * warps)) rounds; among the warp counts that reach the minimal number of rounds take the
+// SMALLEST (same rounds, less issue contention and less lockstep imbalance per round).  want (tuning override, 0 = none) wins where it fits.
+static int launch_shape(const void* fn, const cudaDeviceProp& prop, int per_env_bytes, int const_bytes, int n_env, bool min_rounds, int want, LaunchShape& s) {
+  cudaFuncAttributes fa; CUDA_OK(cudaFuncGetAttributes(&fa, fn));
+  const int sms = prop.multiProcessorCount, fit = warps_that_fit(prop, per_env_bytes, const_bytes), maxw = fa.maxThreadsPerBlock/32;
+  int wpc = fit < maxw ? fit : maxw; if (n_env < wpc) wpc = n_env;
+  if (wpc < 1) return fail("model working set exceeds shared memory of one CTA");
+  if (min_rounds) { int best = wpc, rounds = (n_env + sms*wpc - 1)/(sms*wpc); for (int q = wpc - 1; q >= 1; q--) if ((n_env + sms*q - 1)/(sms*q) == rounds) best = q;
+    if ((size_t)per_env_bytes*best + const_bytes > 100*1024) wpc = best; }
+  if (want >= 1 && want <= (maxw < fit ? maxw : fit)) wpc = want;
+  s.warps = wpc; s.smem = const_bytes + wpc*per_env_bytes;
+  CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem));
+  int c = 1; CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, fn, wpc*32, s.smem)); if (c < 1) c = 1;
+  const int need = (n_env + wpc - 1)/wpc, cap = sms*c; s.grid = need < cap ? need : cap;
+  return 0;
+}
+
+// Everything myo_batch_create does after allocating the batch; on failure the caller destroys the partly built batch.
+static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg) {
+  const int n_env = b->n_env;
+  fill_devmodel(m, cfg, b->dm);
+  if (b->cfg.frame_skip <= 0) b->cfg.frame_skip = 1;
+  b->tol = cfg->solver_tolerance > 0 ? cfg->solver_tolerance : 1e-10;
+  if (cfg->task == MYO_TASK_POSE && b->dm.nq != b->dm.nv) return fail("pose task needs nq == nv");
+  if (cfg->task == MYO_TASK_POSE) b->obs_dim = 2*b->dm.nq + b->dm.nv + b->dm.na;
+  else if (cfg->task == MYO_TASK_WALK) b->obs_dim = (b->dm.nq - 2) + b->dm.nv + 16 + 4*b->dm.nu;
+  else if (cfg->task == MYO_TASK_HOLD) b->obs_dim = (b->dm.nq - 7) + (b->dm.nv - 6) + 6 + b->dm.na;
+  else if (cfg->task == MYO_TASK_REACH) { if (cfg->task_i[0] < 1 || cfg->task_i[0] > 7 || 3*cfg->task_i[0] > b->dm.nq) return fail("reach task: 1..7 tips and 3*ntip <= nq");
+    b->obs_dim = b->dm.nq + b->dm.nv + 6*cfg->task_i[0] + b->dm.na; }
+  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+  b->const_bytes = b->dm.nD*8 + ((b->dm.nI16w + 1)/2)*8;
+  const int per = b->dm.n_per_warp*8, fit = warps_that_fit(prop, per, b->const_bytes);
+  if (b->dm.neq + b->dm.nlimrow + b->dm.maxcon > 255) return fail("equality + limit rows + contact capacity exceed the 255 regulariser slots of the row map");
+  // Launch configurations.  Product: the launch_bounds(320) kernel (168 registers, <= 10 warps) unless more warps fit in shared memory AND cut the
+  // number of rounds, then the launch_bounds(448) kernel (128 registers, <= 14 warps).  Debug kernel: its own configuration (<= 10 warps).
+  cudaFuncAttributes fa_p, fa_w, fa_d; CUDA_OK(cudaFuncGetAttributes(&fa_p, myo_env_kernel)); CUDA_OK(cudaFuncGetAttributes(&fa_w, myo_env_kernel_w14)); CUDA_OK(cudaFuncGetAttributes(&fa_d, myo_env_kernel_dbg));
+  const bool big = (size_t)per*(fit < 4 ? fit : 4) + b->const_bytes > 50*1024;      // a 4-warp CTA already takes > 50 KB: one CTA per SM, sized by the round count (small models run several CTAs per SM instead)
+  auto rounds_of = [&](const LaunchShape& s) { const int sms = prop.multiProcessorCount; return (n_env + sms*s.warps - 1)/(sms*s.warps); }; LaunchShape sp, sw;
+  if (launch_shape((const void*)myo_env_kernel, prop, per, b->const_bytes, n_env, big, 0, sp) || launch_shape((const void*)myo_env_kernel_w14, prop, per, b->const_bytes, n_env, big, 0, sw)) return -1;
+  b->use_w14 = sw.warps > sp.warps && rounds_of(sw) < rounds_of(sp);      // (small models too: the elbow runs 4096 envs in 2 rounds of 14 warps instead of 3 of 10 -- registers, not shared memory, keep it at one CTA per SM)
+  if (const char* e = getenv("MYO_B200_W14")) b->use_w14 = atoi(e) != 0 && fa_w.maxThreadsPerBlock > fa_p.maxThreadsPerBlock;      // tuning override
+  const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;      // tuning override (never above what fits)
+  if (launch_shape(b->use_w14 ? (const void*)myo_env_kernel_w14 : (const void*)myo_env_kernel, prop, per, b->const_bytes, n_env, big, want, b->prod) ||
+      launch_shape((const void*)myo_env_kernel_dbg, prop, per, b->const_bytes, n_env, big, want, b->dbg)) return -1;
+  b->balanced = b->prod.smem > 100*1024; b->dbg_balanced = b->dbg.smem > 100*1024;      // the balanced slot map for CTAs that fill an SM
+  // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
+  b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
+  if (b->regroup) { b->perm_rounds = (SLOTS_PER_CTA(1, n_env, b->prod.grid, b->prod.warps) + b->prod.warps - 1)/b->prod.warps; b->perm_slots = b->prod.grid*b->prod.warps*b->perm_rounds; }
+  // device memory, after every check
+  { const int32_t* I = m->I.data(); const double* D = m->D.data();
+    size_t nI = (size_t)b->dm.nI16w*4, nD = (size_t)MYO_SEC_LEN(I, MYO_SEC_HOT_D)*8;      /* ALL hot doubles go to HBM; the first dm.nD of them are staged per CTA */
+    CUDA_OK(cudaMalloc(&b->dI, nI ? nI : 16)); CUDA_OK(cudaMalloc(&b->dD, nD ? nD : 16));
+    CUDA_OK(cudaMemcpy(b->dI, MYO_ISEC(I, MYO_SEC_HOT_I16), nI, cudaMemcpyHostToDevice)); CUDA_OK(cudaMemcpy(b->dD, MYO_DSEC(I, D, MYO_SEC_HOT_D), nD, cudaMemcpyHostToDevice)); }
+  CUDA_OK(cudaMalloc(&b->dCtrl, (size_t)n_env*imax(b->dm.nu, 1)*8)); CUDA_OK(cudaMemset(b->dCtrl, 0, (size_t)n_env*imax(b->dm.nu, 1)*8));
+  b->dm.gI16 = b->dI; b->dm.gD = b->dD; b->dm.g_ctrl = b->dCtrl;
+  if (b->regroup) { CUDA_OK(cudaMalloc(&b->dLoad, (size_t)n_env*4)); CUDA_OK(cudaMemset(b->dLoad, 0, (size_t)n_env*4)); CUDA_OK(cudaMalloc(&b->dPerm, (size_t)b->perm_slots*4)); }
+  if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
+    n_env, b->use_w14 ? "launch_bounds(448)" : "launch_bounds(320)", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
   return 0;
 }
 
@@ -707,73 +767,26 @@ extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const
   if (e != cudaSuccess || ndev == 0) return fail("myo_batch_create: no CUDA device available (this library has no CPU fallback)");
   if (device < 0 || device >= ndev) return fail("myo_batch_create: bad device index");
   CUDA_OK(cudaSetDevice(device));
-  myo_batch* b = new myo_batch(); memset(&b->bufs, 0, sizeof(b->bufs)); b->model = m; b->device = device; b->n_env = n_env; b->cfg = *cfg; b->bound = false; b->launches = 0; b->seed = 0; b->env_offset = 0;
-  fill_devmodel(m, cfg, b->dm);
-  if (b->cfg.frame_skip <= 0) b->cfg.frame_skip = 1;
-  if (cfg->task == MYO_TASK_POSE && b->dm.nq != b->dm.nv) { delete b; return fail("pose task needs nq == nv"); }
-  b->obs_dim = 0;
-  if (cfg->task == MYO_TASK_POSE) b->obs_dim = 2*b->dm.nq + b->dm.nv + b->dm.na;
-  else if (cfg->task == MYO_TASK_WALK) b->obs_dim = (b->dm.nq - 2) + b->dm.nv + 16 + 4*b->dm.nu;
-  else if (cfg->task == MYO_TASK_HOLD) b->obs_dim = (b->dm.nq - 7) + (b->dm.nv - 6) + 6 + b->dm.na;
-  else if (cfg->task == MYO_TASK_REACH) { if (cfg->task_i[0] < 1 || cfg->task_i[0] > 7 || 3*cfg->task_i[0] > b->dm.nq) { delete b; return fail("reach task: 1..7 tips and 3*ntip <= nq"); }
-    b->obs_dim = b->dm.nq + b->dm.nv + 6*cfg->task_i[0] + b->dm.na; }
-  { const int32_t* I = m->I.data(); const double* D = m->D.data();
-    size_t nI = (size_t)b->dm.nI16w*4, nD = (size_t)MYO_SEC_LEN(I, MYO_SEC_HOT_D)*8;      /* ALL hot doubles go to HBM; the first dm.nD of them are staged per CTA */
-    CUDA_OK(cudaMalloc(&b->dI, nI ? nI : 16)); CUDA_OK(cudaMalloc(&b->dD, nD ? nD : 16));
-    CUDA_OK(cudaMemcpy(b->dI, MYO_ISEC(I, MYO_SEC_HOT_I16), nI, cudaMemcpyHostToDevice)); CUDA_OK(cudaMemcpy(b->dD, MYO_DSEC(I, D, MYO_SEC_HOT_D), nD, cudaMemcpyHostToDevice)); }
-  CUDA_OK(cudaMalloc(&b->dCtrl, (size_t)n_env*imax(b->dm.nu, 1)*8)); CUDA_OK(cudaMemset(b->dCtrl, 0, (size_t)n_env*imax(b->dm.nu, 1)*8));
-  b->dm.gI16 = b->dI; b->dm.gD = b->dD; b->dm.g_ctrl = b->dCtrl;
-  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  b->const_bytes = b->dm.nD*8 + ((b->dm.nI16w + 1)/2)*8;
-  int per = b->dm.n_per_warp*8, maxs = (int)prop.sharedMemPerBlockOptin - b->const_bytes - 64;
-  // Launch configurations.  Product: the launch_bounds(320) kernel (168 registers, <= 10 warps) unless more warps fit in shared memory AND cut the
-  // number of rounds, then the launch_bounds(448) kernel (128 registers, <= 14 warps).  Debug kernel: its own configuration (<= 10 warps).
-  cudaFuncAttributes fa_p, fa_w, fa_d; CUDA_OK(cudaFuncGetAttributes(&fa_p, myo_env_kernel)); CUDA_OK(cudaFuncGetAttributes(&fa_w, myo_env_kernel_w14)); CUDA_OK(cudaFuncGetAttributes(&fa_d, myo_env_kernel_dbg));
-  const int sms = prop.multiProcessorCount, fit = maxs/per;
-  if (fit < 1) { delete b; return fail("model working set exceeds shared memory of one CTA"); }
-  if (b->dm.neq + b->dm.nlimrow + b->dm.maxcon > 255) { delete b; return fail("equality + limit rows + contact capacity exceed the 255 regulariser slots of the row map"); }
-  const bool big = (size_t)per*(fit < 4 ? fit : 4) + b->const_bytes > 50*1024;      // a 4-warp CTA already takes > 50 KB: one CTA per SM, sized by the round count below (small models run several CTAs per SM instead)
-  auto pick = [&](int maxw) { int wpc = fit < maxw ? fit : maxw; if (n_env < wpc) wpc = n_env;
-    // wave quantisation: with one CTA per SM the batch takes ceil(n_env / (SMs * wpc)) rounds; among the warp counts that reach the
-    // minimal number of rounds take the SMALLEST (same rounds, less issue contention and less lockstep imbalance per round)
-    if (big) { int best = wpc, rounds = (n_env + sms*wpc - 1)/(sms*wpc); for (int q = wpc - 1; q >= 1; q--) if ((n_env + sms*q - 1)/(sms*q) == rounds) best = q;
-      if ((size_t)b->dm.n_per_warp*8*best + b->const_bytes > 100*1024) wpc = best; }
-    return wpc; };
-  auto rounds_of = [&](int wpc) { return (n_env + sms*wpc - 1)/(sms*wpc); };
-  int wp = pick(fa_p.maxThreadsPerBlock/32), ww = pick(fa_w.maxThreadsPerBlock/32), wd = pick(fa_d.maxThreadsPerBlock/32);
-  b->use_w14 = ww > wp && rounds_of(ww) < rounds_of(wp);      // (small models too: the elbow runs 4096 envs in 2 rounds of 14 warps instead of 3 of 10 -- registers, not shared memory, keep it at one CTA per SM)
-  if (const char* e = getenv("MYO_B200_W14")) b->use_w14 = atoi(e) != 0 && fa_w.maxThreadsPerBlock > fa_p.maxThreadsPerBlock;      // tuning override
-  int wpc = b->use_w14 ? ww : wp;
-  if (const char* e = getenv("MYO_B200_WARPS_PER_CTA")) { int q = atoi(e), cap = (b->use_w14 ? fa_w.maxThreadsPerBlock : fa_p.maxThreadsPerBlock)/32; if (cap > fit) cap = fit;
-    if (q >= 1 && q <= cap) wpc = q; if (q >= 1 && q <= (fa_d.maxThreadsPerBlock/32 < fit ? fa_d.maxThreadsPerBlock/32 : fit)) wd = q; }     // tuning override (never above what fits)
-  b->warps_per_cta = wpc; b->smem_bytes = b->const_bytes + wpc*per; b->dbg_warps = wd; b->dbg_smem = b->const_bytes + wd*per;
-  CUDA_OK(cudaFuncSetAttribute(myo_env_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, b->smem_bytes));
-  CUDA_OK(cudaFuncSetAttribute(myo_env_kernel_w14, cudaFuncAttributeMaxDynamicSharedMemorySize, b->smem_bytes));
-  CUDA_OK(cudaFuncSetAttribute(myo_env_kernel_dbg, cudaFuncAttributeMaxDynamicSharedMemorySize, b->dbg_smem));
-  { int c = 1; if (b->use_w14) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_env_kernel_w14, wpc*32, b->smem_bytes); else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_env_kernel, wpc*32, b->smem_bytes);
-    if (c < 1) c = 1; int need = (n_env + wpc - 1)/wpc, cap = sms*c; b->grid = need < cap ? need : cap; }
-  { int c = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_env_kernel_dbg, wd*32, b->dbg_smem); if (c < 1) c = 1; int need = (n_env + wd - 1)/wd, cap = sms*c; b->dbg_grid = need < cap ? need : cap; }
-  // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
-  b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
-  b->dLoad = nullptr; b->dPerm = nullptr; b->perm_rounds = 0; b->perm_slots = 0; b->perm_built = false;
-  if (b->regroup) { const int per_cta = (n_env + b->grid - 1)/b->grid; b->perm_rounds = (per_cta + wpc - 1)/wpc; b->perm_slots = b->grid*wpc*b->perm_rounds;
-    CUDA_OK(cudaMalloc(&b->dLoad, (size_t)n_env*4)); CUDA_OK(cudaMemset(b->dLoad, 0, (size_t)n_env*4)); CUDA_OK(cudaMalloc(&b->dPerm, (size_t)b->perm_slots*4)); }
-  if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
-    n_env, b->use_w14 ? "launch_bounds(448)" : "launch_bounds(320)", b->warps_per_cta, b->grid, b->smem_bytes, b->const_bytes, per, fit, b->dbg_warps, b->dbg_grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
+  myo_batch* b = new myo_batch(); b->model = m; b->device = device; b->n_env = n_env; b->cfg = *cfg;
+  if (const int rc = batch_setup(b, m, cfg)) { myo_batch_destroy(b); return rc; }
   *out = b; return 0;
 }
-extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); if (b->dLoad) cudaFree(b->dLoad); if (b->dPerm) cudaFree(b->dPerm);
-  if (b->dRI) cudaFree(b->dRI); if (b->dRD) cudaFree(b->dRD); if (b->dPose) cudaFree(b->dPose); delete b; }
+// The readout's device memory and set-up (also on a failed data_setup, which leaves the batch as if it had not run)
+static void data_release(myo_batch* b) {
+  cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
+  memset(&b->data, 0, sizeof(b->data)); b->data_shape = LaunchShape(); b->data_ready = false; }
+extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
+  data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
-// Launch shape of the product kernels' env steps, as launch() and env_kernel_body compute it.  Fields (first min(n, 8) written):
+// Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 8) written):
 // use_w14, warps_per_cta, grid, rounds per CTA, regroup, balanced, smem_bytes, perm_slots.
 extern "C" int myo_batch_launch_info(const myo_batch* b, int32_t* out, int n) {
   if (!b || !out || n < 1) return fail("myo_batch_launch_info: bad arguments");
-  const int nw = b->warps_per_cta, grid = b->grid, balanced = b->smem_bytes > 100*1024;
+  const int nw = b->prod.warps, grid = b->prod.grid;
   // per_cta and the round loop of env_kernel_body (for j0 = 0; j0 < per_cta; j0 += nw)
-  const int per_cta = b->regroup ? b->perm_rounds*nw : (balanced ? (b->n_env + grid - 1)/grid : ((b->n_env + nw - 1)/nw + grid - 1)/grid*nw);
-  const int32_t v[8] = {b->use_w14 ? 1 : 0, nw, grid, (per_cta + nw - 1)/nw, b->regroup ? 1 : 0, balanced, b->smem_bytes, b->perm_slots};
+  const int per_cta = b->regroup ? b->perm_rounds*nw : SLOTS_PER_CTA(b->balanced, b->n_env, grid, nw);
+  const int32_t v[8] = {b->use_w14 ? 1 : 0, nw, grid, (per_cta + nw - 1)/nw, b->regroup ? 1 : 0, b->balanced, b->prod.smem, b->perm_slots};
   for (int i = 0; i < n && i < 8; i++) out[i] = v[i];
   return 0;
 }
@@ -827,18 +840,18 @@ static int launch(myo_batch* b, StepArgs& a, void* stream) {
   CUDA_OK(cudaSetDevice(b->device));
   a.b = b->bufs; a.cfg = b->cfg; a.n_env = b->n_env; a.obs_dim = b->obs_dim; a.dt = b->dm.timestep*b->cfg.frame_skip;
   a.seed = b->seed; a.env_offset = b->env_offset;
-  a.tol = b->cfg.solver_tolerance > 0 ? b->cfg.solver_tolerance : 1e-10;
+  a.tol = b->tol;
   // the debug instantiation serves forward-debug calls, bound parity taps / cycle counters and the barrier / lockstep tuning knobs
   const myo_buffers& q = b->bufs;
   const bool dbg = a.mode == 1 || b->cfg.barrier_mode != 0 || b->cfg.reserved_i > 1 || q.tap_qacc || q.tap_actuator_force || q.tap_ten_length || q.tap_qfrc_smooth ||
                    q.tap_ncon || q.tap_contact_pair || q.tap_contact_dist || q.tap_moment || q.tap_qM || q.tap_phase_cycles;
-  if (dbg) { a.balanced = b->dbg_smem > 100*1024; myo_env_kernel_dbg<<<b->dbg_grid, b->dbg_warps*32, b->dbg_smem, (cudaStream_t)stream>>>(b->dm, a); }
-  else { a.balanced = b->smem_bytes > 100*1024;
+  if (dbg) { a.balanced = b->dbg_balanced; myo_env_kernel_dbg<<<b->dbg.grid, b->dbg.warps*32, b->dbg.smem, (cudaStream_t)stream>>>(b->dm, a); }
+  else { const LaunchShape& s = b->prod; a.balanced = b->balanced;
     if (a.mode == 0 && b->regroup) {      // env steps: regroup by last step's load first (same stream), then step through the permutation
-      myo_regroup_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->dLoad, b->dPerm, b->n_env, b->grid, b->warps_per_cta, b->perm_slots);
+      myo_regroup_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots);
       a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; b->perm_built = true; b->launches++; }
-    if (b->use_w14) myo_env_kernel_w14<<<b->grid, b->warps_per_cta*32, b->smem_bytes, (cudaStream_t)stream>>>(b->dm, a);
-    else myo_env_kernel<<<b->grid, b->warps_per_cta*32, b->smem_bytes, (cudaStream_t)stream>>>(b->dm, a); }
+    if (b->use_w14) myo_env_kernel_w14<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
+    else myo_env_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a); }
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
 extern "C" int myo_batch_step(myo_batch* b, void* stream) {
@@ -891,18 +904,10 @@ static int data_setup(myo_batch* b) {
   a.nbody = nb; a.nsite = ns; a.nlevel = nlevel; a.lvl = b->dRI; a.parent = b->dRI + o_parent; a.jadr = b->dRI + o_jadr; a.jnum = b->dRI + o_jnum;
   a.jtype = b->dRI + o_jtype; a.jq = b->dRI + o_jq; a.site_body = b->dRI + o_sb; a.pair_geom = b->dRI + o_pg;
   a.bpos = b->dRD + od[0]; a.bquat = b->dRD + od[1]; a.jpos = b->dRD + od[2]; a.jaxis = b->dRD + od[3]; a.qpos0 = b->dRD + od[4]; a.site_pos = b->dRD + od[5];
-  a.pose_buf = b->dPose; a.n_env = b->n_env; a.tol = b->cfg.solver_tolerance > 0 ? b->cfg.solver_tolerance : 1e-10;
-  // launch shape: as many env-warps per CTA as the kernel's thread limit and shared memory allow, balanced env -> CTA map
+  a.pose_buf = b->dPose; a.n_env = b->n_env; a.tol = b->tol;
   cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
-  cudaFuncAttributes fa; CUDA_OK(cudaFuncGetAttributes(&fa, myo_data_kernel));
-  const int per = b->dm.n_per_warp*8, fit = ((int)prop.sharedMemPerBlockOptin - b->const_bytes - 64)/per;
-  int wpc = fa.maxThreadsPerBlock/32; if (wpc > fit) wpc = fit; if (wpc > b->n_env) wpc = b->n_env;
-  if (wpc < 1) return fail("myo_batch_data: model working set exceeds shared memory of one CTA");
-  b->data_warps = wpc; b->data_smem = b->const_bytes + wpc*per;
-  CUDA_OK(cudaFuncSetAttribute(myo_data_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, b->data_smem));
-  int c = 1; CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, myo_data_kernel, wpc*32, b->data_smem)); if (c < 1) c = 1;
-  const int need = (b->n_env + wpc - 1)/wpc; b->data_grid = need < prop.multiProcessorCount*c ? need : prop.multiProcessorCount*c;
-  return 0;
+  if (launch_shape((const void*)myo_data_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->data_shape)) return -1;
+  b->data_ready = true; return 0;
 }
 
 extern "C" int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream) {
@@ -913,8 +918,8 @@ extern "C" int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* str
   const bool dyn = d->qacc || d->ncon || d->contact_geom || d->contact_dist || d->contact_pos || d->contact_frame || d->contact_force;
   if (!pose && !act && !dyn) return 0;
   CUDA_OK(cudaSetDevice(b->device));
-  if (!b->dRI) { const int rc = data_setup(b); if (rc) return rc; }
-  DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE);
-  myo_data_kernel<<<b->data_grid, b->data_warps*32, a.depth == DATA_NONE ? 0 : b->data_smem, (cudaStream_t)stream>>>(b->dm, a);
+  if (!b->data_ready) { if (const int rc = data_setup(b)) { data_release(b); return rc; } }
+  DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE); const LaunchShape& s = b->data_shape;
+  myo_data_kernel<<<s.grid, s.warps*32, a.depth == DATA_NONE ? 0 : s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

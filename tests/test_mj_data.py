@@ -65,6 +65,21 @@ def test_data_buffer_fields_match_header():
     assert _header_struct("myo_buffers")[0] == abi.BUFFER_FIELDS
 
 
+def _header_region_list(macro):
+    src = open(os.path.join(ROOT, "include", "myo_b200.h")).read()
+    body = re.search(r"#define %s\(X\)((?:.*\\\n)*.*)" % macro, src).group(1)
+    return tuple(re.findall(r"X\((\w+)\)", body))
+
+
+def test_layout_regions_match_header():
+    """The names and slot order of myo_model_layout's regions: the X-macro lists the library is built from against abi.LAYOUT_*."""
+    from myosuite_b200 import abi
+    assert _header_region_list("MYO_LAYOUT_PERSISTENT") == abi.LAYOUT_PERSISTENT
+    assert _header_region_list("MYO_LAYOUT_SCRATCH") == abi.LAYOUT_SCRATCH
+    src = open(os.path.join(ROOT, "include", "myo_b200.h")).read()
+    assert int(re.search(r"#define MYO_LAYOUT_N (\d+)", src).group(1)) == abi.LAYOUT_N == 93
+
+
 def test_data_export():
     from myosuite_b200 import abi, build
     assert "myo_batch_data" in abi.EXPORTS
