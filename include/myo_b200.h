@@ -145,6 +145,24 @@ typedef struct {
   double* contact_force;     /* [n, maxcon, 6] mj_contactForce: the pyramid forces decoded into the contact frame, normal first */
 } myo_data_buffers;
 
+/* Caller-owned device buffers of myo_batch_inverse (MuJoCo's mj_inverse): the generalized force that produces the acceleration qacc at
+ * each env's current (qpos, qvel) with the per-env overrides (env_prm) applied,
+ *   qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint
+ * M with armature; qfrc_passive = -damping qvel; qfrc_constraint = J' efc_force with MuJoCo's soft-constraint inverse: jar = J qacc - aref,
+ * efc_force = -D jar on equality rows and on limit and contact rows where jar < 0, else 0.  Contacts, rows and their order are those of
+ * mj_forward at the same state (myo_batch_data's contact list).  act, ctrl and the warm start are not read.  Only the non-null outputs
+ * are written. */
+typedef struct {
+  const double* qacc;        /* [n, nv] in, required */
+  double* qfrc_inverse;      /* [n, nv] out, required */
+  double* qfrc_constraint;   /* [n, nv] nullable */
+  double* contact_force;     /* [n, maxcon, 6] nullable: mj_contactForce of the inverse's efc_force, in myo_data_buffers.contact_force's layout */
+  double* actuator_moment;   /* [n, nu, nv] nullable, dense: gear x the tendon moment (mjData.actuator_moment through mju_sparse2dense) */
+} myo_inverse_buffers;
+#define MYO_INV_NOCONSTRAINT 1   /* mjDSBL_CONSTRAINT: no collision, no constraint rows, qfrc_constraint = 0 */
+#define MYO_INV_DISCRETE 2       /* mjENBL_INVDISCRETE: qacc is (qvel' - qvel) / h of one Euler substep with implicit damping; it is converted to
+                                    the continuous qacc_c = M^-1 (M + h B) qacc of the forward pass, which everything above then uses */
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -207,6 +225,11 @@ int myo_batch_forward_debug(myo_batch* b, const double* ctrl_dev /* [n, nu] */, 
  * alone needs kinematics, the actuation group adds tendons and muscles, the dynamics group adds collision and the constraint solve.
  * Replaces reading env.unwrapped.mj_data after reset() / step() (envs/env_base.py:77-92, robot/robot.py:595-607). */
 int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream);
+
+/* Inverse dynamics of every env (myo_inverse_buffers), one launch on `stream`; flags: MYO_INV_* (0 = MuJoCo's defaults).  The state is
+ * not advanced and no bound buffer is written.  Fails on a null batch, buffers, qacc or qfrc_inverse, an unbound batch or unknown flag bits.
+ * Replaces mujoco.mj_inverse (MyoSuite tutorials 6_Inverse_Dynamics and 9_Computed_muscle_control). */
+int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int flags, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

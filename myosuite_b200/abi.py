@@ -60,10 +60,20 @@ class MyoDataBuffers(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in DATA_FIELDS]
 
 
+# myo_inverse_buffers (include/myo_b200.h): inverse dynamics of myo_batch_inverse, output -> trailing shape in the model's sizes
+INVERSE_FIELDS = ["qacc", "qfrc_inverse", "qfrc_constraint", "contact_force", "actuator_moment"]
+INVERSE_SHAPES = {"qfrc_inverse": ("nv",), "qfrc_constraint": ("nv",), "contact_force": ("maxcon", 6), "actuator_moment": ("nu", "nv")}
+INV_NOCONSTRAINT, INV_DISCRETE = 1, 2           # MYO_INV_* flags
+
+
+class MyoInverseBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in INVERSE_FIELDS]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
-           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data"]
+           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -121,6 +131,7 @@ def _bind(L):
     L.myo_batch_observe.argtypes = [c_vp, c_vp]
     L.myo_batch_forward_debug.argtypes = [c_vp, c_vp, ctypes.c_int, c_vp]
     L.myo_batch_data.argtypes = [c_vp, ctypes.POINTER(MyoDataBuffers), c_vp]
+    L.myo_batch_inverse.argtypes = [c_vp, ctypes.POINTER(MyoInverseBuffers), ctypes.c_int, c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -230,6 +241,20 @@ class Batch:
                 raise ValueError("%s must be contiguous" % k)
             setattr(d, k, t.data_ptr())
         _check(self.L.myo_batch_data(self.handle, ctypes.byref(d), stream), self.L)
+
+    def inverse(self, stream=None, flags=0, **tensors):
+        """Inverse dynamics (myo_batch_inverse) into the given torch CUDA tensors (names of INVERSE_FIELDS: qacc in, the others out; qacc and
+        qfrc_inverse are required).  flags: INV_NOCONSTRAINT | INV_DISCRETE."""
+        d = MyoInverseBuffers()
+        for k, t in tensors.items():
+            if k not in INVERSE_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_inverse(self.handle, ctypes.byref(d), flags, stream), self.L)
 
     @property
     def launches(self):

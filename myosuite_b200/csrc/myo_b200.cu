@@ -494,20 +494,26 @@ __device__ void data_contacts(const DevModel& m, const Warp w, const DataArgs& a
   __syncwarp();
 }
 
-// after the Newton solve: qacc, ncon and mj_contactForce of every contact (the forces of its rows, -D jar where jar < 0, decoded from the pyramid)
+// mj_contactForce of every contact into out [maxcon, 6] (one env's rows), in model pair order, 0 padded: the forces of its rows, -D jar
+// where jar = S_jar < 0, decoded from the pyramid (normal = sum of the edges, tangent i = (edge 2i - edge 2i+1) mu_i)
+__device__ __forceinline__ void write_contact_force(const DevModel& m, const Warp w, double* out) {
+  const int ncon = WI_(ncon);
+  for (int c = w.lane; c < m.maxcon; c += 32) if (c >= ncon) for (int k = 0; k < 6; k++) out[6*c + k] = 0;
+  const idx_t* pr = CI(PPAIR); const double* pd = CD(PPAIR_d);
+  for (int c = w.lane; c < ncon; c += 32) { const int rn = S_crown[c], nr = CNR(rn), rb = CROW(rn); double f[6] = {0, 0, 0, 0, 0, 0};
+    if (nr) { const double Dc = S_D[S_DCON(c)]; double q[4] = {0, 0, 0, 0};
+      for (int k = 0; k < nr; k++) { const double x = S_jar[rb + k]; q[k] = x < 0 ? -Dc*x : 0.0; }
+      if (nr == 1) f[0] = q[0];
+      else { const double* P = pd + pr[PPAIR_ISTRIDE*S_cpair[c] + 6]*PPAIR_STRIDE; f[0] = q[0] + q[1] + q[2] + q[3]; f[1] = (q[0] - q[1])*P[2]; f[2] = (q[2] - q[3])*P[3]; } }
+    for (int k = 0; k < 6; k++) out[6*CRANK(rn) + k] = f[k]; }
+}
+
+// after the Newton solve: qacc, ncon and mj_contactForce of every contact
 __device__ void data_solve(const DevModel& m, const Warp w, const DataArgs& a, int env) {
-  const myo_data_buffers& d = a.d; const int ncon = WI_(ncon); const size_t r0 = (size_t)env*m.maxcon;
+  const myo_data_buffers& d = a.d; const int ncon = WI_(ncon);
   if (d.qacc) for (int i = w.lane; i < m.nv; i += 32) d.qacc[(size_t)env*m.nv + i] = S_a[i];
   if (d.ncon && w.lane == 0) d.ncon[env] = ncon;
-  if (d.contact_force) {
-    for (int c = w.lane; c < m.maxcon; c += 32) if (c >= ncon) for (int k = 0; k < 6; k++) d.contact_force[6*(r0 + c) + k] = 0;
-    const idx_t* pr = CI(PPAIR); const double* pd = CD(PPAIR_d);
-    for (int c = w.lane; c < ncon; c += 32) { const int rn = S_crown[c], nr = CNR(rn), rb = CROW(rn); double f[6] = {0, 0, 0, 0, 0, 0};
-      if (nr) { const double Dc = S_D[S_DCON(c)]; double q[4] = {0, 0, 0, 0};
-        for (int k = 0; k < nr; k++) { const double x = S_jar[rb + k]; q[k] = x < 0 ? -Dc*x : 0.0; }
-        if (nr == 1) f[0] = q[0];
-        else { const double* P = pd + pr[PPAIR_ISTRIDE*S_cpair[c] + 6]*PPAIR_STRIDE; f[0] = q[0] + q[1] + q[2] + q[3]; f[1] = (q[0] - q[1])*P[2]; f[2] = (q[2] - q[3])*P[3]; } }
-      for (int k = 0; k < 6; k++) d.contact_force[6*(r0 + CRANK(rn)) + k] = f[k]; } }
+  if (d.contact_force) write_contact_force(m, w, d.contact_force + 6*(size_t)env*m.maxcon);
   __syncwarp();
 }
 
@@ -543,6 +549,68 @@ extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_c
   }
 }
 
+// ------------------------------------------------------------------ inverse dynamics (myo_batch_inverse)
+// mj_inverse at the stored state of every env, one env per warp on the balanced map: qfrc_inverse = M qacc - qfrc_passive + qfrc_bias -
+// J' efc_force with efc_force = -D (J qacc - aref) on equality rows and on the other rows where that is negative.  Nothing is stored back,
+// and act, ctrl and the warm start are not read: the passive term goes straight into fsm and no actuation phase runs.
+// Scratch lifetimes where they differ from the step's solve stage:
+//   T (mom)      the actuator moments leave for HBM right after the tendon phase: C (cin), written next, may overlap T
+//   efA / H      aref is copied into efV (con region, dead after the constraint phase) before the discrete conversion writes LD / Dinv in
+//                the Hessian region, which holds aref at its head when arefInH
+//   vg / vp      vg holds B qacc, then M^-1 B qacc, then qfrc_constraint; vp is not used
+//   efR, efV     jar (read again by the contact-force decoding); efV: aref, then the row forces -D jar (folded by rows_applyT_add)
+struct InvArgs { myo_inverse_buffers d; myo_buffers b; int n_env, flags; };
+
+extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __grid_constant__ DevModel m, const __grid_constant__ InvArgs a) {
+  __shared__ __align__(8) unsigned long long mbar;
+  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  STAGE_MODEL(m, mbar)
+  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  const myo_inverse_buffers& d = a.d; const bool constraints = !(a.flags & MYO_INV_NOCONSTRAINT), discrete = a.flags & MYO_INV_DISCRETE;
+  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
+  for (int j = wid; j < per_cta; j += nw) {
+    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
+    if (env >= a.n_env) break;
+    if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
+    load_env_state(m, w, a.b, env);
+    phase_kinematics(m, w);
+    if (d.actuator_moment) { phase_tendon_all(m, w);      // dense [nu, nv]: gear x the tendon moment
+      const idx_t* at = CI(PA_tendon); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof); const double* __restrict__ PAm = GD(PAM_d); const double* mom = SCR(s_mom);
+      for (int i = w.lane; i < m.nu; i += 32) { double* row = d.actuator_moment + ((size_t)env*m.nu + i)*m.nv; const double gear = LDC(PAm + i*PAM_STRIDE + 4); const int t = at[i];
+        for (int k = 0; k < m.nv; k++) row[k] = 0;
+        for (int z = nadr[t]; z < nadr[t+1]; z++) row[nzd[z]] += gear*mom[z]; }
+      __syncwarp(); }
+    { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; }
+    __syncwarp();
+    phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w);       // fsm = qfrc_passive - qfrc_bias
+    if (constraints) { phase_collision(m, w); phase_constraints(m, w); }
+    const int nefc = WI_(nefc);
+    for (int r = w.lane; r < nefc; r += 32) S_jv[r] = S_aref[r];
+    for (int i = w.lane; i < m.nv; i += 32) S_a[i] = d.qacc[(size_t)env*m.nv + i];
+    __syncwarp();
+    if (discrete) {      // (M + h B) qacc = M qacc_c: qacc_c = qacc + h M^-1 B qacc, with the integrator's choice of solver
+      const double* dofp = CD(PDOF_d);      // (the program drops the tree-sparse lists where that choice is dense and no Newton step is sparse)
+      for (int i = w.lane; i < m.nv; i += 32) S_g[i] = dofp[2*i+1]*S_a[i];
+      if (m.nv >= 8 && m.nv <= 36) { load_M_dense(m, w, S_H, 0.0); chol_dense(S_H, m.nv, S_g, w.lane); }
+      else { ldl_factor(m, w, W_(qM), S_LD, S_Dinv); ldl_solve(m, w, S_LD, S_Dinv, S_g); }
+      for (int i = w.lane; i < m.nv; i += 32) S_a[i] += m.timestep*S_g[i];
+      __syncwarp(); }
+    mul_M(m, w, S_Ma, S_a);
+    for (int i = w.lane; i < m.nv; i += 32) S_g[i] = 0;
+    __syncwarp();
+    if (constraints) {      // (the row operators walk the equality rows whether or not the constraint phase ran)
+      rows_apply(m, w, S_a, S_jar); __syncwarp();
+      for (int r = w.lane; r < nefc; r += 32) { const double x = S_jar[r] - S_jv[r]; S_jar[r] = x; S_jv[r] = (r < m.neq || x < 0) ? -S_D[S_drow[r]]*x : 0.0; }
+      __syncwarp();
+      rows_applyT_add(m, w, S_jv, S_g); }      // qfrc_constraint
+    for (int i = w.lane; i < m.nv; i += 32) { const size_t o = (size_t)env*m.nv + i;
+      d.qfrc_inverse[o] = S_Ma[i] - W_(fsm)[i] - S_g[i];
+      if (d.qfrc_constraint) d.qfrc_constraint[o] = S_g[i]; }
+    if (d.contact_force) write_contact_force(m, w, d.contact_force + 6*(size_t)env*m.maxcon);
+    __syncwarp();
+  }
+}
+
 // ================================================================== host side (C-ABI)
 static thread_local std::string g_err;
 static int fail(const std::string& s) { g_err = s; return -1; }
@@ -571,7 +639,8 @@ struct LaunchShape { int warps, smem, grid; };      // env-warps per CTA, dynami
 struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
   LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
-  int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready; };
+  int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
+  LaunchShape inv_shape; bool inv_ready; };      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -921,5 +990,19 @@ extern "C" int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* str
   if (!b->data_ready) { if (const int rc = data_setup(b)) { data_release(b); return rc; } }
   DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE); const LaunchShape& s = b->data_shape;
   myo_data_kernel<<<s.grid, s.warps*32, a.depth == DATA_NONE ? 0 : s.smem, (cudaStream_t)stream>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+extern "C" int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int flags, void* stream) {
+  if (!b || !d) return fail("myo_batch_inverse: null");
+  if (!d->qacc || !d->qfrc_inverse) return fail("myo_batch_inverse: qacc and qfrc_inverse are required");
+  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_inverse: unknown flag bits");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  CUDA_OK(cudaSetDevice(b->device));
+  if (!b->inv_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+    if (launch_shape((const void*)myo_inverse_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->inv_shape)) return -1;
+    b->inv_ready = true; }
+  InvArgs a; a.d = *d; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags; const LaunchShape& s = b->inv_shape;
+  myo_inverse_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

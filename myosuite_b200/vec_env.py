@@ -153,7 +153,7 @@ class MyoVecEnv:
             t["final_obs"] = torch.full((n, self.obs_dim), float("nan"), dtype=f32, device=dv)
         self._h_action = None
         # mjData readout (data()): buffers allocated on first request; site_source places the sites the task moves per episode
-        self._data, self.state_version = {}, 0
+        self._data, self._inv, self.state_version = {}, {}, 0         # (inverse(): its output tensors, likewise)
         src = tasks.site_sources(self.task, m, kw, self.tip_names)
         self._site_source = None if src is None else torch.as_tensor(src, device=dv).contiguous()
 
@@ -332,6 +332,34 @@ class MyoVecEnv:
         self.batch.data(stream=self._stream(), **bufs)
         return {f: self._data[f] for f in fields}
 
+    INVERSE_FIELDS = tuple(abi.INVERSE_SHAPES)
+
+    def inverse(self, qacc, constraints=True, discrete=False, fields=("qfrc_inverse",)):
+        """MuJoCo's mj_inverse for every env at its current (qpos, qvel): the generalized force that produces the acceleration `qacc`
+        (float64 CUDA tensor [num_envs, nv] on this batch's device), {field: tensor [num_envs, ...]} for the requested INVERSE_FIELDS:
+        qfrc_inverse, qfrc_constraint, contact_force [maxcon, 6] (mj_contactForce) and the dense actuator_moment [nu, nv].
+        constraints=False is mjDSBL_CONSTRAINT (no contacts, limits or equalities); discrete=True reads qacc as (qvel' - qvel) / h of one
+        Euler substep (mjENBL_INVDISCRETE).  act, ctrl and the warm start do not enter.  One launch; the tensors are allocated on first
+        request and reused, like data()'s.  Not a state change."""
+        torch = self.torch
+        fields = tuple(fields)
+        bad = [f for f in fields if f not in self.INVERSE_FIELDS]
+        if bad:
+            raise KeyError("unknown inverse fields %s (available: %s)" % (bad, list(self.INVERSE_FIELDS)))
+        m, n = self.mj_model, self.num_envs
+        if not isinstance(qacc, torch.Tensor) or qacc.dtype != torch.float64 or qacc.device != self.device or tuple(qacc.shape) != (n, m.nv):
+            raise ValueError("qacc must be a float64 tensor of shape (%d, %d) on %s, got %s" % (
+                n, m.nv, self.device, (type(qacc).__name__, getattr(qacc, "dtype", None), getattr(qacc, "device", None), tuple(getattr(qacc, "shape", ())))))
+        size = dict(nu=m.nu, nv=m.nv, maxcon=self.dims.maxcon)
+        outs = set(fields) | {"qfrc_inverse"}
+        for f in outs:
+            if f not in self._inv:
+                shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in abi.INVERSE_SHAPES[f])
+                self._inv[f] = torch.full(shape, float("nan"), dtype=torch.float64, device=self.device)
+        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
+        self.batch.inverse(stream=self._stream(), flags=flags, qacc=qacc.contiguous(), **{f: self._inv[f] for f in outs})
+        return {f: self._inv[f] for f in fields}
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -488,6 +516,19 @@ class MyoEnv:
         self.vec.refresh_obs()
         r = self._fetch()
         return r["obs"], r["reward"], r["done"], self.get_env_infos()
+
+    def mj_inverse(self, qacc, constraints=True, discrete=False):
+        """mujoco.mj_inverse for this env at its current state: {field: numpy array} of MyoVecEnv.inverse's INVERSE_FIELDS (qfrc_inverse,
+        qfrc_constraint, contact_force [maxcon, 6], actuator_moment [nu, nv]) for the acceleration qacc [nv].  One launch, one
+        device-to-host copy."""
+        v = self.vec
+        q = v.torch.as_tensor(np.asarray(qacc, dtype=np.float64).reshape(1, -1), device=v.device)
+        out = v.inverse(q, constraints=constraints, discrete=discrete, fields=v.INVERSE_FIELDS)
+        flat = v.torch.cat([x[0].reshape(-1) for x in out.values()]).cpu().numpy()
+        res, o = {}, 0
+        for k, x in out.items():
+            res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
+        return res
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)
     def get_obs_dict(self, *sim_args):

@@ -1,9 +1,11 @@
-"""Cost of the mjData readout (MyoVecEnv.data, myo_batch_data) next to one env step, at the benchmarked launch shapes.
+"""Cost of the mjData readout (MyoVecEnv.data, myo_batch_data) and of the inverse dynamics (MyoVecEnv.inverse, myo_batch_inverse) next to
+one env step, at the benchmarked launch shapes.
 
     python tools/data_cost.py [--reps 50] [--warmup 10] [--out FILE.json]
 
-For each case: warm-up steps from a reset, then `reps` rounds that each time one env step and one readout of every group (pose, actuation,
-dynamics, all fields) with CUDA events on the batch's stream, in alternating order.  Prints medians (and min / max) in microseconds and the
+For each case: warm-up steps from a reset, then `reps` rounds that each time one env step, one readout of every group (pose, actuation,
+dynamics, all fields) and the inverse of the readout's qacc (with constraints, without them, with every output) with CUDA events on the
+batch's stream, in alternating order.  Prints medians (and min / max) in microseconds and the
 GPU name, power limit and SM clock read through nvidia-smi's query interface (read-only).  Writes nothing unless --out is given."""
 import argparse
 import json
@@ -20,6 +22,8 @@ GROUPS = {"pose": ("xpos", "xquat", "xmat", "site_xpos"),
           "actuation": ("actuator_length", "actuator_velocity", "actuator_force", "qfrc_actuator"),
           "dynamics": ("qacc", "ncon", "contact_geom", "contact_dist", "contact_pos", "contact_frame", "contact_force"),
           "all": ()}
+INVERSE = {"inverse": dict(fields=("qfrc_inverse",)), "inverse_free": dict(constraints=False, fields=("qfrc_inverse",)),
+           "inverse_all": dict(fields=("qfrc_inverse", "qfrc_constraint", "contact_force", "actuator_moment"))}
 
 
 def gpu_info():
@@ -52,9 +56,12 @@ def main():
             env.step(acts[k % 8])
             for fields in GROUPS.values():
                 env.data(*fields)
+        qacc = env.data("qacc")["qacc"].clone()
+        for kw in INVERSE.values():
+            env.inverse(qacc, **kw)
         torch.cuda.synchronize()
-        t = {k: [] for k in ["step"] + list(GROUPS)}
-        order = ["step"] + list(GROUPS)
+        order = ["step"] + list(GROUPS) + list(INVERSE)
+        t = {k: [] for k in order}
         for r in range(args.reps):
             seq = order if r % 2 == 0 else order[::-1]
             for k in seq:
@@ -62,17 +69,19 @@ def main():
                 e0.record(stream)
                 if k == "step":
                     env.step(acts[r % 8])
+                elif k in INVERSE:
+                    env.inverse(qacc, **INVERSE[k])
                 else:
                     env.data(*GROUPS[k])
                 e1.record(stream)
                 e1.synchronize()
                 t[k].append(e0.elapsed_time(e1) * 1e3)
         s = {k: dict(median_us=float(np.median(v)), min_us=float(np.min(v)), max_us=float(np.max(v))) for k, v in t.items()}
-        for k in GROUPS:
+        for k in order[1:]:
             s[k]["per_step"] = s[k]["median_us"] / s["step"]["median_us"]
         res["cases"][name] = dict(env_id=eid, n_env=n, frame_skip=env.frame_skip, **s)
         print("%-13s n %4d  step %8.1f us | " % (name, n, s["step"]["median_us"])
-              + "  ".join("%s %7.1f us (%.3f step)" % (k, s[k]["median_us"], s[k]["per_step"]) for k in GROUPS), flush=True)
+              + "  ".join("%s %7.1f us (%.3f step)" % (k, s[k]["median_us"], s[k]["per_step"]) for k in order[1:]), flush=True)
         del env
         torch.cuda.empty_cache()
     res["gpu_after"] = gpu_info()
