@@ -163,6 +163,27 @@ typedef struct {
 #define MYO_INV_DISCRETE 2       /* mjENBL_INVDISCRETE: qacc is (qvel' - qvel) / h of one Euler substep with implicit damping; it is converted to
                                     the continuous qacc_c = M^-1 (M + h B) qacc of the forward pass, which everything above then uses */
 
+/* Caller-owned device buffers of myo_batch_rollout (MuJoCo's mj_step, nstep intervals of `substeps` mj_steps each).  ctrl is MuJoCo's
+ * ctrl: clipped to ctrlrange inside the step, as mj_step does, with no action remap, fatigue or reafferentation.  qfrc_applied is
+ * mjData.qfrc_applied: added to qfrc_smooth, so it enters the constraint solve and the implicit-damping Euler step.  The start state
+ * fields are nullable: a null one is taken from the batch's bound buffer of the same name.  Every output is nullable; row t holds
+ * mjData after the last mj_step of interval t. */
+typedef struct {
+  const double* ctrl;        /* [n, nstep, nu] in, required; row t is held for the substeps of interval t */
+  const double* qfrc_applied;/* [n, nstep, nv] in, nullable (zero) */
+  const double* qpos0;       /* [n, nq] start state, nullable (bound qpos) */
+  const double* qvel0;       /* [n, nv] nullable (bound qvel) */
+  const double* act0;        /* [n, na] nullable (bound act) */
+  const double* qacc_warmstart0; /* [n, nv] nullable (bound qacc_warmstart) */
+  const double* time0;       /* [n] nullable (bound time) */
+  double* qpos;              /* [n, nstep, nq] out */
+  double* qvel;              /* [n, nstep, nv] out */
+  double* act;               /* [n, nstep, na] out */
+  double* qacc;              /* [n, nstep, nv] out: mjData.qacc, which is also the next interval's warm start */
+  double* time;              /* [n, nstep] out */
+  int32_t* overflow;         /* [n] out: set when a substep of the rollout dropped contacts (myo_buffers.overflow's meaning), else 0 */
+} myo_rollout_buffers;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -230,6 +251,14 @@ int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream);
  * not advanced and no bound buffer is written.  Fails on a null batch, buffers, qacc or qfrc_inverse, an unbound batch or unknown flag bits.
  * Replaces mujoco.mj_inverse (MyoSuite tutorials 6_Inverse_Dynamics and 9_Computed_muscle_control). */
 int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int flags, void* stream);
+
+/* Rollout of every env (myo_rollout_buffers): nstep intervals of `substeps` mj_steps each, from the given or the bound start state, with
+ * the caller's ctrl and applied forces; one launch per interval on `stream`.  The per-env overrides (env_prm) apply; fatigue, the task
+ * layer (obs, reward, done, counters) and auto-reset do not run.  No bound buffer is written, and results of later env steps and
+ * readouts do not change (the load-sorted grouping of the next env step may).  Fails on a null batch, buffers or ctrl, an unbound
+ * batch, nstep < 1 or substeps < 1.  Replaces mj_step loops over data.ctrl / data.qfrc_applied (MyoSuite tutorials
+ * 6_Inverse_Dynamics and 9_Computed_muscle_control; sampling-based control, system identification, trajectory replay). */
+int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

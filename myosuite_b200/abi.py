@@ -70,10 +70,21 @@ class MyoInverseBuffers(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in INVERSE_FIELDS]
 
 
+# myo_rollout_buffers (include/myo_b200.h): mj_step rollouts of myo_batch_rollout.  Inputs, start state, then the outputs -> trailing shape
+# after [n, nstep] in the model's sizes (overflow is [n], int32)
+ROLLOUT_FIELDS = ["ctrl", "qfrc_applied", "qpos0", "qvel0", "act0", "qacc_warmstart0", "time0", "qpos", "qvel", "act", "qacc", "time", "overflow"]
+ROLLOUT_SHAPES = {"qpos": ("nq",), "qvel": ("nv",), "act": ("na",), "qacc": ("nv",), "time": ()}
+ROLLOUT_STATE = {"qpos": "qpos0", "qvel": "qvel0", "act": "act0", "qacc_warmstart": "qacc_warmstart0", "time": "time0"}     # initial_state key -> field
+
+
+class MyoRolloutBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in ROLLOUT_FIELDS]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
-           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse"]
+           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -132,6 +143,7 @@ def _bind(L):
     L.myo_batch_forward_debug.argtypes = [c_vp, c_vp, ctypes.c_int, c_vp]
     L.myo_batch_data.argtypes = [c_vp, ctypes.POINTER(MyoDataBuffers), c_vp]
     L.myo_batch_inverse.argtypes = [c_vp, ctypes.POINTER(MyoInverseBuffers), ctypes.c_int, c_vp]
+    L.myo_batch_rollout.argtypes = [c_vp, ctypes.POINTER(MyoRolloutBuffers), ctypes.c_int, ctypes.c_int, c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -255,6 +267,20 @@ class Batch:
                 raise ValueError("%s must be contiguous" % k)
             setattr(d, k, t.data_ptr())
         _check(self.L.myo_batch_inverse(self.handle, ctypes.byref(d), flags, stream), self.L)
+
+    def rollout(self, nstep, substeps, stream=None, **tensors):
+        """mj_step rollout (myo_batch_rollout) of nstep intervals of `substeps` mj_steps with the given torch CUDA tensors (names of
+        ROLLOUT_FIELDS: ctrl [n, nstep, nu] required, qfrc_applied and the start state *0 in, the others out)."""
+        d = MyoRolloutBuffers()
+        for k, t in tensors.items():
+            if k not in ROLLOUT_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_rollout(self.handle, ctypes.byref(d), nstep, substeps, stream), self.L)
 
     @property
     def launches(self):

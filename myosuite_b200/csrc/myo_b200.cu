@@ -25,6 +25,8 @@ struct StepArgs {
   int load_wn, load_wi;         // load key = (load_wn * contacts + load_wi * Newton iterations) averaged over the substeps
   unsigned long long seed; long long env_offset;
   double tol, dt;
+  myo_rollout_buffers roll;     // rollout kernels: the caller's ctrl / qfrc_applied and output rows (b points the state at the carry)
+  int roll_t, roll_nstep;       // rollout kernels: the interval this launch runs, of how many
 };
 static const int LOAD_WN = 2, LOAD_WI = 3;      // the load key's weights (StepArgs.load_wn / load_wi) for the product kernels' env steps
 
@@ -284,8 +286,11 @@ __device__ __forceinline__ void load_env_state(const DevModel& m, const Warp w, 
 // ------------------------------------------------------------------ the kernel
 // DBG = false: the product step / reset / observe kernel (modes 0, 2, 3): no parity taps, no cycle counters, fixed barrier scheme.
 // DBG = true: everything -- forward-debug mode (1), parity taps, per-phase cycle counters, the barrier / lockstep-group tuning knobs.
+// ROLL = true: the rollout kernels (myo_batch_rollout), mode 0 only: one interval of a.roll with the caller's ctrl row (m.g_ctrl is neither
+// read nor written) and qfrc_applied added to qfrc_smooth; the launch's cfg has no task, fatigue or reafferentation, and its state
+// buffers are the library's carry, which is also copied into the output rows of the interval.
 // MAXT: launch bound (threads per CTA) -> register budget of the instantiation.
-template <bool DBG, int MAXT>
+template <bool DBG, int MAXT, bool ROLL = false>
 __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArgs& a) {
   __shared__ __align__(8) unsigned long long mbar;
   const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -308,16 +313,16 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
     const bool live = (j0 + wid) < per_cta && env >= 0 && env < a.n_env; const long long tstep_ = prof ? clock64() : 0; int load_acc = 0;
     if (live) {
       load_env_state(m, w, b, env);
-      if (a.mode == 2) {
+      if (!ROLL && a.mode == 2) {
         if (!a.reset_mask || a.reset_mask[env]) { env_reset(m, w, a, env);
           task_observe(m, w, a, env, 0, 0.0);
           if (w.lane == 0) { if (b.done) b.done[env] = 0; if (b.truncated) b.truncated[env] = 0; if (b.reward) b.reward[env] = 0; if (b.overflow) b.overflow[env] = 0; } }
-      } else if (a.mode == 3) {   // observe: obs/reward/done of the current state, nothing advanced (env.forward(), env_base.py:393-432)
+      } else if (!ROLL && a.mode == 3) {   // observe: obs/reward/done of the current state, nothing advanced (env.forward(), env_base.py:393-432)
         { const RwDone rd = task_observe(m, w, a, env, b.step_count ? b.step_count[env] : 0, b.time ? b.time[env] : 0.0);
           if (w.lane == 0) { if (b.reward) b.reward[env] = (float)rd.rw; if (b.done) b.done[env] = rd.done != 0; } }
       } else if (DBG && a.mode == 1) {
         for (int i = w.lane; i < m.nu; i += 32) m.g_ctrl[(size_t)env*m.nu+i] = a.dbg_ctrl[(size_t)env*m.nu+i];
-      } else if (a.mode == 0) {
+      } else if (!ROLL && a.mode == 0) {
         // ---- action -> ctrl  (base_v0.py:83-96); fatigue (fatigue.py:38-76)
         for (int i = w.lane; i < m.nu; i += 32) { double c = (double)b.action[(size_t)env*m.nu+i];
           if (a.cfg.reaf_dst != a.cfg.reaf_src && i == a.cfg.reaf_dst) c = (double)b.action[(size_t)env*m.nu+a.cfg.reaf_src];
@@ -352,7 +357,10 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
       const bool tap = DBG && s == nsub-1;
       PH(0, phase_kinematics(m, w));
       PH(1, phase_tendon_all(m, w); if (tap && b.tap_moment) { const double* mom = SCR(s_mom); for (int i = w.lane; i < m.nnz; i += 32) b.tap_moment[(size_t)env*m.nnz+i] = mom[i]; });
-      PH(2, phase_actuation(m, w, integrate, m.g_ctrl + (size_t)env*m.nu, tap && b.tap_actuator_force ? b.tap_actuator_force + (size_t)env*m.nu : nullptr, tap && b.tap_ten_length ? b.tap_ten_length + (size_t)env*m.nu : nullptr));
+      PH(2, phase_actuation(m, w, integrate, ROLL ? a.roll.ctrl + ((size_t)env*a.roll_nstep + a.roll_t)*m.nu : m.g_ctrl + (size_t)env*m.nu, tap && b.tap_actuator_force ? b.tap_actuator_force + (size_t)env*m.nu : nullptr, tap && b.tap_ten_length ? b.tap_ten_length + (size_t)env*m.nu : nullptr);
+            if (ROLL && a.roll.qfrc_applied) { const double* f = a.roll.qfrc_applied + ((size_t)env*a.roll_nstep + a.roll_t)*m.nv;      // mjData.qfrc_applied
+              for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] += f[i];
+              __syncwarp(); });
       PH(3, phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w));
       PH(4, phase_collision(m, w); overflow_seen |= WI_(overflow));
       PH(5, phase_constraints(m, w); if (tap) write_taps_contacts(m, w, a, env));
@@ -376,7 +384,7 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
         double tnow = b.time ? b.time[env] : 0.0; for (int s_ = 0; s_ < a.cfg.frame_skip; s_++) tnow += m.timestep;
         if (overflow_seen && w.lane == 0 && b.overflow) b.overflow[env] |= 1;      // sticky until the next reset of this env
         if (!DBG && a.load && w.lane == 0) a.load[env] = load_acc/(nsub > 0 ? nsub : 1);
-        if (a.cfg.task != MYO_TASK_NONE) { const RwDone rd = task_observe(m, w, a, env, b.step_count ? b.step_count[env] : 0, tnow); const double rw = rd.rw; const bool done = rd.done != 0;
+        if (!ROLL && a.cfg.task != MYO_TASK_NONE) { const RwDone rd = task_observe(m, w, a, env, b.step_count ? b.step_count[env] : 0, tnow); const double rw = rd.rw; const bool done = rd.done != 0;
           int sc = b.step_count ? b.step_count[env]+1 : 0; bool trunc = a.cfg.max_episode_steps > 0 && sc >= a.cfg.max_episode_steps;
           __syncwarp();
           // truncated follows gym's TimeLimit: set whenever the step budget is reached, also when the episode terminated on the same step
@@ -399,6 +407,12 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
       for (int i = w.lane; i < m.nq; i += 32) b.qpos[(size_t)env*m.nq+i] = W_(qpos)[i];
       for (int i = w.lane; i < m.nv; i += 32) { b.qvel[(size_t)env*m.nv+i] = W_(qvel)[i]; if (store_qws) b.qacc_warmstart[(size_t)env*m.nv+i] = W_(qws)[i]; }
       for (int i = w.lane; i < m.na; i += 32) b.act[(size_t)env*m.na+i] = W_(act)[i];
+      if (ROLL) { const myo_rollout_buffers& r = a.roll; const size_t row = (size_t)env*a.roll_nstep + a.roll_t;      // mjData after the interval
+        if (r.qpos) for (int i = w.lane; i < m.nq; i += 32) r.qpos[row*m.nq+i] = W_(qpos)[i];
+        if (r.qvel) for (int i = w.lane; i < m.nv; i += 32) r.qvel[row*m.nv+i] = W_(qvel)[i];
+        if (r.act) for (int i = w.lane; i < m.na; i += 32) r.act[row*m.na+i] = W_(act)[i];
+        if (r.qacc) for (int i = w.lane; i < m.nv; i += 32) r.qacc[row*m.nv+i] = W_(qws)[i];
+        if (r.time && w.lane == 0) r.time[row] = b.time[env]; }
       __syncwarp();
     }
   }
@@ -412,6 +426,9 @@ extern "C" __global__ void __launch_bounds__(320) myo_env_kernel(const __grid_co
 extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
 // parity taps / forward-debug / profiling counters / tuning knobs
 extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<true, 320>(m, a); }
+// rollout (myo_batch_rollout): the product body's mode 0 with the caller's ctrl and applied forces, under the two product launch bounds
+extern "C" __global__ void __launch_bounds__(320) myo_roll_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320, true>(m, a); }
+extern "C" __global__ void __launch_bounds__(448) myo_roll_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448, true>(m, a); }
 
 // ------------------------------------------------------------------ mjData readout (myo_batch_data)
 // One forward pass over the stored state of every env, one env per warp on the balanced map (env = CTA + grid * slot).  Each field is
@@ -640,7 +657,9 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
   int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
-  LaunchShape inv_shape; bool inv_ready; };      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
+  LaunchShape inv_shape; bool inv_ready;      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
+  // rollout (myo_batch_rollout), set up by its first call: carry state [n, nq + 2 nv + na + 1] (qpos | qvel | act | warm start | time)
+  bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -815,7 +834,7 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
       launch_shape((const void*)myo_env_kernel_dbg, prop, per, b->const_bytes, n_env, big, want, b->dbg)) return -1;
   b->balanced = b->prod.smem > 100*1024; b->dbg_balanced = b->dbg.smem > 100*1024;      // the balanced slot map for CTAs that fill an SM
   // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
-  b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
+  b->big = big; b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
   if (b->regroup) { b->perm_rounds = (SLOTS_PER_CTA(1, n_env, b->prod.grid, b->prod.warps) + b->prod.warps - 1)/b->prod.warps; b->perm_slots = b->prod.grid*b->prod.warps*b->perm_rounds; }
   // device memory, after every check
   { const int32_t* I = m->I.data(); const double* D = m->D.data();
@@ -845,7 +864,7 @@ static void data_release(myo_batch* b) {
   cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
   memset(&b->data, 0, sizeof(b->data)); b->data_shape = LaunchShape(); b->data_ready = false; }
 extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
-  data_release(b); delete b; }
+  cudaFree(b->dCarry); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
 // Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 8) written):
@@ -1005,4 +1024,52 @@ extern "C" int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int
   InvArgs a; a.d = *d; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags; const LaunchShape& s = b->inv_shape;
   myo_inverse_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+// First rollout of a batch: the launch shape of the rollout kernel that matches the env step's instantiation (from its own attributes,
+// with the env step's sizing rule and tuning override) and the carry state.  With the env step's shape the rollout also runs on its slot
+// map (load-sorted when the batch regroups); with another shape, on the balanced map without regrouping.
+static int roll_setup(myo_batch* b) {
+  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+  const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;
+  if (launch_shape(b->use_w14 ? (const void*)myo_roll_kernel_w14 : (const void*)myo_roll_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, b->big, want, b->roll_shape)) return -1;
+  const bool same = b->roll_shape.warps == b->prod.warps && b->roll_shape.grid == b->prod.grid && b->roll_shape.smem == b->prod.smem;
+  b->roll_regroup = same && b->regroup; b->roll_balanced = same ? b->balanced : 1;
+  const DevModel& d = b->dm;
+  CUDA_OK(cudaMalloc(&b->dCarry, (size_t)b->n_env*(d.nq + 2*d.nv + d.na + 1)*8));
+  b->roll_ready = true; return 0;
+}
+
+extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
+  if (!b || !r) return fail("myo_batch_rollout: null");
+  if (!r->ctrl) return fail("myo_batch_rollout: ctrl is required");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (nstep < 1 || substeps < 1) return fail("myo_batch_rollout: nstep and substeps must be >= 1");
+  CUDA_OK(cudaSetDevice(b->device));
+  if (!b->roll_ready) { if (const int rc = roll_setup(b)) { cudaFree(b->dCarry); b->dCarry = nullptr; return rc; } }
+  const DevModel& d = b->dm; const size_t n = b->n_env; cudaStream_t st = (cudaStream_t)stream;
+  // the carry: the start state, from the caller's rows or the bound buffers
+  myo_buffers c; memset(&c, 0, sizeof(c));
+  c.qpos = b->dCarry; c.qvel = c.qpos + n*d.nq; c.act = c.qvel + n*d.nv; c.qacc_warmstart = c.act + n*d.na; c.time = c.qacc_warmstart + n*d.nv;
+  const myo_buffers& q = b->bufs;
+  const struct { double* dst; const double* src; int width; } init[5] = {{c.qpos, r->qpos0 ? r->qpos0 : q.qpos, d.nq}, {c.qvel, r->qvel0 ? r->qvel0 : q.qvel, d.nv},
+    {c.act, r->act0 ? r->act0 : q.act, d.na}, {c.qacc_warmstart, r->qacc_warmstart0 ? r->qacc_warmstart0 : q.qacc_warmstart, d.nv}, {c.time, r->time0 ? r->time0 : q.time, 1}};
+  for (const auto& f : init) {
+    if (f.width == 0) continue;
+    if (f.src) CUDA_OK(cudaMemcpyAsync(f.dst, f.src, n*f.width*8, cudaMemcpyDeviceToDevice, st));
+    else CUDA_OK(cudaMemsetAsync(f.dst, 0, n*f.width*8, st)); }      // (an unbound time buffer: the rollout starts at 0)
+  if (r->overflow) CUDA_OK(cudaMemsetAsync(r->overflow, 0, n*4, st));
+  c.env_prm = q.env_prm; c.overflow = r->overflow;
+  StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 0; a.b = c; a.roll = *r; a.roll_nstep = nstep;
+  a.cfg = b->cfg; a.cfg.task = MYO_TASK_NONE; a.cfg.muscle_condition = MYO_COND_NONE; a.cfg.reaf_dst = a.cfg.reaf_src = 0; a.cfg.auto_reset = 0; a.cfg.frame_skip = substeps;
+  a.n_env = b->n_env; a.dt = d.timestep*substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset; a.balanced = b->roll_balanced;
+  const LaunchShape& s = b->roll_shape;
+  if (b->roll_regroup) { a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; }
+  for (int t = 0; t < nstep; t++) {
+    a.roll_t = t;
+    if (b->roll_regroup) { myo_regroup_kernel<<<1, 1024, 0, st>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots); b->launches++; }
+    if (b->use_w14) myo_roll_kernel_w14<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+    else myo_roll_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+    CUDA_OK(cudaGetLastError()); b->launches++; }
+  return 0;
 }

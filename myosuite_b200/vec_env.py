@@ -360,6 +360,61 @@ class MyoVecEnv:
         self.batch.inverse(stream=self._stream(), flags=flags, qacc=qacc.contiguous(), **{f: self._inv[f] for f in outs})
         return {f: self._inv[f] for f in fields}
 
+    ROLLOUT_FIELDS = tuple(abi.ROLLOUT_SHAPES) + ("overflow",)
+
+    def rollout(self, ctrl, qfrc_applied=None, substeps=1, initial_state=None, fields=("qpos", "qvel", "act", "qacc", "time")):
+        """MuJoCo's mj_step for every env: nstep intervals of `substeps` mj_steps each, with the MuJoCo ctrl row ctrl[:, t] held for the
+        substeps of interval t.  ctrl is mjData.ctrl, NOT the env's action: it is clipped to ctrlrange as mj_step does, and neither the
+        action sigmoid (normalize_act), fatigue nor reafferentation is applied; a caller who starts from actions applies the remap itself
+        (1 / (1 + exp(-5 (a - 0.5))) when normalize_act is set).  qfrc_applied [num_envs, nstep, nv] (mjData.qfrc_applied, None = zero)
+        is added to qfrc_smooth.  Both are float64 CUDA tensors on this batch's device, contiguous, ctrl [num_envs, nstep, nu].
+        initial_state: {"qpos", "qvel", "act", "qacc_warmstart", "time": float64 tensor [num_envs, width] ([num_envs] for time)}; a key
+        left out is taken from the env's current state.  Returns {field: tensor [num_envs, nstep, ...]} of ROLLOUT_FIELDS, mjData after
+        the last mj_step of each interval: qpos, qvel, act, qacc (also the next warm start: a rollout resumes exactly from row t with
+        initial_state = its qpos, qvel, act, time and qacc as qacc_warmstart), time; overflow [num_envs] int32 is set where a substep
+        dropped contacts.  The tensors are allocated per call.  Per-env overrides (env_prm) apply; the task layer, counters and auto-reset
+        do not run, and the env's own state and episode are left as they were: not a state change.  One launch per interval."""
+        torch = self.torch
+        fields = tuple(fields)
+        bad = [f for f in fields if f not in self.ROLLOUT_FIELDS]
+        if bad:
+            raise KeyError("unknown rollout fields %s (available: %s)" % (bad, list(self.ROLLOUT_FIELDS)))
+        m, n = self.mj_model, self.num_envs
+        substeps = int(substeps)
+        if substeps < 1:
+            raise ValueError("substeps must be >= 1, got %d" % substeps)
+
+        def check(name, x, shape):
+            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
+                    or not x.is_contiguous()):
+                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
+                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
+                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+        nstep = int(ctrl.shape[1]) if isinstance(ctrl, torch.Tensor) and ctrl.dim() == 3 else 0
+        if nstep < 1:
+            raise ValueError("ctrl must be a float64 tensor [num_envs, nstep >= 1, nu], got %s" % (tuple(getattr(ctrl, "shape", ())),))
+        check("ctrl", ctrl, (n, nstep, m.nu))
+        bufs = {"ctrl": ctrl}
+        if qfrc_applied is not None:
+            check("qfrc_applied", qfrc_applied, (n, nstep, m.nv))
+            bufs["qfrc_applied"] = qfrc_applied
+        width = dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=())
+        for k, v in (initial_state or {}).items():
+            if k not in abi.ROLLOUT_STATE:
+                raise KeyError("unknown initial_state key %r (available: %s)" % (k, list(abi.ROLLOUT_STATE)))
+            if v is not None:
+                check("initial_state[%r]" % k, v, (n,) + width[k])
+                bufs[abi.ROLLOUT_STATE[k]] = v
+        size = dict(nq=m.nq, nv=m.nv, na=m.na)
+        out = {}
+        for f in fields:
+            if f == "overflow":
+                out[f] = torch.zeros(n, dtype=torch.int32, device=self.device)
+            else:
+                out[f] = torch.full((n, nstep) + tuple(size[x] for x in abi.ROLLOUT_SHAPES[f]), float("nan"), dtype=torch.float64, device=self.device)
+        self.batch.rollout(nstep, substeps, stream=self._stream(), **bufs, **out)
+        return out
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -528,6 +583,26 @@ class MyoEnv:
         res, o = {}, 0
         for k, x in out.items():
             res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
+        return res
+
+    def mj_rollout(self, ctrl, qfrc_applied=None, substeps=1, initial_state=None):
+        """mujoco.mj_step rollout of this env (MyoVecEnv.rollout): ctrl [nstep, nu] is MuJoCo's ctrl, not the action (no sigmoid remap:
+        apply normalize_act's 1 / (1 + exp(-5 (a - 0.5))) yourself when starting from actions), qfrc_applied [nstep, nv] or None,
+        initial_state {key: array} or None (the current state).  Returns {field: numpy array [nstep, ...]} of qpos, qvel, act, qacc, time
+        and the int overflow flag.  The env's own state is left as it was.  One device-to-host copy."""
+        v = self.vec
+        torch = v.torch
+        as_dev = lambda x, shape: torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        c = np.asarray(ctrl, dtype=np.float64)
+        nstep = c.reshape(-1, self.mj_model.nu).shape[0]
+        q = None if qfrc_applied is None else as_dev(qfrc_applied, (1, nstep, self.mj_model.nv))
+        st = None if initial_state is None else {k: as_dev(x, (1,) if k == "time" else (1, -1)) for k, x in initial_state.items()}
+        out = v.rollout(as_dev(c, (1, nstep, -1)), qfrc_applied=q, substeps=substeps, initial_state=st, fields=v.ROLLOUT_FIELDS)
+        flat = torch.cat([x[0].reshape(-1).double() for x in out.values()]).cpu().numpy()
+        res, o = {}, 0
+        for k, x in out.items():
+            res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
+        res["overflow"] = int(res["overflow"])
         return res
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)

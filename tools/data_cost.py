@@ -1,11 +1,12 @@
-"""Cost of the mjData readout (MyoVecEnv.data, myo_batch_data) and of the inverse dynamics (MyoVecEnv.inverse, myo_batch_inverse) next to
-one env step, at the benchmarked launch shapes.
+"""Cost of the mjData readout (MyoVecEnv.data, myo_batch_data), of the inverse dynamics (MyoVecEnv.inverse, myo_batch_inverse) and of
+mj_step rollouts (MyoVecEnv.rollout, myo_batch_rollout) next to one env step, at the benchmarked launch shapes.
 
     python tools/data_cost.py [--reps 50] [--warmup 10] [--out FILE.json]
 
 For each case: warm-up steps from a reset, then `reps` rounds that each time one env step, one readout of every group (pose, actuation,
-dynamics, all fields) and the inverse of the readout's qacc (with constraints, without them, with every output) with CUDA events on the
-batch's stream, in alternating order.  Prints medians (and min / max) in microseconds and the
+dynamics, all fields), the inverse of the readout's qacc (with constraints, without them, with every output) and two rollouts from the
+current state with CUDA events on the batch's stream, in alternating order.  The rollouts: "rollout", 8 intervals of frame_skip substeps,
+reported per interval (the physics of one env step); "rollout_1", frame_skip intervals of one substep, reported per call (the same physics).  Prints medians (and min / max) in microseconds and the
 GPU name, power limit and SM clock read through nvidia-smi's query interface (read-only).  Writes nothing unless --out is given."""
 import argparse
 import json
@@ -24,6 +25,7 @@ GROUPS = {"pose": ("xpos", "xquat", "xmat", "site_xpos"),
           "all": ()}
 INVERSE = {"inverse": dict(fields=("qfrc_inverse",)), "inverse_free": dict(constraints=False, fields=("qfrc_inverse",)),
            "inverse_all": dict(fields=("qfrc_inverse", "qfrc_constraint", "contact_force", "actuator_moment"))}
+ROLLOUT_NSTEP = 8           # intervals of the "rollout" row
 
 
 def gpu_info():
@@ -59,8 +61,13 @@ def main():
         qacc = env.data("qacc")["qacc"].clone()
         for kw in INVERSE.values():
             env.inverse(qacc, **kw)
+        fs = env.frame_skip
+        roll = {"rollout": (torch.rand(n, ROLLOUT_NSTEP, m.nu, generator=g, dtype=torch.float64).to(env.device), fs, ROLLOUT_NSTEP),
+                "rollout_1": (torch.rand(n, fs, m.nu, generator=g, dtype=torch.float64).to(env.device), 1, 1)}      # (ctrl, substeps, divisor)
+        for ctrl, sub, _ in roll.values():
+            env.rollout(ctrl, substeps=sub)
         torch.cuda.synchronize()
-        order = ["step"] + list(GROUPS) + list(INVERSE)
+        order = ["step"] + list(GROUPS) + list(INVERSE) + list(roll)
         t = {k: [] for k in order}
         for r in range(args.reps):
             seq = order if r % 2 == 0 else order[::-1]
@@ -71,11 +78,13 @@ def main():
                     env.step(acts[r % 8])
                 elif k in INVERSE:
                     env.inverse(qacc, **INVERSE[k])
+                elif k in roll:
+                    env.rollout(roll[k][0], substeps=roll[k][1])
                 else:
                     env.data(*GROUPS[k])
                 e1.record(stream)
                 e1.synchronize()
-                t[k].append(e0.elapsed_time(e1) * 1e3)
+                t[k].append(e0.elapsed_time(e1) * 1e3 / (roll[k][2] if k in roll else 1))
         s = {k: dict(median_us=float(np.median(v)), min_us=float(np.min(v)), max_us=float(np.max(v))) for k, v in t.items()}
         for k in order[1:]:
             s[k]["per_step"] = s[k]["median_us"] / s["step"]["median_us"]
