@@ -100,7 +100,7 @@ def reward_dict(task, obs_dict, weights, cfg):
                                      ("sparse", -1.0 * d), ("solved", d < thd), ("done", d > far_th)))
     elif task == "reach":                                                  # reach_v0.py:120-160
         d = np.linalg.norm(obs_dict["reach_err"], axis=-1); ntip = cfg["ntip"]
-        far_th = np.where(np.asarray(obs_dict["time"]) > 2 * cfg["dt"], cfg["far_th"] * ntip, np.inf); near = _near(task, ntip)
+        far_th = np.where(np.squeeze(obs_dict["time"]) > 2 * cfg["dt"], cfg["far_th"] * ntip, np.inf); near = _near(task, ntip)      # (the single env's time is [1])
         r = collections.OrderedDict((("reach", -1.0 * d), ("bonus", 1.0 * (d < 2 * near) + 1.0 * (d < near)), ("act_reg", -1.0 * act_mag), ("penalty", -1.0 * (d > far_th)),
                                      ("sparse", -1.0 * d), ("solved", d < near), ("done", d > far_th)))
     elif task == "stand":                                                  # walk_v0.py:104-140 (ReachEnvV0 of the legs)

@@ -45,6 +45,16 @@ def registered_ids():
 
 
 _MODEL_OF_XML = {v[0]: k for k, v in assets.MODEL_XML.items()}
+
+
+def condition_model(m, muscle_condition):
+    """The model a batch of `muscle_condition` simulates: sarcopenia halves the peak force of every muscle in a copy of m
+    (base_v0.py:62-67: gainprm[:,2] *= 0.5, biasprm untouched); fatigue and reafferentation act on ctrl and keep m itself."""
+    if muscle_condition == "sarcopenia":
+        import copy
+        m = copy.deepcopy(m)
+        m.actuator_gainprm[:, 2] *= 0.5
+    return m
 stand_target_centre = tasks.stand_target_centre          # (importable from here as before)
 
 
@@ -72,10 +82,7 @@ class MyoVecEnv:
         self._check_kwargs(kw)
         self.mj_model = m = model if model is not None else assets.load(_MODEL_OF_XML[kw["model_path"]])
         self.muscle_condition = kw.get("muscle_condition", "")
-        if self.muscle_condition == "sarcopenia":       # base_v0.py:62-67: gainprm[:,2] *= 0.5 (biasprm untouched)
-            import copy
-            self.mj_model = m = copy.deepcopy(m)
-            m.actuator_gainprm[:, 2] *= 0.5
+        self.mj_model = m = condition_model(m, self.muscle_condition)
         prog, self.prog_info = program.build_program(m)
         self.prog = prog
         self.I, self.D = blob.pack(m, prog)

@@ -7,11 +7,19 @@ the reference's own unmodified code (tests/golden/make_golden.py).
 import numpy as np
 
 
-def action_to_ctrl(a, normalize_act=True):
-    """myosuite/envs/myo/base_v0.py:83-96 (all actuators of the hot-path models are muscles)."""
+def action_to_ctrl(a, normalize_act=True, reaf=None, muscle=None):
+    """myosuite/envs/myo/base_v0.py:83-108 without fatigue (see Fatigue / env_step for that branch).
+    reaf: (EPL, EIP) actuator ids of the reafferentation condition or None; after the remap the EPL entry takes the EIP entry and
+    the EIP entry is zeroed (base_v0.py:104-108).  muscle: bool mask of actuator_dyntype == mjDYN_MUSCLE, or None for all muscles
+    (true of every shipped model, tests/test_variants.py); the sigmoid applies to the masked entries only (base_v0.py:84-90)."""
     a = np.array(a, dtype=np.float64, copy=True)
     if normalize_act:
-        a = 1.0 / (1.0 + np.exp(-5.0 * (a - 0.5)))
+        m = slice(None) if muscle is None else np.asarray(muscle, dtype=bool)
+        a[m] = 1.0 / (1.0 + np.exp(-5.0 * (a[m] - 0.5)))
+    if reaf is not None:
+        dst, src = reaf
+        a[dst] = a[src]
+        a[src] = 0.0
     return a
 
 
@@ -59,9 +67,9 @@ def pose_reward(qpos, act, target, pose_thd, weights=(1.0, 4.0, 1.0, 50.0), far_
     return r
 
 
-def env_step(oracle, action, frame_skip, normalize_act=True, fatigue=None):
+def env_step(oracle, action, frame_skip, normalize_act=True, fatigue=None, reaf=None):
     """One control step on the physics oracle: base_v0.py:82-118 + robot.py:901-905 (same ctrl for all substeps)."""
-    ctrl = action_to_ctrl(action, normalize_act)
+    ctrl = action_to_ctrl(action, normalize_act, reaf=reaf)
     if fatigue is not None:
         ctrl = fatigue.compute_act(ctrl)[0].copy()
     oracle.set(ctrl=ctrl)

@@ -13,25 +13,13 @@ envs right before the checked step: their step starts from the randomised reset 
 the mid-episode bounds too."""
 import time
 
-import numpy as np
 import pytest
 
-import philox_ref as P
-from parity_helpers import _in_regime, relerr
+from parity_helpers import LAUNCH_ENV, Oracles, replay_product_step  # noqa: F401  (Oracles: imported from here by other modules)
 
 pytestmark = pytest.mark.gpu
 
 HAND = "myoHandPoseRandom-v0"
-WARM = 6                 # control steps from reset before the checked one
-SEED = 7
-N_RESET, N_CONTACT, N_PRESAMPLE, N_RANDOM, N_IDLE_NB = 16, 16, 256, 48, 8
-# tolerances of the mid-episode parity tests (test_gpu_parity.py) and of the task tests (obs / reward)
-QPOS_ATOL, QVEL_REL, ACT_ATOL, QACC_REL, FATIGUE_RTOL = 2e-7, 1e-5, 1e-12, 1e-6, 1e-12
-OBS_TOL = {"walk": (1e-4, 2e-5)}            # (rtol, atol); every other task (2e-6, 2e-6)
-RWD_TOL = {"walk": 1e-4}                    # rel = abs; every other task 1e-5
-THRESHOLD_MARGIN = 1e-5                     # reward / done are not compared for envs this close to a task threshold
-MAX_SKIP_REGIME = 0.25                      # largest share of the selected envs that may lie outside the contact regime
-
 # case -> (env id, n_env, environment of the library, env kwargs, expected launch_info subset).  The expected shapes are those of the
 # launch heuristic of myo_batch_create on an H100 SXM (132 SMs, 227 KB of shared memory per CTA); a change there fails the case.
 CASES = {
@@ -50,7 +38,6 @@ CASES = {
     "stand_fatigue": ("myoFatiLegStandRandom-v0", 2048, {}, {}, dict(use_w14=0, warps_per_cta=6, rounds=3, regroup=1)),
 }
 N_FIRST = {"stand": 48, "stand_fatigue": 48}      # envs reset right before the checked step (0 for the other cases)
-LAUNCH_ENV = ("MYO_B200_REGROUP", "MYO_B200_W14", "MYO_B200_WARPS_PER_CTA")
 REPORT = []
 
 
@@ -63,296 +50,11 @@ def report():
         print("  " + line)
 
 
-def slot_table(info, n, perm):
-    """[rounds, warps_per_cta, grid] table of the env each (round, warp, CTA) slot stepped, -1 for an idle slot."""
-    R, nw, grid = info["rounds"], info["warps_per_cta"], info["grid"]
-    if info["regroup"]:
-        return perm.reshape(R, nw, grid)          # slot cta + grid*(round*nw + warp) (myo_regroup_kernel)
-    j = np.arange(R * nw)[:, None]; c = np.arange(grid)[None, :]           # j = j0 + wid
-    # env_kernel_body, myo_b200.cu:266-269: per_cta, then env = c + grid*(j0 + wid) (balanced) or (c + grid*(j0/nw))*nw + wid
-    if info["balanced"]:
-        per_cta = -(-n // grid); env = c + grid * j
-    else:
-        per_cta = -(-(-(-n // nw)) // grid) * nw; env = (c + grid * (j // nw)) * nw + j % nw
-    return np.where((j < per_cta) & (env < n), env, -1).reshape(R, nw, grid)
-
-
-def check_map(T, n):
-    """Every env in [0, n) is stepped by exactly one slot; every other slot is idle (-1)."""
-    live = T[T >= 0]
-    assert np.array_equal(np.sort(live), np.arange(n)), "slot map does not cover every env exactly once"
-    assert np.all((T >= 0) | (T == -1))
-
-
-class Oracles:
-    """The oracle of one env's model.  Hold: the object's geom size is the env's own (env_prm[3:6]); it is patched into a copy of the
-    packed model at the offsets found by packing the model once more with other sizes."""
-
-    def __init__(self, env):
-        from oracle.oracle_py import Oracle
-        self.env, self.Oracle, self.off = env, Oracle, None
-        self.base = Oracle(env.I, env.D)
-        if env.task == "hold":
-            import copy
-            from myosuite_b200 import blob
-            m2 = copy.deepcopy(env.mj_model); g = m2.name2id("geom", "object")
-            m2.geom_size[g] = m2.geom_size[g] + np.array([1.0, 2.0, 3.0])
-            I2, D2 = blob.pack(m2, env.prog)
-            self.off = np.nonzero(D2 != env.D)[0]
-            assert np.array_equal(I2, env.I) and len(self.off) == 3 and np.allclose(D2[self.off] - env.D[self.off], [1.0, 2.0, 3.0])
-
-    def get(self, prm=None):
-        if self.off is None:
-            return self.base
-        D = self.env.D.copy(); D[self.off] = prm[3:6]
-        return self.Oracle(self.env.I, D)
-
-
-def load_state(o, env, S, e):
-    m = env.mj_model
-    o.reset()
-    o.set(qpos=S["qpos"][e], qvel=S["qvel"][e], act=S["act"][e, :m.na], qacc_warmstart=S["qacc_warmstart"][e])
-    o.f("time")[:] = S["time"][e]
-    o.f("wrap_warm")[:] = 1     # inverse wraps: cold start at the first substep, then from the previous substep's root, as the kernel does
-
-
-def task_obs(env, o, steps, tnow, target, prm):
-    """obs, dense reward, done of the oracle's current state through env_oracle, and the distance of the task's decisive quantity to
-    the nearest threshold it is compared with."""
-    from oracle import env_oracle
-    m, dt = env.mj_model, env.dt
-    if env.task == "pose":
-        q, v, a = o.f("qpos").copy(), o.f("qvel").copy(), o.f("act").copy()
-        thd, far = float(env.cfg.pose_thd), (np.pi if env.torso else 4 * np.pi / 2)
-        r = env_oracle.pose_reward(q, a, target, thd, far_th=far)
-        return env_oracle.pose_obs(q, v, a, target, dt), r["dense"], r["done"], min(abs(-r["pose"] - t) for t in (thd, 1.5 * thd, far))
-    o.set(ctrl=np.zeros(m.nu)); o.forward()          # forward quantities of the observed state (the walk test's convention: ctrl = 0)
-    if env.task == "walk":
-        cfg = dict(hip_period=100, min_height=0.8, max_rot=0.8, target_x_vel=0.0, target_y_vel=1.2, target_rot=m.key_qpos[0][3:7])
-        obs, r = env_oracle.walk_obs_reward(m, o, steps, dt, env_oracle.walk_ids(m), cfg)
-        com_z = float(np.sum(m.body_mass * o.f("xipos").reshape(-1, 3)[:, 2]) / np.sum(m.body_mass))
-        return obs, r["dense"], r["done"], min(abs(com_z - 0.8), abs(abs(env_oracle.quat2mat00(o.f("qpos")[3:7])) - 0.8))
-    if env.task == "hold":
-        obs, r = env_oracle.hold_obs_reward(m, o, dt, prm[:3])
-        return obs, r["dense"], r["done"], min(abs(-r["goal_dist"] - t) for t in (0.010, 0.020, 0.300))
-    from test_leg_stand import STAND_WEIGHTS
-    ntip, far_th, shape = len(env.tip_names), float(env.kwargs.get("far_th", 0.35)), tuple(env.cfg.reach_shape)
-    obs, r = env_oracle.reach_obs_reward(m, o, dt, env.tip_names, target[:3 * ntip].reshape(ntip, 3), tnow, far_th=far_th, shape=shape,
-                                         weights=STAND_WEIGHTS if env.task == "stand" else None)
-    near = ntip * (shape[3] if any(shape) else 0.0125)
-    ths = [near, 2 * near] + ([far_th * ntip] if tnow > 2 * dt else [])
-    return obs, r["dense"], r["done"], min(abs(-r["sparse"] - t) for t in ths)
-
-
-def select(T, rng, contact_top, reset_envs):
-    """env -> reasons it is checked (see the module docstring).  Every (round, warp slot) pair that steps an env in some CTA is
-    checked in two CTAs (one when only one CTA uses it: the last round of the fixed balanced map)."""
-    R, nw, grid = T.shape
-    chosen = {}
-
-    def add(e, why):
-        chosen.setdefault(int(e), set()).add(why)
-    for r in range(R):
-        for w in range(nw):
-            ctas = np.nonzero(T[r, w] >= 0)[0]
-            for c in rng.choice(ctas, min(2, len(ctas)), replace=False):
-                add(T[r, w, c], "cover")
-    flat = T.reshape(-1)                                     # flat index == slot index
-    add(flat[np.nonzero(flat >= 0)[0].max()], "last")
-    for c in (0, grid - 1):
-        if T[R - 1, nw - 1, c] >= 0:
-            add(T[R - 1, nw - 1, c], "last")
-    nb = [T[r, w, c] for r in range(R) for c in range(grid) for w in range(nw)
-          if T[r, w, c] >= 0 and ((w > 0 and T[r, w - 1, c] < 0) or (w + 1 < nw and T[r, w + 1, c] < 0))]
-    for e in rng.permutation(nb)[:N_IDLE_NB]:
-        add(e, "idle-nb")
-    for e in contact_top:
-        add(e, "contacts")
-    for e in reset_envs:
-        add(e, "reset")
-    for e in rng.choice(T[T >= 0], N_RANDOM, replace=False):
-        add(e, "random")
-    return chosen
-
-
-def perm_or_none(env, info):
-    return env.batch.perm() if info["regroup"] else None
-
-
 @pytest.mark.parametrize("case", list(CASES))
 def test_product_step_vs_oracle(case, monkeypatch):
-    import torch
-    from myosuite_b200 import vec_env
-    from oracle import env_oracle
     eid, n, lib_env, kw, expect = CASES[case]
-    n_first = N_FIRST.get(case, 0)
     for k in LAUNCH_ENV:
         monkeypatch.delenv(k, raising=False)
     for k, v in lib_env.items():
         monkeypatch.setenv(k, v)
-    t0 = time.time()
-    env = vec_env.MyoVecEnv(eid, n, seed=SEED, **kw)
-    m = env.mj_model
-    assert "tap_qacc" not in env.t
-    info = env.batch.launch_info()
-    assert {k: info[k] for k in expect} == expect, info
-    assert info["rounds"] >= 2 and info["warps_per_cta"] >= 2
-    assert info["perm_slots"] == (info["grid"] * info["warps_per_cta"] * info["rounds"] if info["regroup"] else 0)
-
-    # ---- reached states: reset + WARM control steps of seeded random actions, auto-reset on; the slot map checked on every step
-    env.reset(seed=SEED)
-    g = torch.Generator(device="cpu").manual_seed(SEED)
-    for _ in range(WARM):
-        env.step((torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device))
-        check_map(slot_table(info, n, perm_or_none(env, info)), n)
-    rng = np.random.default_rng(SEED)
-    trunc_set = rng.choice(n, n // 4, replace=False)
-    first_set = []
-    if n_first:          # their checked step is the first of an episode
-        first_set = rng.choice(np.setdiff1d(np.arange(n), trunc_set), n_first, replace=False)
-        mask = np.zeros(n, np.uint8); mask[first_set] = 1
-        env.reset(mask=torch.as_tensor(mask, device=env.device))
-    S0 = env.get_env_state()
-    sc = S0["step_count"].copy(); sc[trunc_set] = env.max_episode_steps - 1
-    env.set_env_state({"step_count": sc})
-    S = env.get_env_state()
-    assert np.array_equal(S["qacc_warmstart"], S0["qacc_warmstart"]) and np.array_equal(S["qpos"], S0["qpos"])
-    assert np.all(S["step_count"][first_set] == 0) and np.all(S["time"][first_set] == 0) and np.all(S["qacc_warmstart"][first_set] == 0)
-    ov0 = env.t["overflow"].cpu().numpy().copy()
-    a = (torch.rand(n, m.nu, generator=g) * 2 - 1).numpy().astype(np.float32)
-
-    # ---- contact-heavy envs: one oracle forward per env of a pre-sample, on the snapshot
-    oracles = Oracles(env)
-    pre = rng.choice(n, min(N_PRESAMPLE, n), replace=False); ncon = []
-    for e in pre:
-        o = oracles.get(S.get("env_prm", [None] * n)[e]); load_state(o, env, S, e)
-        o.set(ctrl=env_oracle.action_to_ctrl(a[e].astype(np.float64), bool(env.cfg.normalize_act))); o.forward(); ncon.append(o.ncon)
-    contact_top = pre[np.argsort(ncon, kind="stable")[::-1][:N_CONTACT]]
-
-    # ---- the checked step
-    obs, rew, done, trunc, info_d = env.step(torch.as_tensor(a, device=env.device))
-    torch.cuda.synchronize()
-    obs, rew, done, trunc = (x.cpu().numpy().copy() for x in (obs, rew, done, trunc))
-    last_ret, ov = info_d["last_return"].cpu().numpy().copy(), env.t["overflow"].cpu().numpy().copy()
-    N = env.get_env_state()
-    T = slot_table(info, n, perm_or_none(env, info))
-    check_map(T, n)
-    resets = np.nonzero(done | trunc)[0]
-    assert np.all(trunc[trunc_set]) and len(resets) >= n // 4
-    chosen = select(T, rng, contact_top, rng.choice(trunc_set, N_RESET, replace=False))
-    for e in first_set:
-        chosen.setdefault(int(e), set()).add("first-step")
-
-    where = {int(e): (r, w, c) for (r, w, c), e in np.ndenumerate(T) if e >= 0}
-    worst = dict(qpos=0.0, qvel=0.0, qacc=0.0, obs=0.0, reward=0.0, qpos_first=0.0, qvel_first=0.0, qacc_first=0.0)
-    cnt = dict(checked=0, phys=0, first=0, reset=0, threshold=0, overflow=0, regime=0)
-    covered = {}
-    rtol, atol = OBS_TOL.get(env.task, (2e-6, 2e-6)); rw_tol = RWD_TOL.get(env.task, 1e-5)
-
-    def check(e, why):
-        """Replay env e's step on the oracle and compare; False when the env lies outside the parity claim."""
-        msg = "%s env %d (round, warp, cta) %s, checked as %s" % (case, e, where[e], sorted(why))
-        if ov0[e] or ov[e]:               # a substep dropped contacts: outside the parity claim (rate bounded in test_gpu_parity.py)
-            cnt["overflow"] += 1
-            return False
-        prm = S["env_prm"][e] if "env_prm" in S else None
-        o = oracles.get(prm); load_state(o, env, S, e)
-        fat = None
-        if "fatigue" in S:
-            fat = env_oracle.Fatigue(m.nu, dt=env.dt, tauact=m.actuator_dynprm[:, 0], taudeact=m.actuator_dynprm[:, 1])
-            fat.MA, fat.MR, fat.MF = (S["fatigue"][e, k].copy() for k in range(3))
-        ctrl = env_oracle.action_to_ctrl(a[e].astype(np.float64), bool(env.cfg.normalize_act))        # env_oracle.env_step, one substep at a time
-        o.set(ctrl=fat.compute_act(ctrl)[0].copy() if fat is not None else ctrl)
-        in_regime = True
-        for _ in range(env.n_frames):
-            o.step(1); in_regime = in_regime and _in_regime(o, m)
-        if not in_regime:                 # deep ellipsoid penetration on some substep: outside the parity claim, as in test_rollout_parity
-            cnt["regime"] += 1
-            return False
-        tnow = float(S["time"][e])
-        for _ in range(env.n_frames):
-            tnow += m.opt_timestep
-        qpos, qvel, act, qacc = (o.f(k).copy() for k in ("qpos", "qvel", "act", "qacc"))
-        target = S["target"][e]
-        x_obs, x_rw, x_done, margin = task_obs(env, o, int(S["step_count"][e]), tnow, target, prm)
-        x_trunc = int(S["step_count"][e]) + 1 >= env.max_episode_steps
-        # ---- reward / done / TimeLimit / returns of the step, pre-reset
-        if margin > THRESHOLD_MARGIN:
-            worst["reward"] = max(worst["reward"], abs(float(rew[e]) - x_rw))
-            assert rew[e] == pytest.approx(x_rw, rel=rw_tol, abs=rw_tol), msg
-            assert bool(done[e]) == bool(x_done), msg
-        else:
-            cnt["threshold"] += 1
-        assert bool(trunc[e]) == x_trunc, msg
-        R = np.float32(S["ep_return"][e]) + rew[e]                     # f32 running return, as the kernel adds it
-        if done[e] or trunc[e]:
-            assert last_ret[e] == R, msg
-            cnt["reset"] += 1
-            # ---- the stored state is a fresh reset ...
-            assert np.all(N["act"][e] == 0) and np.all(N["qacc_warmstart"][e] == 0) and N["time"][e] == 0, msg
-            assert N["step_count"][e] == 0 and N["episode_count"][e] == S["episode_count"][e] + 1 and N["ep_return"][e] == 0, msg
-            # (no case runs the walk task's random keyframe reset)
-            assert np.array_equal(N["qvel"][e], np.reshape(env.init_qvel, (-1, m.nv))[0]), msg
-            # qpos, target, per-env object: the draws of the stream of the episode count the env had before the step
-            P.compare_reset(env, N, P.replay_env(env, env.seed_value, S["episode_count"][[e]], [e]), msg, rows=[e])
-            if "fatigue" in N:
-                assert env.cfg.fatigue_reset == 0
-                assert np.all(N["fatigue"][e, 0] == 0) and np.all(N["fatigue"][e, 1] == 1) and np.all(N["fatigue"][e, 2] == 0), msg
-            # ... and its obs is the obs of that state
-            o = oracles.get(N["env_prm"][e] if "env_prm" in N else None); load_state(o, env, N, e)
-            r_obs = task_obs(env, o, 0, 0.0, N["target"][e], N["env_prm"][e] if "env_prm" in N else None)[0]
-            np.testing.assert_allclose(obs[e], r_obs, rtol=rtol, atol=atol, err_msg=msg)
-        else:
-            # ---- physics and state of a step that did not end the episode: the mid-episode tolerances on every such env
-            first = "first-step" in why                     # a step from a fresh reset state: the same bounds, its own worst case
-            cnt["phys"] += 1; cnt["first"] += first
-            sfx = "_first" if first else ""
-            worst["qpos" + sfx] = max(worst["qpos" + sfx], float(np.abs(N["qpos"][e] - qpos).max()))
-            worst["qvel" + sfx] = max(worst["qvel" + sfx], relerr(N["qvel"][e], qvel))
-            worst["qacc" + sfx] = max(worst["qacc" + sfx], relerr(N["qacc_warmstart"][e], qacc))
-            np.testing.assert_allclose(N["qpos"][e], qpos, rtol=0, atol=QPOS_ATOL, err_msg=msg)
-            assert relerr(N["qvel"][e], qvel) < QVEL_REL, msg
-            assert relerr(N["qacc_warmstart"][e], qacc) < QACC_REL, msg           # the stored warm start is the last substep's qacc
-            np.testing.assert_allclose(N["act"][e, :m.na], act, rtol=0, atol=ACT_ATOL, err_msg=msg)
-            if fat is not None:
-                np.testing.assert_allclose(N["fatigue"][e], np.stack([fat.MA, fat.MR, fat.MF]), rtol=FATIGUE_RTOL, atol=1e-15, err_msg=msg)
-            assert N["time"][e] == tnow, msg                                   # bit-equal: frame_skip additions of the timestep
-            assert N["step_count"][e] == S["step_count"][e] + 1 and N["episode_count"][e] == S["episode_count"][e], msg
-            assert N["ep_return"][e] == R, msg
-            worst["obs"] = max(worst["obs"], float(np.abs(obs[e] - x_obs).max()))
-            np.testing.assert_allclose(obs[e], x_obs, rtol=rtol, atol=atol, err_msg=msg)
-        cnt["checked"] += 1
-        r, w, c = where[e]
-        covered.setdefault((r, w), set()).add(c)
-        return True
-
-    for e in sorted(chosen):
-        check(e, chosen[e])
-    # every (round, warp slot) pair in two CTAs: an env skipped above (overflow, deep penetration) is replaced by one from another CTA
-    nw, R = info["warps_per_cta"], info["rounds"]
-    live = {(r, w): int(np.sum(T[r, w] >= 0)) for r in range(R) for w in range(nw) if np.any(T[r, w] >= 0)}
-    assert sum(v >= 2 for v in live.values()) >= (R - 1) * nw          # all but the last round's slots run in many CTAs
-    replaced = 0
-    for (r, w), v in live.items():
-        for c in rng.permutation(np.nonzero(T[r, w] >= 0)[0]):
-            if len(covered.get((r, w), ())) >= min(2, v):
-                break
-            if int(T[r, w, c]) not in chosen and c not in covered.get((r, w), ()):
-                chosen[int(T[r, w, c])] = {"cover-replacement"}; replaced += 1
-                check(int(T[r, w, c]), chosen[int(T[r, w, c])])
-    full = sum(len(covered.get(k, ())) >= min(2, v) for k, v in live.items())
-    first_rep = ("  first steps after a reset %d: qpos %.1e  qvel %.1e  qacc %.1e" % (cnt["first"], worst["qpos_first"], worst["qvel_first"], worst["qacc_first"])
-                 if n_first else "")
-    REPORT.append("%-12s %-26s n %4d  %s  warps %2d  grid %3d  rounds %d  %s  checked %3d of %3d (physics %3d, auto-reset %2d; skipped: deep penetration %d, "
-                  "contact overflow %d; reward/done near a threshold %d)  (round, slot) pairs checked in 2 CTAs %d/%d (%d replacements)  "
-                  "worst: qpos %.1e  qvel %.1e  qacc %.1e  obs %.1e  reward %.1e%s  [%.1f s]"
-                  % (case, eid, n, "w14" if info["use_w14"] else "k320", nw, info["grid"], R, "regroup" if info["regroup"] else ("balanced" if info["balanced"] else "contiguous"),
-                     cnt["checked"], len(chosen), cnt["phys"], cnt["reset"], cnt["regime"], cnt["overflow"], cnt["threshold"], full, len(live), replaced,
-                     worst["qpos"], worst["qvel"], worst["qacc"], worst["obs"], worst["reward"], first_rep, time.time() - t0))
-    print(REPORT[-1])
-    assert cnt["reset"] >= N_RESET
-    assert full == len(live), "(round, slot) pairs not checked in two CTAs"
-    assert cnt["phys"] >= 32 and cnt["first"] >= n_first // 2
-    # envs outside the parity claim stay rare: deep ellipsoid penetration on ~6 % of the env-steps of a random-action rollout (regime test),
-    # more among the contact-heavy picks here; contact overflow ~1e-5 of env-steps
-    assert cnt["regime"] <= MAX_SKIP_REGIME * len(chosen) and cnt["overflow"] <= 3
+    replay_product_step(case, eid, n, kw, expect, n_first=N_FIRST.get(case, 0), report=REPORT)
