@@ -184,6 +184,41 @@ typedef struct {
   int32_t* overflow;         /* [n] out: set when a substep of the rollout dropped contacts (myo_buffers.overflow's meaning), else 0 */
 } myo_rollout_buffers;
 
+/* Caller-owned device buffers of myo_batch_ik: damped least-squares inverse kinematics of ns sites (one list for the batch) to per-env
+ * targets.  From q = q0 (qpos0, or the bound qpos) each iteration k = 0, 1, ... runs mj_kinematics at q; the site errors
+ * e_s = target_pos_s - site_xpos_s and, with orientation targets, w_s = log(mat(target_quat_s) site_xmat_s') (world-frame rotation
+ * vector, angle in [0, pi]); stops with converged = 1 when every |e_s| <= tol and every |w_s| <= tol, or with converged = 0 at
+ * k = max_iter; else solves
+ *   H = sum_s (wp_s jacp_s' jacp_s + wr_s jacr_s' jacr_s) + eq_weight sum_e J_e' J_e + posture_weight P + damping I
+ *   g = sum_s (wp_s jacp_s' e_s + wr_s jacr_s' w_s) - eq_weight sum_e J_e' c_e + posture_weight P (qpos_ref - q)
+ * for H dq = g (joint equalities e with residual c_e and row J_e as the constraint rows have them; P: 1 on hinge and slide dofs, 0 on
+ * free-joint dofs; a dof outside dof_mask gets an identity row and column and g = 0), caps |dq| at max_step, and sets
+ * q <- q (+) dq (mj_integratePos with dt = 1), then clamps every limited hinge or slide joint to its range.  Every output describes the
+ * returned qpos; max_iter = 0 returns q0 with its Jacobians (mj_jacSite) and errors. */
+#define MYO_IK_MAXSITE 16
+typedef struct {
+  const int32_t* site_id;    /* [ns] in, required: model site ids */
+  const double* site_quat;   /* [ns, 4] in, required: each site's frame in its body, mjModel.site_quat (the model blob carries no site frames) */
+  const double* site_weight; /* [ns, 2] nullable (1, 1): position and orientation weight of each site */
+  const double* target_pos;  /* [n, ns, 3] in, required */
+  const double* target_quat; /* [n, ns, 4] nullable (position targets only): w x y z, normalised here */
+  const double* qpos0;       /* [n, nq] start, nullable (bound qpos) */
+  const double* qpos_ref;    /* [n, nq] posture reference, nullable (the start) */
+  const uint8_t* dof_mask;   /* [nv] nullable (every dof moves): 0 holds the dof */
+  double* qpos;              /* [n, nq] out, required */
+  int32_t* niter;            /* [n] nullable: updates applied */
+  int32_t* converged;        /* [n] nullable */
+  double* err;               /* [n, ns, 2] nullable: |e_s|, |w_s| (0 without orientation targets) */
+  double* site_xpos;         /* [n, ns, 3] nullable */
+  double* site_xmat;         /* [n, ns, 9] nullable */
+  double* jacp;              /* [n, ns, 3, nv] nullable: mj_jacSite */
+  double* jacr;              /* [n, ns, 3, nv] nullable */
+} myo_ik_buffers;
+typedef struct {
+  int32_t nsite, max_iter;
+  double tol, damping, max_step, posture_weight, eq_weight;
+} myo_ik_params;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -259,6 +294,13 @@ int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int flags, voi
  * batch, nstep < 1 or substeps < 1.  Replaces mj_step loops over data.ctrl / data.qfrc_applied (MyoSuite tutorials
  * 6_Inverse_Dynamics and 9_Computed_muscle_control; sampling-based control, system identification, trajectory replay). */
 int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream);
+
+/* Inverse kinematics of every env (myo_ik_buffers, myo_ik_params), one launch on `stream`; each env iterates until its own stop test.
+ * No bound buffer is written: adopting a solution is a separate state change.  Fails before any launch on a null batch, buffers,
+ * site_id, site_quat, target_pos or qpos, an unbound batch, nsite outside [1, MYO_IK_MAXSITE], a site id outside [0, nsite), damping <= 0,
+ * max_step <= 0, tol < 0, max_iter < 0 or a non-finite parameter.  Replaces mj_jacSite and the mink / dm_control IK loops over it
+ * (MyoSuite tutorial 8_inverse_kinematics, marker and fingertip retargeting). */
+int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_params* p, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

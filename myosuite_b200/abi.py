@@ -81,10 +81,28 @@ class MyoRolloutBuffers(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in ROLLOUT_FIELDS]
 
 
+# myo_ik_buffers / myo_ik_params (include/myo_b200.h): inverse kinematics of myo_batch_ik.  Inputs, then the outputs -> trailing shape
+# after [n] in the call's sizes (ns sites)
+IK_FIELDS = ["site_id", "site_quat", "site_weight", "target_pos", "target_quat", "qpos0", "qpos_ref", "dof_mask",
+             "qpos", "niter", "converged", "err", "site_xpos", "site_xmat", "jacp", "jacr"]
+IK_SHAPES = {"qpos": ("nq",), "niter": (), "converged": (), "err": ("ns", 2), "site_xpos": ("ns", 3), "site_xmat": ("ns", 9),
+             "jacp": ("ns", 3, "nv"), "jacr": ("ns", 3, "nv")}
+IK_MAXSITE = 16                                 # MYO_IK_MAXSITE
+
+
+class MyoIkBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in IK_FIELDS]
+
+
+class MyoIkParams(ctypes.Structure):
+    _fields_ = [("nsite", c_i32), ("max_iter", c_i32)] + [(n, c_f64) for n in ("tol", "damping", "max_step", "posture_weight", "eq_weight")]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
-           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout"]
+           "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout",
+           "myo_batch_ik"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -144,6 +162,7 @@ def _bind(L):
     L.myo_batch_data.argtypes = [c_vp, ctypes.POINTER(MyoDataBuffers), c_vp]
     L.myo_batch_inverse.argtypes = [c_vp, ctypes.POINTER(MyoInverseBuffers), ctypes.c_int, c_vp]
     L.myo_batch_rollout.argtypes = [c_vp, ctypes.POINTER(MyoRolloutBuffers), ctypes.c_int, ctypes.c_int, c_vp]
+    L.myo_batch_ik.argtypes = [c_vp, ctypes.POINTER(MyoIkBuffers), ctypes.POINTER(MyoIkParams), c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -281,6 +300,20 @@ class Batch:
                 raise ValueError("%s must be contiguous" % k)
             setattr(d, k, t.data_ptr())
         _check(self.L.myo_batch_rollout(self.handle, ctypes.byref(d), nstep, substeps, stream), self.L)
+
+    def ik(self, params, stream=None, **tensors):
+        """Inverse kinematics (myo_batch_ik) with the given torch CUDA tensors (names of IK_FIELDS: site_id, target_pos and qpos are
+        required) and a MyoIkParams."""
+        d = MyoIkBuffers()
+        for k, t in tensors.items():
+            if k not in IK_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_ik(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
 
     @property
     def launches(self):

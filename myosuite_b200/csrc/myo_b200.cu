@@ -628,6 +628,143 @@ extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __gri
   }
 }
 
+// ------------------------------------------------------------------ inverse kinematics (myo_batch_ik)
+// Damped least squares to site targets (include/myo_b200.h: myo_ik_buffers), one env per warp on the balanced map.  Each warp runs its own
+// iterations and leaves on its own stop test; nothing is stored back.  Lane s < ns holds site s: its pose and errors stay in registers,
+// and the normal equations are summed site by site, so the per-env slice is the step kernels' whatever ns is.  Lane l owns rows l and
+// l + 32 of the packed H (the dense solver's padded order, identity padding) and the same entries of g.
+// Scratch lifetimes within one iteration:
+//   K (xpos, xmat)   written by the kinematics, read once into the site lanes' registers; dead before H is touched (H may overlap it)
+//   va, vMa, vMp     one site's three Jacobian rows at a time (position, then rotation), read by every lane's rows of H
+//   vg, H            g and H from the first site to the solve; vg then holds the step dq until the joint update
+struct IkArgs {
+  myo_ik_buffers d; myo_ik_params p; const double* bound_qpos; int n_env;
+  int site_body[MYO_IK_MAXSITE];                    // program body of each site, -1 for a static body (site_frame is then in world coordinates)
+  unsigned long long site_dofs[MYO_IK_MAXSITE];     // bit i: dof i moves the site's body (the ancestor dofs; the host checks nv <= 64)
+  double site_frame[MYO_IK_MAXSITE][12];            // site position in its program body; for a static body: world position, world body rotation
+};
+
+// log(Q R'): world-frame rotation vector from the site rotation R to the unit target quaternion Q, angle in [0, pi]
+__device__ __forceinline__ void ik_rotvec(const double* Q, const double* R, double* out) {
+  double T[9], E[9]; quat2mat(T, Q);
+  #pragma unroll
+  for (int i = 0; i < 3; i++)
+    #pragma unroll
+    for (int j = 0; j < 3; j++) E[3*i+j] = T[3*i]*R[3*j] + T[3*i+1]*R[3*j+1] + T[3*i+2]*R[3*j+2];
+  double q[4]; const double tr = E[0] + E[4] + E[8];      // rotation matrix -> quaternion, largest pivot first
+  if (tr > 0) { const double s = 2*sqrt(tr + 1); q[0] = 0.25*s; q[1] = (E[7] - E[5])/s; q[2] = (E[2] - E[6])/s; q[3] = (E[3] - E[1])/s; }
+  else if (E[0] > E[4] && E[0] > E[8]) { const double s = 2*sqrt(1 + E[0] - E[4] - E[8]); q[0] = (E[7] - E[5])/s; q[1] = 0.25*s; q[2] = (E[1] + E[3])/s; q[3] = (E[2] + E[6])/s; }
+  else if (E[4] > E[8]) { const double s = 2*sqrt(1 + E[4] - E[0] - E[8]); q[0] = (E[2] - E[6])/s; q[1] = (E[1] + E[3])/s; q[2] = 0.25*s; q[3] = (E[5] + E[7])/s; }
+  else { const double s = 2*sqrt(1 + E[8] - E[0] - E[4]); q[0] = (E[3] - E[1])/s; q[1] = (E[2] + E[6])/s; q[2] = (E[5] + E[7])/s; q[3] = 0.25*s; }
+  if (q[0] < 0) { q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3]; }
+  const double sn = sqrt(q[1]*q[1] + q[2]*q[2] + q[3]*q[3]), f = sn > 0 ? 2*atan2(sn, q[0])/sn : 2/q[0];
+  out[0] = f*q[1]; out[1] = f*q[2]; out[2] = f*q[3];
+}
+
+extern "C" __global__ void __launch_bounds__(320) myo_ik_kernel(const __grid_constant__ DevModel m, const __grid_constant__ IkArgs a) {
+  __shared__ __align__(8) unsigned long long mbar;
+  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  STAGE_MODEL(m, mbar)
+  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  const myo_ik_buffers& d = a.d; const int ns = a.p.nsite, nv = m.nv, np = m.nvp, lane = w.lane; const bool rot = d.target_quat != nullptr;
+  unsigned long long keep = ~0ull;      // dofs that may move
+  if (d.dof_mask) keep = (unsigned long long)__ballot_sync(FULL, lane < nv && d.dof_mask[lane]) | (unsigned long long)__ballot_sync(FULL, lane + 32 < nv && d.dof_mask[lane + 32]) << 32;
+  double* H = S_H; double* g = S_g; double* bx = S_a; double* by = S_Ma; double* bz = S_Mp;
+  const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr); const idx_t* lin = CI(PD_lin);
+  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
+  for (int jslot = wid; jslot < per_cta; jslot += nw) {
+    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, jslot - wid, wid);
+    if (env >= a.n_env) break;
+    const double* q0 = (d.qpos0 ? d.qpos0 : a.bound_qpos) + (size_t)env*m.nq; const double* ref = d.qpos_ref ? d.qpos_ref + (size_t)env*m.nq : q0;
+    for (int i = lane; i < m.nq; i += 32) W_(qpos)[i] = q0[i];
+    __syncwarp();
+    for (int it = 0; ; it++) {
+      phase_kinematics(m, w);
+      // site pose and errors (lane s)
+      double p[3] = {0, 0, 0}, R[9], e[3] = {0, 0, 0}, wv[3] = {0, 0, 0}, ep = 0, er = 0;
+      if (lane < ns) { const int k = a.site_body[lane]; const double* f = a.site_frame[lane]; double Rb[9];
+        if (k < 0) { for (int c = 0; c < 3; c++) p[c] = f[c]; for (int c = 0; c < 9; c++) Rb[c] = f[3+c]; }
+        else { const double* X = SCR(s_xmat) + 9*k; mat_vec(p, X, f); for (int c = 0; c < 3; c++) p[c] += SCR(s_xpos)[3*k+c]; for (int c = 0; c < 9; c++) Rb[c] = X[c]; }
+        { double S[9]; quat2mat(S, d.site_quat + 4*lane); mat_mul(R, Rb, S); }
+        const double* t = d.target_pos + ((size_t)env*ns + lane)*3;
+        for (int c = 0; c < 3; c++) e[c] = t[c] - p[c];
+        ep = sqrt(dot3(e, e));
+        if (rot) { const double* tq = d.target_quat + ((size_t)env*ns + lane)*4; double Q[4] = {tq[0], tq[1], tq[2], tq[3]}; quat_norm(Q); ik_rotvec(Q, R, wv); er = sqrt(dot3(wv, wv)); } }
+      const bool conv = __all_sync(FULL, lane >= ns || (ep <= a.p.tol && (!rot || er <= a.p.tol)));
+      if (conv || it == a.p.max_iter) {      // outputs at the returned q
+        for (int i = lane; i < m.nq; i += 32) d.qpos[(size_t)env*m.nq + i] = W_(qpos)[i];
+        if (lane == 0) { if (d.niter) d.niter[env] = it; if (d.converged) d.converged[env] = conv; }
+        if (lane < ns) { const size_t r = (size_t)env*ns + lane;
+          if (d.err) { d.err[2*r] = ep; d.err[2*r+1] = er; }
+          if (d.site_xpos) for (int c = 0; c < 3; c++) d.site_xpos[3*r + c] = p[c];
+          if (d.site_xmat) for (int c = 0; c < 9; c++) d.site_xmat[9*r + c] = R[c]; }
+        if (d.jacp || d.jacr) for (int s = 0; s < ns; s++) { const double ps[3] = {__shfl_sync(FULL, p[0], s), __shfl_sync(FULL, p[1], s), __shfl_sync(FULL, p[2], s)};
+          const size_t r = ((size_t)env*ns + s)*3;
+          for (int i = lane; i < nv; i += 32) { double jp[3] = {0, 0, 0}, jr[3] = {0, 0, 0};
+            if ((a.site_dofs[s] >> i) & 1) { dof_point_vel(m, w, i, ps, jp); if (!lin[i]) for (int c = 0; c < 3; c++) jr[c] = W_(dax)[3*i + c]; }
+            for (int c = 0; c < 3; c++) { if (d.jacp) d.jacp[(r + c)*nv + i] = jp[c]; if (d.jacr) d.jacr[(r + c)*nv + i] = jr[c]; } } }
+        __syncwarp();
+        break; }
+      // normal equations, site by site
+      double gi[2] = {0, 0};
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i < np) { for (int j = 0; j <= i; j++) H[TRI(i,j)] = 0; if (i >= nv) H[TRI(i,i)] = 1; } }
+      for (int s = 0; s < ns; s++) {
+        const double ps[3] = {__shfl_sync(FULL, p[0], s), __shfl_sync(FULL, p[1], s), __shfl_sync(FULL, p[2], s)};
+        const double es[3] = {__shfl_sync(FULL, e[0], s), __shfl_sync(FULL, e[1], s), __shfl_sync(FULL, e[2], s)};
+        const double ws[3] = {__shfl_sync(FULL, wv[0], s), __shfl_sync(FULL, wv[1], s), __shfl_sync(FULL, wv[2], s)};
+        const double wp = d.site_weight ? d.site_weight[2*s] : 1.0, wr = d.site_weight ? d.site_weight[2*s+1] : 1.0;
+        const unsigned long long mk = a.site_dofs[s];
+        double jp[2][3], jr[2][3];
+        #pragma unroll
+        for (int c = 0; c < 2; c++) { const int i = lane + 32*c; for (int k = 0; k < 3; k++) jp[c][k] = jr[c][k] = 0;
+          if (i < nv && ((mk >> i) & 1)) { dof_point_vel(m, w, i, ps, jp[c]); if (!lin[i]) for (int k = 0; k < 3; k++) jr[c][k] = W_(dax)[3*i + k]; }
+          gi[c] += wp*dot3(jp[c], es) + (rot ? wr*dot3(jr[c], ws) : 0.0); }
+        #pragma unroll 1
+        for (int pass = 0; pass < (rot ? 2 : 1); pass++) { const double wt = pass ? wr : wp;
+          #pragma unroll
+          for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i < nv) { const double* J = pass ? jr[c] : jp[c]; bx[i] = J[0]; by[i] = J[1]; bz[i] = J[2]; } }
+          __syncwarp();
+          #pragma unroll
+          for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i >= nv || !((mk >> i) & 1)) continue; const double* J = pass ? jr[c] : jp[c];
+            for (unsigned long long bits = mk & ((2ull << i) - 1); bits; bits &= bits - 1) { const int j = __ffsll((long long)bits) - 1;
+              H[TRI(i,j)] += wt*(J[0]*bx[j] + J[1]*by[j] + J[2]*bz[j]); } }
+          __syncwarp(); } }
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i < np) g[i] = i < nv ? gi[c] : 0.0; }
+      __syncwarp();
+      if (a.p.eq_weight != 0 && lane == 0) {      // joint equalities: row 1 at d1, -deriv at d2
+        const idx_t* eq = CI(PEQ); const double* eqd = CD(PEQ_d); const double we = a.p.eq_weight;
+        for (int k = 0; k < m.neq; k++) { const int q1 = eq[PEQ_ISTRIDE*k], d1 = eq[PEQ_ISTRIDE*k+1], q2 = eq[PEQ_ISTRIDE*k+2], d2 = eq[PEQ_ISTRIDE*k+3]; double deriv;
+          const double cpos = eq_residual(eqd + k*PEQ_STRIDE, W_(qpos), q1, q2, deriv);
+          H[TRI(d1,d1)] += we; g[d1] -= we*cpos;
+          if (q2 >= 0) { const double j2 = -deriv; H[TRI(d2,d2)] += we*j2*j2; H[d1 > d2 ? TRI(d1,d2) : TRI(d2,d1)] += we*j2; g[d2] -= we*j2*cpos; } } }
+      __syncwarp();
+      if (a.p.posture_weight != 0) { const double rho = a.p.posture_weight;      // hinge and slide dofs toward the reference
+        for (int j = lane; j < m.njnt; j += 32) if (jtype[j] == 2 || jtype[j] == 3) { const int da = jd[j], qa = jq[j]; H[TRI(da,da)] += rho; g[da] += rho*(ref[qa] - W_(qpos)[qa]); } }
+      __syncwarp();
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i >= nv) continue;
+        H[TRI(i,i)] += a.p.damping;
+        if (!((keep >> i) & 1)) { for (int j = 0; j < i; j++) H[TRI(i,j)] = 0; H[TRI(i,i)] = 1; g[i] = 0; }
+        else if (~keep) for (int j = 0; j < i; j++) if (!((keep >> j) & 1)) H[TRI(i,j)] = 0; }
+      __syncwarp();
+      chol_dense(H, nv, g, lane);
+      __syncwarp();
+      double ss = 0;
+      for (int i = lane; i < nv; i += 32) ss += g[i]*g[i];
+      const double nrm = sqrt(warp_sum(ss));
+      if (nrm > a.p.max_step) { const double sc = a.p.max_step/nrm; for (int i = lane; i < nv; i += 32) g[i] *= sc; }
+      __syncwarp();
+      integrate_pos(m, w, W_(qpos), g, 1.0);
+      __syncwarp();
+      { const idx_t* lim = CI(PLIM); const double* __restrict__ limd = GD(PLIM_d);
+        for (int l = lane; l < m.nlim; l += 32) { double* q = W_(qpos) + lim[2*l+1]; *q = clipd(*q, LDC(limd + l*PLIM_STRIDE), LDC(limd + l*PLIM_STRIDE + 1)); } }
+      __syncwarp();
+    }
+  }
+}
+
 // ================================================================== host side (C-ABI)
 static thread_local std::string g_err;
 static int fail(const std::string& s) { g_err = s; return -1; }
@@ -659,7 +796,8 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
   LaunchShape inv_shape; bool inv_ready;      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
   // rollout (myo_batch_rollout), set up by its first call: carry state [n, nq + 2 nv + na + 1] (qpos | qvel | act | warm start | time)
-  bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced; };
+  bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced;
+  LaunchShape ik_shape; bool ik_ready; };      // launch shape of myo_ik_kernel, set by the first myo_batch_ik
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1072,4 +1210,64 @@ extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int
     else myo_roll_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
     CUDA_OK(cudaGetLastError()); b->launches++; }
   return 0;
+}
+
+// Per-site kernel arguments of myo_batch_ik from the model blob: the site's program body, its ancestor dofs (the Jacobian's non-zero
+// columns) and its position in that body, or, on a static body, its world position and the body's world rotation (MuJoCo's pose chain)
+static int ik_sites(const myo_batch* b, const int32_t* sid, int ns, IkArgs& a) {
+  const int32_t* I = b->model->I.data(); const double* D = b->model->D.data();
+  const int nsite = MYO_DIM(I, MYO_DIM_nsite);
+  const int32_t *parent = MYO_ISEC(I, MYO_SEC_body_parentid), *dofadr = MYO_ISEC(I, MYO_SEC_body_dofadr), *dofnum = MYO_ISEC(I, MYO_SEC_body_dofnum);
+  const int32_t *sbody = MYO_ISEC(I, MYO_SEC_site_bodyid), *pbm = MYO_ISEC(I, MYO_SEC_PB_model_id);
+  const double *spos = MYO_DSEC(I, D, MYO_SEC_site_pos), *bpos = MYO_DSEC(I, D, MYO_SEC_body_pos), *bquat = MYO_DSEC(I, D, MYO_SEC_body_quat);
+  for (int s = 0; s < ns; s++) {
+    if (sid[s] < 0 || sid[s] >= nsite) return fail("myo_batch_ik: site id " + std::to_string(sid[s]) + " outside [0, nsite)");
+    const int body = sbody[sid[s]]; int k = -1;
+    for (int q = 0; q < b->dm.nbd; q++) if (pbm[q] == body) k = q;
+    unsigned long long mk = 0;
+    for (int bb = body; bb > 0; bb = parent[bb]) for (int i = dofadr[bb]; i < dofadr[bb] + dofnum[bb]; i++) mk |= 1ull << i;
+    double* f = a.site_frame[s]; const double* sp = spos + 3*sid[s];
+    for (int c = 0; c < 12; c++) f[c] = 0;
+    f[3] = f[7] = f[11] = 1;
+    if (k >= 0) for (int c = 0; c < 3; c++) f[c] = sp[c];
+    else {      // static body: xpos = xpos(parent) + xmat(parent) body_pos, xquat = xquat(parent) body_quat, from the world down
+      std::vector<int> chain; for (int bb = body; bb > 0; bb = parent[bb]) chain.push_back(bb);
+      double x[3] = {0, 0, 0}, q[4] = {1, 0, 0, 0}, R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+      for (int t = (int)chain.size() - 1; t >= 0; t--) { const int bb = chain[t]; const double* bp = bpos + 3*bb; const double* r = bquat + 4*bb;
+        for (int c = 0; c < 3; c++) x[c] += R[3*c]*bp[0] + R[3*c+1]*bp[1] + R[3*c+2]*bp[2];
+        const double n[4] = {q[0]*r[0]-q[1]*r[1]-q[2]*r[2]-q[3]*r[3], q[0]*r[1]+q[1]*r[0]+q[2]*r[3]-q[3]*r[2], q[0]*r[2]-q[1]*r[3]+q[2]*r[0]+q[3]*r[1], q[0]*r[3]+q[1]*r[2]-q[2]*r[1]+q[3]*r[0]};
+        const double nn = sqrt(n[0]*n[0] + n[1]*n[1] + n[2]*n[2] + n[3]*n[3]); for (int c = 0; c < 4; c++) q[c] = n[c]/nn;
+        const double w_ = q[0], x_ = q[1], y_ = q[2], z_ = q[3];
+        const double M[9] = {w_*w_+x_*x_-y_*y_-z_*z_, 2*(x_*y_-w_*z_), 2*(x_*z_+w_*y_), 2*(x_*y_+w_*z_), w_*w_-x_*x_+y_*y_-z_*z_, 2*(y_*z_-w_*x_), 2*(x_*z_-w_*y_), 2*(y_*z_+w_*x_), w_*w_-x_*x_-y_*y_+z_*z_};
+        for (int c = 0; c < 9; c++) R[c] = M[c]; }
+      for (int c = 0; c < 3; c++) f[c] = x[c] + R[3*c]*sp[0] + R[3*c+1]*sp[1] + R[3*c+2]*sp[2];
+      for (int c = 0; c < 9; c++) f[3+c] = R[c]; }
+    a.site_body[s] = k; a.site_dofs[s] = mk; }
+  return 0;
+}
+
+static_assert(sizeof(DevModel) + sizeof(IkArgs) <= 4096, "myo_ik_kernel's arguments fit the 4 KB kernel parameter space");
+
+extern "C" int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_params* p, void* stream) {
+  if (!b || !d || !p) return fail("myo_batch_ik: null");
+  if (!d->site_id || !d->site_quat || !d->target_pos || !d->qpos) return fail("myo_batch_ik: site_id, site_quat, target_pos and qpos are required");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  const int ns = p->nsite;
+  if (ns < 1 || ns > MYO_IK_MAXSITE) return fail("myo_batch_ik: nsite must be in [1, " + std::to_string(MYO_IK_MAXSITE) + "]");
+  if (!std::isfinite(p->tol) || !std::isfinite(p->damping) || !std::isfinite(p->max_step) || !std::isfinite(p->posture_weight) || !std::isfinite(p->eq_weight))
+    return fail("myo_batch_ik: non-finite parameter");
+  if (p->damping <= 0 || p->max_step <= 0 || p->tol < 0 || p->max_iter < 0 || p->posture_weight < 0 || p->eq_weight < 0)
+    return fail("myo_batch_ik: needs damping > 0, max_step > 0, tol >= 0, max_iter >= 0, posture_weight >= 0 and eq_weight >= 0");
+  if (b->dm.nv > 64) return fail("myo_batch_ik: models with more than 64 dofs are not supported");
+  CUDA_OK(cudaSetDevice(b->device));
+  int32_t sid[MYO_IK_MAXSITE]; cudaStream_t st = (cudaStream_t)stream;      // the site list decides the kernel arguments: read it back
+  CUDA_OK(cudaMemcpyAsync(sid, d->site_id, (size_t)ns*4, cudaMemcpyDeviceToHost, st)); CUDA_OK(cudaStreamSynchronize(st));
+  IkArgs a; memset(&a, 0, sizeof(a));
+  if (const int rc = ik_sites(b, sid, ns, a)) return rc;
+  if (!b->ik_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+    if (launch_shape((const void*)myo_ik_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->ik_shape)) return -1;
+    b->ik_ready = true; }
+  a.d = *d; a.p = *p; a.bound_qpos = b->bufs.qpos; a.n_env = b->n_env; const LaunchShape& s = b->ik_shape;
+  myo_ik_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

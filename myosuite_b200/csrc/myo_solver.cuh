@@ -115,6 +115,15 @@ __device__ void rows_applyT_add(const DevModel& m, const Warp w, double* wgt, do
 }
 
 // ------------------------------------------------------------------ constraint assembly
+// residual of joint equality record c (PEQ_d) at qpos: q1 - q1_0 - poly(q2 - q2_0), or q1 - q1_0 - c[0] without a second joint (q2 < 0);
+// deriv = d poly / d q2 (0 without a second joint), so that the row's Jacobian is 1 at d1 and -deriv at d2.  The same expressions as the
+// equality rows of phase_constraints below, which keeps its own inline copy: routing it through this helper reorders the step kernels'
+// machine code.
+__device__ __forceinline__ double eq_residual(const double* c, const double* qpos, int q1, int q2, double& deriv) {
+  const double pos0 = qpos[q1]-c[5];
+  if (q2 >= 0) { double x = qpos[q2]-c[6]; deriv = c[1]+x*(2*c[2]+x*(3*c[3]+x*4*c[4])); return pos0-(c[0]+x*(c[1]+x*(c[2]+x*(c[3]+x*c[4])))); }
+  deriv = 0; return pos0-c[0]; }
+
 __device__ void phase_constraints(const DevModel& m, const Warp w) {
   // joint equalities (always active)
   const idx_t* eq = CI(PEQ); const double* eqd = CD(PEQ_d);
@@ -497,6 +506,20 @@ __device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, dou
 }
 
 // ------------------------------------------------------------------ semi-implicit Euler with implicit joint damping
+// qpos <- qpos (+) h v (mj_integratePos): hinge and slide joints add; a free joint adds the position and turns its quaternion by
+// exp(h omega / 2) in the body frame, then normalises it.  Lanes over the joints; the caller syncs.  phase_integrate keeps its own
+// inline copy of this loop over qpos / qvel, for the same reason as phase_constraints' equality rows.
+__device__ __forceinline__ void integrate_pos(const DevModel& m, const Warp w, double* qpos, const double* v, double h) {
+  const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr);
+  for (int j = w.lane; j < m.njnt; j += 32) { int qa = jq[j], da = jd[j];
+    if (jtype[j] == 0) { for (int c = 0; c < 3; c++) qpos[qa+c] += h*v[da+c];
+      double wv[3] = {v[da+3], v[da+4], v[da+5]}, nn = sqrt(dot3(wv,wv)), ang = h*nn;
+      if (nn < MYO_MINVAL) { wv[0]=1; wv[1]=0; wv[2]=0; } else { wv[0]/=nn; wv[1]/=nn; wv[2]/=nn; }
+      double sn, cs; sincos(0.5*ang, &sn, &cs); double ql[4] = {cs, wv[0]*sn, wv[1]*sn, wv[2]*sn}, qn[4]; quat_mul(qn, qpos+qa+3, ql); quat_norm(qn);
+      for (int c = 0; c < 4; c++) qpos[qa+3+c] = qn[c]; }
+    else qpos[qa] += h*v[da]; }
+}
+
 __device__ void phase_integrate(const DevModel& m, const Warp w, long long* cyc) {
   int n = m.nv; double h = m.timestep; long long tc = cyc ? clock64() : 0;
   // (M + h B) qacc' = M qacc  (= qfrc_smooth + qfrc_constraint at the solver optimum)

@@ -422,6 +422,82 @@ class MyoVecEnv:
         self.batch.rollout(nstep, substeps, stream=self._stream(), **bufs, **out)
         return out
 
+    IK_FIELDS = tuple(abi.IK_SHAPES)
+    # defaults of ik(): tol in metres and radians; at these, targets from forward kinematics of random in-range configurations are
+    # reached from init_qpos at the rates DESIGN.md section 2 lists
+    IK_DEFAULTS = dict(max_iter=200, tol=1e-6, damping=1e-3, max_step=0.5, posture=0.0, eq_weight=1.0)
+
+    def ik(self, sites, target_pos, target_quat=None, qpos_init=None, qpos_ref=None, dofs=None, site_weight=None,
+           max_iter=IK_DEFAULTS["max_iter"], tol=IK_DEFAULTS["tol"], damping=IK_DEFAULTS["damping"], max_step=IK_DEFAULTS["max_step"],
+           posture=IK_DEFAULTS["posture"], eq_weight=IK_DEFAULTS["eq_weight"], fields=("qpos", "niter", "converged", "err")):
+        """Damped least-squares inverse kinematics of every env (myo_batch_ik; include/myo_b200.h states the iteration): sites (names or
+        ids, 1..16 of them) toward target_pos [num_envs, ns, 3] and, when given, target_quat [num_envs, ns, 4] (w x y z), from qpos_init
+        [num_envs, nq] (None: the current qpos), with the posture term pulling hinge and slide joints toward qpos_ref [num_envs, nq] (None:
+        the start) at weight `posture`, the joint equalities at weight eq_weight and per-site (position, orientation) weights site_weight
+        [ns, 2].  dofs: joint names or a bool mask [nv] of the dofs that may move (None: all).  Joint limits hold by clamping after each
+        step.  Tensors are contiguous float64 CUDA tensors on this batch's device.  Returns {field: tensor [num_envs, ...]} of IK_FIELDS:
+        qpos, niter, converged (int32), err [ns, 2] (|position error|, |rotation error|), site_xpos [ns, 3], site_xmat [ns, 9],
+        jacp / jacr [ns, 3, nv], all at the returned qpos; allocated per call.  One launch; not a state change (adopt a solution with
+        set_state(qpos=...)).  A trajectory of T frames is one call on a batch of T envs."""
+        torch, m, n = self.torch, self.mj_model, self.num_envs
+        fields = tuple(fields)
+        bad = [f for f in fields if f not in self.IK_FIELDS]
+        if bad:
+            raise KeyError("unknown ik fields %s (available: %s)" % (bad, list(self.IK_FIELDS)))
+        sid = [m.name2id("site", x) if isinstance(x, str) else int(x) for x in ([sites] if isinstance(sites, (str, int)) else sites)]
+        ns = len(sid)
+        if not 1 <= ns <= abi.IK_MAXSITE or any(not 0 <= x < m.nsite for x in sid):
+            raise ValueError("sites must be 1..%d site names or ids in [0, %d), got %s" % (abi.IK_MAXSITE, m.nsite, sites))
+
+        def check(name, x, shape):
+            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
+                    or not x.is_contiguous()):
+                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
+                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
+                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+        check("target_pos", target_pos, (n, ns, 3))
+        bufs = {"target_pos": target_pos}
+        for name, x, shape in (("target_quat", target_quat, (n, ns, 4)), ("qpos0", qpos_init, (n, m.nq)), ("qpos_ref", qpos_ref, (n, m.nq)),
+                               ("site_weight", site_weight, (ns, 2))):
+            if x is not None:
+                check("qpos_init" if name == "qpos0" else name, x, shape)
+                bufs[name] = x
+        if dofs is not None:
+            if isinstance(dofs, torch.Tensor) or isinstance(dofs, np.ndarray):
+                mask = np.asarray(dofs.cpu() if isinstance(dofs, torch.Tensor) else dofs)
+                if mask.dtype != np.bool_ or mask.shape != (m.nv,):
+                    raise ValueError("dofs must be joint names or a bool mask of shape (%d,), got %s %s" % (m.nv, mask.dtype, mask.shape))
+            else:
+                mask = np.zeros(m.nv, bool)
+                for j in [m.name2id("joint", x) for x in ([dofs] if isinstance(dofs, str) else dofs)]:
+                    nd = {0: 6, 1: 3}.get(int(m.jnt_type[j]), 1)
+                    mask[m.jnt_dofadr[j]:m.jnt_dofadr[j] + nd] = True
+            bufs["dof_mask"] = torch.as_tensor(mask.astype(np.uint8), device=self.device)
+        params = abi.MyoIkParams(nsite=ns, max_iter=int(max_iter), tol=float(tol), damping=float(damping), max_step=float(max_step),
+                                 posture_weight=float(posture), eq_weight=float(eq_weight))
+        if not (params.max_iter >= 0 and params.tol >= 0 and params.damping > 0 and params.max_step > 0 and params.posture_weight >= 0
+                and params.eq_weight >= 0 and np.all(np.isfinite([tol, damping, max_step, posture, eq_weight]))):
+            raise ValueError("ik needs max_iter >= 0, tol >= 0, damping > 0, max_step > 0, posture >= 0 and eq_weight >= 0, all finite")
+        bufs["site_id"] = torch.as_tensor(np.asarray(sid, np.int32), device=self.device)
+        bufs["site_quat"] = torch.as_tensor(np.ascontiguousarray(m.site_quat[sid], dtype=np.float64), device=self.device)
+        size = dict(nq=m.nq, nv=m.nv, ns=ns)
+        out = {}
+        for f in set(fields) | {"qpos"}:
+            shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in abi.IK_SHAPES[f])
+            out[f] = (torch.full(shape, -1, dtype=torch.int32, device=self.device) if f in ("niter", "converged")
+                      else torch.full(shape, float("nan"), dtype=torch.float64, device=self.device))
+        self.batch.ik(params, stream=self._stream(), **bufs, **out)
+        return {f: out[f] for f in fields}
+
+    def jac_site(self, sites, qpos=None):
+        """mj_jacSite of every env: (jacp, jacr [num_envs, ns, 3, nv], site_xpos [num_envs, ns, 3], site_xmat [num_envs, ns, 9]) at qpos
+        [num_envs, nq] (None: the current qpos).  The same launch as ik() with max_iter = 0."""
+        n = self.num_envs
+        ns = 1 if isinstance(sites, (str, int)) else len(sites)
+        r = self.ik(sites, self.torch.zeros((n, ns, 3), dtype=self.torch.float64, device=self.device), qpos_init=qpos, max_iter=0,
+                    fields=("jacp", "jacr", "site_xpos", "site_xmat"))
+        return r["jacp"], r["jacr"], r["site_xpos"], r["site_xmat"]
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -611,6 +687,23 @@ class MyoEnv:
             res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
         res["overflow"] = int(res["overflow"])
         return res
+
+    def mj_ik(self, sites, target_pos, target_quat=None, qpos_init=None, qpos_ref=None, dofs=None, site_weight=None,
+              fields=("qpos", "niter", "converged", "err"), **params):
+        """Inverse kinematics of this env (MyoVecEnv.ik): target_pos [ns, 3], target_quat [ns, 4] or None, qpos_init / qpos_ref [nq] or
+        None, dofs and site_weight as there; params: max_iter, tol, damping, max_step, posture, eq_weight.  Returns {field: numpy array}
+        (niter and converged as ints).  Not a state change.  One device-to-host copy per field."""
+        v = self.vec
+        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        ns = 1 if isinstance(sites, (str, int)) else len(sites)
+        out = v.ik(sites, as_dev(target_pos, (1, ns, 3)), target_quat=as_dev(target_quat, (1, ns, 4)), qpos_init=as_dev(qpos_init, (1, -1)),
+                   qpos_ref=as_dev(qpos_ref, (1, -1)), dofs=dofs, site_weight=as_dev(site_weight, (ns, 2)), fields=fields, **params)
+        return {k: (int(x[0]) if k in ("niter", "converged") else x[0].cpu().numpy()) for k, x in out.items()}
+
+    def mj_jacSite(self, site):
+        """mujoco.mj_jacSite at the current state: (jacp [3, nv], jacr [3, nv]) as numpy arrays."""
+        jp, jr, _, _ = self.vec.jac_site([site])
+        return jp[0, 0].cpu().numpy(), jr[0, 0].cpu().numpy()
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)
     def get_obs_dict(self, *sim_args):

@@ -7,7 +7,13 @@ For each case: warm-up steps from a reset, then `reps` rounds that each time one
 dynamics, all fields), the inverse of the readout's qacc (with constraints, without them, with every output) and two rollouts from the
 current state with CUDA events on the batch's stream, in alternating order.  The rollouts: "rollout", 8 intervals of frame_skip substeps,
 reported per interval (the physics of one env step); "rollout_1", frame_skip intervals of one substep, reported per call (the same physics).  Prints medians (and min / max) in microseconds and the
-GPU name, power limit and SM clock read through nvidia-smi's query interface (read-only).  Writes nothing unless --out is given."""
+GPU name, power limit and SM clock read through nvidia-smi's query interface (read-only).  Writes nothing unless --out is given.
+
+The "ik" case (MyoVecEnv.ik, myo_batch_ik): the hand, 4096 envs, the five fingertip sites, targets from forward kinematics of random
+in-range configurations, start at qpos0, in alternating order with one env step: "ik" at the default parameters (per call, with the mean
+and largest number of iterations), "ik_10" (tol = 0, max_iter = 10: every env runs 10 iterations) and "jac_site" (max_iter = 0).  Per
+iteration = (ik_10 - jac_site) / 10.  Beside them, the C reference (tests/ik_oracle.c, oracle_ik) at the same defaults on one host core
+for the first --ref-envs targets.  --cases selects cases by name."""
 import argparse
 import json
 import os
@@ -26,6 +32,7 @@ GROUPS = {"pose": ("xpos", "xquat", "xmat", "site_xpos"),
 INVERSE = {"inverse": dict(fields=("qfrc_inverse",)), "inverse_free": dict(constraints=False, fields=("qfrc_inverse",)),
            "inverse_all": dict(fields=("qfrc_inverse", "qfrc_constraint", "contact_force", "actuator_moment"))}
 ROLLOUT_NSTEP = 8           # intervals of the "rollout" row
+IK_ENV, IK_N, IK_SITES = "myoHandPoseRandom-v0", 4096, ("THtip", "IFtip", "MFtip", "RFtip", "LFtip")
 
 
 def gpu_info():
@@ -37,6 +44,75 @@ def gpu_info():
         return ["unknown (%s)" % e]
 
 
+def _timed(stream, fn):
+    import torch
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    fn()
+    e1.record(stream)
+    e1.synchronize()
+    return e0.elapsed_time(e1) * 1e3
+
+
+def ik_case(args):
+    """one IK call, one iteration and jac_site beside one env step on the hand; the C reference on one host core"""
+    import time
+    import numpy as np
+    import torch
+    from myosuite_b200 import blob, program, vec_env
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from ik_oracle import IkOracle
+    env = vec_env.MyoVecEnv(IK_ENV, IK_N, seed=0)
+    m, n = env.mj_model, IK_N
+    env.reset(seed=0)
+    stream = torch.cuda.current_stream(env.device)
+    g = torch.Generator(device="cpu").manual_seed(0)
+    acts = [(torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device) for _ in range(8)]
+    sites = [m.name2id("site", x) for x in IK_SITES]
+    rng = np.random.default_rng(0)
+    qt = np.tile(m.qpos0, (n, 1))
+    for j in range(m.njnt):
+        if m.jnt_type[j] in (2, 3) and m.jnt_limited[j]:
+            qt[:, m.jnt_qposadr[j]] = rng.uniform(*m.jnt_range[j], n)
+    dev = lambda x: torch.as_tensor(np.ascontiguousarray(x), dtype=torch.float64, device=env.device)
+    q0 = dev(np.tile(m.qpos0, (n, 1)))
+    tp = env.jac_site(sites, qpos=dev(qt))[2].contiguous()
+    calls = {"step": lambda k: env.step(acts[k % 8]), "ik": lambda k: env.ik(sites, tp, qpos_init=q0),
+             "ik_10": lambda k: env.ik(sites, tp, qpos_init=q0, max_iter=10, tol=0.0), "jac_site": lambda k: env.jac_site(sites, qpos=q0)}
+    for k in range(args.warmup):
+        for f in calls.values():
+            f(k)
+    torch.cuda.synchronize()
+    order = list(calls)
+    t = {k: [] for k in order}
+    for r in range(args.reps):
+        for k in (order if r % 2 == 0 else order[::-1]):
+            t[k].append(_timed(stream, lambda: calls[k](r)))
+    s = {k: dict(median_us=float(np.median(v)), min_us=float(np.min(v)), max_us=float(np.max(v))) for k, v in t.items()}
+    it = env.ik(sites, tp, qpos_init=q0, fields=("niter", "converged"))
+    niter = it["niter"].cpu().numpy()
+    s["ik"].update(mean_iter=float(niter.mean()), max_iter=int(niter.max()), converged=float(it["converged"].float().mean()))
+    s["per_iteration_us"] = (s["ik_10"]["median_us"] - s["jac_site"]["median_us"]) / 10
+    for k in order[1:]:
+        s[k]["per_step"] = s[k]["median_us"] / s["step"]["median_us"]
+    # the C reference on one host core, same targets and defaults
+    prog, _ = program.build_program(m)
+    I, D = blob.pack(m, prog)
+    o = IkOracle(I, D, m.site_quat)
+    TP = tp.cpu().numpy()
+    t0, iters = time.perf_counter(), 0
+    for e in range(args.ref_envs):
+        iters += o.ik(sites, TP[e], m.qpos0)["niter"]
+    dt = time.perf_counter() - t0
+    s["c_reference"] = dict(envs=args.ref_envs, us_per_call=dt / args.ref_envs * 1e6, us_per_iteration=dt / max(iters, 1) * 1e6)
+    print("ik            n %4d  step %8.1f us | ik %8.1f us (%.3f step; iterations mean %.1f, max %d, converged %.4f) | ik_10 %8.1f us | "
+          "jac_site %7.1f us (%.3f step) | per iteration %6.1f us | C reference, one core: %.0f us per env call, %.1f us per iteration"
+          % (n, s["step"]["median_us"], s["ik"]["median_us"], s["ik"]["per_step"], s["ik"]["mean_iter"], s["ik"]["max_iter"], s["ik"]["converged"],
+             s["ik_10"]["median_us"], s["jac_site"]["median_us"], s["jac_site"]["per_step"], s["per_iteration_us"],
+             s["c_reference"]["us_per_call"], s["c_reference"]["us_per_iteration"]), flush=True)
+    return dict(env_id=IK_ENV, n_env=n, sites=list(IK_SITES), **s)
+
+
 def main():
     import numpy as np
     import torch
@@ -45,9 +121,14 @@ def main():
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--cases", default=",".join([c[0] for c in CASES] + ["ik"]))
+    ap.add_argument("--ref-envs", type=int, default=64)
     args = ap.parse_args()
+    want = set(args.cases.split(","))
     res = {"gpu_before": gpu_info(), "cases": {}}
     for name, eid, n in CASES:
+        if name not in want:
+            continue
         env = vec_env.MyoVecEnv(eid, n, seed=0)
         m = env.mj_model
         env.reset(seed=0)
@@ -93,6 +174,8 @@ def main():
               + "  ".join("%s %7.1f us (%.3f step)" % (k, s[k]["median_us"], s[k]["per_step"]) for k in order[1:]), flush=True)
         del env
         torch.cuda.empty_cache()
+    if "ik" in want:
+        res["cases"]["ik"] = ik_case(args)
     res["gpu_after"] = gpu_info()
     print("GPU [name, power limit, SM clock, max SM clock, throttle reasons] before: %s after: %s" % (res["gpu_before"], res["gpu_after"]))
     if args.out:
