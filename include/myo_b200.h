@@ -219,6 +219,34 @@ typedef struct {
   double tol, damping, max_step, posture_weight, eq_weight;
 } myo_ik_params;
 
+/* Caller-owned device buffers of myo_batch_transition_fd: MuJoCo's mjd_transitionFD (mjd_stepFD) with one mj_step replaced by one interval
+ * of `substeps` mj_steps with ctrl held, x' ~ x'0 + A dx + B du.
+ *   State: x = [dq (nv, the tangent space of mj_integratePos / mj_differentiatePos), qvel (nv), act (na)], nx = 2 nv + na; time is not
+ *     part of it.
+ *   Nominal: x'0 is one interval from the start state with ctrl and qfrc_applied, bit-identical to myo_batch_rollout with nstep = 1 and
+ *     the same substeps from the same start.
+ *   Warm start: every perturbed interval starts from the same start state with the start's qacc_warmstart (mjd_stepFD restores the warm
+ *     start before each perturbation); its inverse-wrap roots start cold, as every rollout interval's do.
+ *   Perturbations: qpos column j: mj_integratePos(qpos, e_j, +-eps); qvel column j: qvel[j] +- eps; act column j: act[j] +- eps
+ *     (unclamped); ctrl column i: ctrl[i] +- eps, where with actuator_ctrllimited fwd = inRange(ctrl, ctrl + eps) and
+ *     back = (centered || !fwd) && inRange(ctrl - eps, ctrl) (without the limit both are possible); state columns always go forward and
+ *     go back when centered.
+ *   Differences: both sides (x'+ (-) x'-) * (1 / (2 eps)); forward only (x'+ (-) x'0) * (1 / eps); back only (x'0 (-) x'-) * (1 / eps);
+ *     neither 0.  (-) is mj_differentiatePos (dt = 1) on the qpos part and subtraction on the rest; 1 / eps and 1 / (2 eps) are the
+ *     IEEE-rounded reciprocals, as mjd_stepFD's mju_scl(ds, ds, 1/h) has them. */
+typedef struct {
+  const double* ctrl;            /* [n, nu] in, required: MuJoCo ctrl, held for the substeps (clipped to ctrlrange inside the step, like rollout) */
+  const double* qfrc_applied;    /* [n, nv] nullable (zero) */
+  const double* qpos0;           /* [n, nq] start state, nullable field by field (bound buffers), as myo_rollout_buffers */
+  const double* qvel0;           /* [n, nv] */
+  const double* act0;            /* [n, na] */
+  const double* qacc_warmstart0; /* [n, nv] */
+  double* A;                     /* [n, nx, nx] out, nullable; nx = 2 nv + na, row-major, A[i][j] = d x'_i / d x_j */
+  double* B;                     /* [n, nx, nu] out, nullable (at least one of A, B) */
+  int32_t* overflow;             /* [n] out, nullable: set when any substep of any of the env's perturbed or nominal steps dropped contacts */
+} myo_fd_buffers;
+typedef struct { double eps; int32_t centered, substeps; } myo_fd_params;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -301,6 +329,14 @@ int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int
  * max_step <= 0, tol < 0, max_iter < 0 or a non-finite parameter.  Replaces mj_jacSite and the mink / dm_control IK loops over it
  * (MyoSuite tutorial 8_inverse_kinematics, marker and fingertip retargeting). */
 int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_params* p, void* stream);
+
+/* Finite-difference transition Jacobians of every env (myo_fd_buffers, myo_fd_params): a nominal rollout interval, then one launch that
+ * runs every (env, column) pair as its own warp, both on `stream`.  The per-env overrides (env_prm) apply; fatigue, the task layer and
+ * auto-reset do not run.  No bound buffer is written: the call advances nothing.  With the iterative solver the columns carry solver noise
+ * of order solver tolerance / eps, as in MuJoCo.  Fails before any launch on a null batch, buffers, params or ctrl, A and B both null, an
+ * unbound batch, eps not finite or not > 0, substeps < 1 or centered not in {0, 1}.  Replaces mujoco.mjd_transitionFD (iLQR / DDP, LQR
+ * about a reference pose, MPC warm starts, controllability and sensitivity studies). */
+int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, const myo_fd_params* p, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

@@ -98,11 +98,24 @@ class MyoIkParams(ctypes.Structure):
     _fields_ = [("nsite", c_i32), ("max_iter", c_i32)] + [(n, c_f64) for n in ("tol", "damping", "max_step", "posture_weight", "eq_weight")]
 
 
+# myo_fd_buffers / myo_fd_params (include/myo_b200.h): finite-difference transition Jacobians of myo_batch_transition_fd.  Inputs, start
+# state, then the outputs (A [n, nx, nx], B [n, nx, nu], overflow [n] int32; nx = 2 nv + na)
+FD_FIELDS = ["ctrl", "qfrc_applied", "qpos0", "qvel0", "act0", "qacc_warmstart0", "A", "B", "overflow"]
+
+
+class MyoFdBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in FD_FIELDS]
+
+
+class MyoFdParams(ctypes.Structure):
+    _fields_ = [("eps", c_f64), ("centered", c_i32), ("substeps", c_i32)]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
            "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout",
-           "myo_batch_ik"]
+           "myo_batch_ik", "myo_batch_transition_fd"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -163,6 +176,7 @@ def _bind(L):
     L.myo_batch_inverse.argtypes = [c_vp, ctypes.POINTER(MyoInverseBuffers), ctypes.c_int, c_vp]
     L.myo_batch_rollout.argtypes = [c_vp, ctypes.POINTER(MyoRolloutBuffers), ctypes.c_int, ctypes.c_int, c_vp]
     L.myo_batch_ik.argtypes = [c_vp, ctypes.POINTER(MyoIkBuffers), ctypes.POINTER(MyoIkParams), c_vp]
+    L.myo_batch_transition_fd.argtypes = [c_vp, ctypes.POINTER(MyoFdBuffers), ctypes.POINTER(MyoFdParams), c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -314,6 +328,20 @@ class Batch:
                 raise ValueError("%s must be contiguous" % k)
             setattr(d, k, t.data_ptr())
         _check(self.L.myo_batch_ik(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
+
+    def transition_fd(self, params, stream=None, **tensors):
+        """Finite-difference transition Jacobians (myo_batch_transition_fd) with the given torch CUDA tensors (names of FD_FIELDS: ctrl
+        [n, nu] and at least one of A, B are required) and a MyoFdParams."""
+        d = MyoFdBuffers()
+        for k, t in tensors.items():
+            if k not in FD_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_transition_fd(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
 
     @property
     def launches(self):

@@ -12,6 +12,14 @@
 // ------------------------------------------------------------------ kernel arguments
 #define MYO_BMASK 0x40      /* phases of the product kernels that start with a CTA barrier (bit k = phase k).  0x40: only the solver entry, whose inner
                                barriers need aligned warps anyway; with load-sorted rounds the warps of a CTA stay close without the other phase barriers. */
+// Transition-FD kernel (myo_batch_transition_fd): work item k = env * ncol + column; columns [0, nxa) are A's (state), the rest B's (ctrl)
+struct FdArgs {
+  double* A; double* B;         // the caller's outputs [n, nx, nx] / [n, nx, nu] (nullable)
+  const double* nom;            // nominal interval's result: the rollout carry, blocks qpos [n, nq] | qvel [n, nv] | act [n, na]
+  double* rows;                 // per-slot rows (slot = CTA * warps + warp): perturbed ctrl [nu], then the + pass's qpos | qvel | act
+  double eps, rinv1, rinv2;     // eps, 1 / eps and 1 / (2 eps), IEEE-rounded on the host
+  int n_env, ncol, nxa, npass;  // npass: 2 when centered (+ pass, then - pass), else 1
+};
 struct StepArgs {
   myo_buffers b; myo_task_cfg cfg;
   int n_env, obs_dim, mode;     // mode 0: env step ; 1: debug forward (ctrl verbatim, optional substeps) ; 2: reset only
@@ -27,6 +35,7 @@ struct StepArgs {
   double tol, dt;
   myo_rollout_buffers roll;     // rollout kernels: the caller's ctrl / qfrc_applied and output rows (b points the state at the carry)
   int roll_t, roll_nstep;       // rollout kernels: the interval this launch runs, of how many
+  FdArgs fd;                    // transition-FD kernel
 };
 static const int LOAD_WN = 2, LOAD_WI = 3;      // the load key's weights (StepArgs.load_wn / load_wi) for the product kernels' env steps
 
@@ -283,14 +292,77 @@ __device__ __forceinline__ void load_env_state(const DevModel& m, const Warp w, 
   __syncwarp();
 }
 
+// ------------------------------------------------------------------ transition FD (myo_batch_transition_fd), per work item
+// The sides a column is perturbed to (mjd_stepFD): a state column always goes forward and goes back when centered; a ctrl column of an
+// actuator with ctrllimited goes forward when inRange(c, c + eps) and back when (centered || !fwd) && inRange(c - eps, c).
+struct FdCol { int col, ctrl; bool fwd, back; };      // ctrl: the actuator of a B column, -1 for an A column
+__device__ __forceinline__ FdCol fd_column(const DevModel& m, const StepArgs& a, int env, int col) {
+  const bool centered = a.fd.npass == 2;
+  FdCol c; c.col = col; c.ctrl = col < a.fd.nxa ? -1 : col - a.fd.nxa; c.fwd = true; c.back = centered;
+  if (c.ctrl >= 0) { const double* __restrict__ pa = GD(PA_d) + CI(PA_cls)[c.ctrl]*PA_STRIDE;
+    if (LDC(pa + 15) != 0) { const double lo = LDC(pa + 13), hi = LDC(pa + 14), x = a.roll.ctrl[(size_t)env*m.nu + c.ctrl], e = a.fd.eps;
+      c.fwd = x >= lo && x <= hi && x + e >= lo && x + e <= hi;
+      c.back = (centered || !c.fwd) && x - e >= lo && x - e <= hi && x >= lo && x <= hi; } }
+  return c; }
+// Pass p of a column runs the - side when centered and p = 1, or when it cannot go forward; it runs at all when that side is possible
+__device__ __forceinline__ bool fd_minus(const StepArgs& a, const FdCol& c, int pass) { return a.fd.npass == 2 ? pass == 1 : !c.fwd; }
+__device__ __forceinline__ bool fd_runs(const StepArgs& a, const FdCol& c, int pass) { return fd_minus(a, c, pass) ? c.back : c.fwd; }
+
+// The perturbation of the start state already in the slice (load_env_state); a ctrl column's ctrl row goes to the slot's global row
+__device__ void fd_perturb(const DevModel& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, double* ctrl_row) {
+  const double h = fd_minus(a, c, pass) ? -a.fd.eps : a.fd.eps;
+  if (c.ctrl >= 0) { const double* src = a.roll.ctrl + (size_t)env*m.nu;
+    for (int i = w.lane; i < m.nu; i += 32) ctrl_row[i] = i == c.ctrl ? src[i] + h : src[i]; }
+  else if (c.col < m.nv) {      // mj_integratePos(qpos, e_j, h), through the Newton gradient's scratch (dead until the solve)
+    for (int i = w.lane; i < m.nv; i += 32) S_g[i] = i == c.col ? 1.0 : 0.0;
+    __syncwarp();
+    integrate_pos(m, w, W_(qpos), S_g, h); }
+  else if (w.lane == 0) { if (c.col < 2*m.nv) W_(qvel)[c.col - m.nv] += h; else W_(act)[c.col - 2*m.nv] += h; }
+  __syncwarp();
+}
+
+// After a pass: the + pass of a centred column parks its result in the slot's row; the last pass writes the column of A or B
+//   both sides (x'+ (-) x'-) * rinv2, forward only (x'+ (-) x'0) * rinv1, back only (x'0 (-) x'-) * rinv1, neither 0
+// ((-): differentiate_pos on qpos, subtraction on qvel and act; x'0 from the nominal carry, the last pass's result in the slice).
+__device__ void fd_store(const DevModel& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, bool ran, double* prow) {
+  const int nq = m.nq, nv = m.nv, na = m.na, nx = 2*nv + na; const bool centered = a.fd.npass == 2;
+  if (centered && pass == 0) {
+    if (ran) { for (int i = w.lane; i < nq; i += 32) prow[i] = W_(qpos)[i];
+      for (int i = w.lane; i < nv; i += 32) prow[nq+i] = W_(qvel)[i];
+      for (int i = w.lane; i < na; i += 32) prow[nq+nv+i] = W_(act)[i]; }
+    __syncwarp(); return; }
+  const size_t n = a.fd.n_env;
+  const double *nq0 = a.fd.nom + (size_t)env*nq, *nv0 = a.fd.nom + n*nq + (size_t)env*nv, *na0 = a.fd.nom + n*(nq + nv) + (size_t)env*na;
+  const double *sq = W_(qpos), *sv = W_(qvel), *sa = W_(act);
+  const double *pq = centered ? prow : sq, *pv = centered ? prow + nq : sv, *pa = centered ? prow + nq + nv : sa;      // the + result
+  const double *q1 = nullptr, *v1 = nullptr, *a1 = nullptr, *q2 = nullptr, *v2 = nullptr, *a2 = nullptr; double r = 0;
+  if (c.fwd && c.back) { q1 = sq; v1 = sv; a1 = sa; q2 = pq; v2 = pv; a2 = pa; r = a.fd.rinv2; }      // (both sides only when centered)
+  else if (c.fwd) { q1 = nq0; v1 = nv0; a1 = na0; q2 = pq; v2 = pv; a2 = pa; r = a.fd.rinv1; }
+  else if (c.back) { q1 = sq; v1 = sv; a1 = sa; q2 = nq0; v2 = nv0; a2 = na0; r = a.fd.rinv1; }
+  double* out; size_t st;
+  if (c.ctrl < 0) { out = a.fd.A + (size_t)env*nx*nx + c.col; st = nx; } else { out = a.fd.B + (size_t)env*nx*m.nu + c.ctrl; st = m.nu; }
+  if (!q1) { for (int i = w.lane; i < nx; i += 32) out[i*st] = 0.0; }
+  else { differentiate_pos(m, w, S_g, q1, q2);
+    __syncwarp();
+    for (int i = w.lane; i < nv; i += 32) out[i*st] = S_g[i]*r;
+    for (int i = w.lane; i < nv; i += 32) out[(nv+i)*st] = (v2[i] - v1[i])*r;
+    for (int i = w.lane; i < na; i += 32) out[(2*nv+i)*st] = (a2[i] - a1[i])*r; }
+  __syncwarp();
+}
+
 // ------------------------------------------------------------------ the kernel
 // DBG = false: the product step / reset / observe kernel (modes 0, 2, 3): no parity taps, no cycle counters, fixed barrier scheme.
 // DBG = true: everything -- forward-debug mode (1), parity taps, per-phase cycle counters, the barrier / lockstep-group tuning knobs.
 // ROLL = true: the rollout kernels (myo_batch_rollout), mode 0 only: one interval of a.roll with the caller's ctrl row (m.g_ctrl is neither
 // read nor written) and qfrc_applied added to qfrc_smooth; the launch's cfg has no task, fatigue or reafferentation, and its state
 // buffers are the library's carry, which is also copied into the output rows of the interval.
+// FD = true (with ROLL): the transition-FD kernel (myo_batch_transition_fd).  Its slots are the work items (env, column) of a.fd on the
+// contiguous map, so that the warps of a round are neighbouring columns of one env; a.n_env counts the items.  Each item runs a.fd.npass
+// consecutive rounds (the + and the - pass when centred), so every warp of every CTA walks the same rounds and solver barriers; a pass
+// whose side the column does not take runs as an idle slot (live = false).  A pass loads the env's start state from a.b, perturbs it
+// (fd_perturb) and, after the substeps, parks or differences its result (fd_store); no state is stored back.
 // MAXT: launch bound (threads per CTA) -> register budget of the instantiation.
-template <bool DBG, int MAXT, bool ROLL = false>
+template <bool DBG, int MAXT, bool ROLL = false, bool FD = false>
 __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArgs& a) {
   __shared__ __align__(8) unsigned long long mbar;
   const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -307,12 +379,18 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
   // With a.perm (big models, env steps of the product kernels) the slot -> env map is the load-sorted one: the envs of a round carry
   // similar contact loads, so the lockstep barriers wait for a slowest env that is close to the average one.
   const bool regrouped = !DBG && a.perm != nullptr;
-  const int per_cta = regrouped ? a.perm_rounds*nw : SLOTS_PER_CTA(a.balanced, a.n_env, (int)gridDim.x, nw);
+  const int per_cta = regrouped ? a.perm_rounds*nw : SLOTS_PER_CTA(a.balanced, a.n_env, (int)gridDim.x, nw)*(FD ? a.fd.npass : 1);
   for (int j0 = 0; j0 < per_cta; j0 += nw) {
-    const int env = regrouped ? a.perm[(int)blockIdx.x + (int)gridDim.x*(j0 + wid)] : slot_env(a.balanced, (int)blockIdx.x, (int)gridDim.x, nw, j0, wid);
-    const bool live = (j0 + wid) < per_cta && env >= 0 && env < a.n_env; const long long tstep_ = prof ? clock64() : 0; int load_acc = 0;
+    const int pass = FD ? j0/nw % a.fd.npass : 0;
+    const int slot = regrouped ? a.perm[(int)blockIdx.x + (int)gridDim.x*(j0 + wid)] : slot_env(a.balanced, (int)blockIdx.x, (int)gridDim.x, nw, FD ? j0/nw/a.fd.npass*nw : j0, wid);
+    const bool item = (j0 + wid) < per_cta && slot >= 0 && slot < a.n_env;
+    const int env = FD ? slot/a.fd.ncol : slot;
+    const FdCol fc = FD && item ? fd_column(m, a, env, slot - env*a.fd.ncol) : FdCol{};
+    double* const fd_row = FD ? a.fd.rows + ((size_t)blockIdx.x*nw + wid)*(m.nu + m.nq + m.nv + m.na) : nullptr;      // this slot's rows
+    const bool live = item && (!FD || fd_runs(a, fc, pass)); const long long tstep_ = prof ? clock64() : 0; int load_acc = 0;
     if (live) {
       load_env_state(m, w, b, env);
+      if (FD) fd_perturb(m, w, a, env, fc, pass, fd_row);
       if (!ROLL && a.mode == 2) {
         if (!a.reset_mask || a.reset_mask[env]) { env_reset(m, w, a, env);
           task_observe(m, w, a, env, 0, 0.0);
@@ -357,7 +435,7 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
       const bool tap = DBG && s == nsub-1;
       PH(0, phase_kinematics(m, w));
       PH(1, phase_tendon_all(m, w); if (tap && b.tap_moment) { const double* mom = SCR(s_mom); for (int i = w.lane; i < m.nnz; i += 32) b.tap_moment[(size_t)env*m.nnz+i] = mom[i]; });
-      PH(2, phase_actuation(m, w, integrate, ROLL ? a.roll.ctrl + ((size_t)env*a.roll_nstep + a.roll_t)*m.nu : m.g_ctrl + (size_t)env*m.nu, tap && b.tap_actuator_force ? b.tap_actuator_force + (size_t)env*m.nu : nullptr, tap && b.tap_ten_length ? b.tap_ten_length + (size_t)env*m.nu : nullptr);
+      PH(2, phase_actuation(m, w, integrate, ROLL ? (FD && fc.ctrl >= 0 ? fd_row : a.roll.ctrl + ((size_t)env*a.roll_nstep + a.roll_t)*m.nu) : m.g_ctrl + (size_t)env*m.nu, tap && b.tap_actuator_force ? b.tap_actuator_force + (size_t)env*m.nu : nullptr, tap && b.tap_ten_length ? b.tap_ten_length + (size_t)env*m.nu : nullptr);
             if (ROLL && a.roll.qfrc_applied) { const double* f = a.roll.qfrc_applied + ((size_t)env*a.roll_nstep + a.roll_t)*m.nv;      // mjData.qfrc_applied
               for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] += f[i];
               __syncwarp(); });
@@ -376,7 +454,10 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
     }
     #undef PH
     if (prof && live && w.lane == 0) { long long* pc = b.tap_phase_cycles + 20*(size_t)env; for (int k = 0; k < 20; k++) pc[k] = cyc[k]; pc[12] = maxcon_seen; pc[13] = maxefc_seen; pc[17] = clock64() - tstep_; }
-    if (live) {
+    if (FD && item) {
+      if (live && overflow_seen && w.lane == 0 && b.overflow) b.overflow[env] = 1;      // (every writer stores 1)
+      fd_store(m, w, a, env, fc, pass, live, fd_row + m.nu); }
+    if (!FD && live) {
       if (DBG && a.mode == 1) { if (integrate && w.lane == 0 && b.time) b.time[env] += nsub*m.timestep; }
       else if (a.mode == 0) {
         // ---- obs / reward / done / TimeLimit / auto-reset
@@ -429,6 +510,9 @@ extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __gri
 // rollout (myo_batch_rollout): the product body's mode 0 with the caller's ctrl and applied forces, under the two product launch bounds
 extern "C" __global__ void __launch_bounds__(320) myo_roll_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320, true>(m, a); }
 extern "C" __global__ void __launch_bounds__(448) myo_roll_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448, true>(m, a); }
+// transition FD (myo_batch_transition_fd): the rollout body over (env, column) work items, under launch_bounds(320)
+extern "C" __global__ void __launch_bounds__(320) myo_fd_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320, true, true>(m, a); }
+static_assert(sizeof(DevModel) + sizeof(StepArgs) <= 4096, "the step kernels' arguments fit the 4 KB kernel parameter space");
 
 // ------------------------------------------------------------------ mjData readout (myo_batch_data)
 // One forward pass over the stored state of every env, one env per warp on the balanced map (env = CTA + grid * slot).  Each field is
@@ -797,7 +881,9 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   LaunchShape inv_shape; bool inv_ready;      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
   // rollout (myo_batch_rollout), set up by its first call: carry state [n, nq + 2 nv + na + 1] (qpos | qvel | act | warm start | time)
   bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced;
-  LaunchShape ik_shape; bool ik_ready; };      // launch shape of myo_ik_kernel, set by the first myo_batch_ik
+  LaunchShape ik_shape; bool ik_ready;      // launch shape of myo_ik_kernel, set by the first myo_batch_ik
+  // transition FD (myo_batch_transition_fd): launch shape of myo_fd_kernel for fd_items work items, and its per-slot rows
+  LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1002,7 +1088,7 @@ static void data_release(myo_batch* b) {
   cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
   memset(&b->data, 0, sizeof(b->data)); b->data_shape = LaunchShape(); b->data_ready = false; }
 extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
-  cudaFree(b->dCarry); data_release(b); delete b; }
+  cudaFree(b->dCarry); cudaFree(b->dFdRows); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
 // Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 8) written):
@@ -1178,12 +1264,18 @@ static int roll_setup(myo_batch* b) {
   b->roll_ready = true; return 0;
 }
 
+static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream);
 extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
   if (!b || !r) return fail("myo_batch_rollout: null");
   if (!r->ctrl) return fail("myo_batch_rollout: ctrl is required");
   if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
   if (nstep < 1 || substeps < 1) return fail("myo_batch_rollout: nstep and substeps must be >= 1");
   CUDA_OK(cudaSetDevice(b->device));
+  return roll_run(b, r, nstep, substeps, stream);
+}
+
+// The launches of a checked rollout, on the current device: the carry from the start state, then one launch per interval
+static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
   if (!b->roll_ready) { if (const int rc = roll_setup(b)) { cudaFree(b->dCarry); b->dCarry = nullptr; return rc; } }
   const DevModel& d = b->dm; const size_t n = b->n_env; cudaStream_t st = (cudaStream_t)stream;
   // the carry: the start state, from the caller's rows or the bound buffers
@@ -1269,5 +1361,45 @@ extern "C" int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_
     b->ik_ready = true; }
   a.d = *d; a.p = *p; a.bound_qpos = b->bufs.qpos; a.n_env = b->n_env; const LaunchShape& s = b->ik_shape;
   myo_ik_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+// Transition FD: the nominal interval is a rollout into the carry (so it is that rollout, bit for bit); then myo_fd_kernel runs every
+// (env, column) item from the env's start state (the caller's rows or the bound buffers, read only) and writes A and B in place.
+extern "C" int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, const myo_fd_params* p, void* stream) {
+  if (!b || !d || !p) return fail("myo_batch_transition_fd: null");
+  if (!d->ctrl) return fail("myo_batch_transition_fd: ctrl is required");
+  if (!d->A && !d->B) return fail("myo_batch_transition_fd: at least one of A and B is required");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (!std::isfinite(p->eps) || !(p->eps > 0)) return fail("myo_batch_transition_fd: eps must be finite and > 0");
+  if (p->substeps < 1) return fail("myo_batch_transition_fd: substeps must be >= 1");
+  if (p->centered != 0 && p->centered != 1) return fail("myo_batch_transition_fd: centered must be 0 or 1");
+  const DevModel& dm = b->dm; const int nx = 2*dm.nv + dm.na, nxa = d->A ? nx : 0, ncol = nxa + (d->B ? dm.nu : 0);
+  const long long items = (long long)b->n_env*ncol;
+  if (items > 0x7fffffffLL) return fail("myo_batch_transition_fd: n_env * columns must fit in int32");
+  CUDA_OK(cudaSetDevice(b->device)); cudaStream_t st = (cudaStream_t)stream;
+  myo_rollout_buffers r; memset(&r, 0, sizeof(r));
+  r.ctrl = d->ctrl; r.qfrc_applied = d->qfrc_applied; r.qpos0 = d->qpos0; r.qvel0 = d->qvel0; r.act0 = d->act0; r.qacc_warmstart0 = d->qacc_warmstart0; r.overflow = d->overflow;
+  if (const int rc = roll_run(b, &r, 1, p->substeps, stream)) return rc;
+  if (items == 0) return 0;
+  if (b->fd_items != items) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+    if (launch_shape((const void*)myo_fd_kernel, prop, dm.n_per_warp*8, b->const_bytes, (int)items, b->big, 0, b->fd_shape)) return -1;
+    b->fd_items = items; }
+  const LaunchShape& s = b->fd_shape;
+  const size_t rows = (size_t)s.grid*s.warps*(dm.nu + dm.nq + dm.nv + dm.na)*8;
+  if (rows > b->fd_rows_bytes) { cudaFree(b->dFdRows); b->dFdRows = nullptr; b->fd_rows_bytes = 0;
+    CUDA_OK(cudaMalloc(&b->dFdRows, rows)); b->fd_rows_bytes = rows; }
+  const myo_buffers& q = b->bufs;
+  myo_buffers c; memset(&c, 0, sizeof(c));      // the start state, read only: no state is stored back in this kernel
+  c.qpos = d->qpos0 ? (double*)d->qpos0 : q.qpos; c.qvel = d->qvel0 ? (double*)d->qvel0 : q.qvel; c.act = d->act0 ? (double*)d->act0 : q.act;
+  c.qacc_warmstart = d->qacc_warmstart0 ? (double*)d->qacc_warmstart0 : q.qacc_warmstart; c.env_prm = q.env_prm; c.overflow = d->overflow;
+  StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 0; a.b = c; a.roll.ctrl = d->ctrl; a.roll.qfrc_applied = d->qfrc_applied; a.roll_nstep = 1; a.roll_t = 0;
+  a.cfg = b->cfg; a.cfg.task = MYO_TASK_NONE; a.cfg.muscle_condition = MYO_COND_NONE; a.cfg.reaf_dst = a.cfg.reaf_src = 0; a.cfg.auto_reset = 0; a.cfg.frame_skip = p->substeps;
+  a.n_env = (int)items; a.dt = dm.timestep*p->substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset; a.balanced = 0;
+  a.fd.A = d->A; a.fd.B = d->B; a.fd.nom = b->dCarry; a.fd.rows = b->dFdRows; a.fd.eps = p->eps; a.fd.rinv1 = 1.0/p->eps; a.fd.rinv2 = 1.0/(2.0*p->eps);
+  a.fd.n_env = b->n_env; a.fd.ncol = ncol; a.fd.nxa = nxa; a.fd.npass = p->centered ? 2 : 1;
+  // (the dynamic shared-memory limit is an attribute of the kernel, not of the batch: a batch of another size may have lowered it since)
+  CUDA_OK(cudaFuncSetAttribute((const void*)myo_fd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem));
+  myo_fd_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

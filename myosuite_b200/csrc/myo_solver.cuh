@@ -520,6 +520,29 @@ __device__ __forceinline__ void integrate_pos(const DevModel& m, const Warp w, d
     else qpos[qa] += h*v[da]; }
 }
 
+// v <- q2 (-) q1 (mj_differentiatePos with dt = 1): hinge and slide joints and a free joint's position subtract; a free joint's quaternion
+// gives mju_subQuat(q2, q1), the rotation vector of q1^-1 q2 in the body frame (the frame integrate_pos turns in), angle in (-pi, pi].
+// The vector part of q1^-1 q2 is formed without fused multiply-adds, so that equal quaternions give exactly 0 (a contracted
+// a0 b1 - b0 a1 leaves the rounding error of one product, which divided by eps would put ~1e-11 into columns that are exactly 0).
+// Lanes over the joints; the caller syncs.
+__device__ __forceinline__ void differentiate_pos(const DevModel& m, const Warp w, double* v, const double* q1, const double* q2) {
+  const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr);
+  for (int j = w.lane; j < m.njnt; j += 32) { int qa = jq[j], da = jd[j];
+    if (jtype[j] == 0) { for (int c = 0; c < 3; c++) v[da+c] = q2[qa+c] - q1[qa+c];
+      const double* a = q1 + qa + 3; const double* b = q2 + qa + 3;
+      #define M_(x, y) __dmul_rn(x, y)
+      const double d[4] = {__dadd_rn(__dadd_rn(__dadd_rn(M_(a[0], b[0]), M_(a[1], b[1])), M_(a[2], b[2])), M_(a[3], b[3])),      // conj(a) b
+        __dsub_rn(__dsub_rn(M_(a[0], b[1]), M_(b[0], a[1])), __dsub_rn(M_(a[2], b[3]), M_(a[3], b[2]))),
+        __dsub_rn(__dsub_rn(M_(a[0], b[2]), M_(b[0], a[2])), __dsub_rn(M_(a[3], b[1]), M_(a[1], b[3]))),
+        __dsub_rn(__dsub_rn(M_(a[0], b[3]), M_(b[0], a[3])), __dsub_rn(M_(a[1], b[2]), M_(a[2], b[1])))};
+      #undef M_
+      double ax[3] = {d[1], d[2], d[3]}; const double s = sqrt(dot3(ax, ax));
+      if (s < MYO_MINVAL) { ax[0] = 1; ax[1] = 0; ax[2] = 0; } else { const double r = 1.0/s; ax[0] *= r; ax[1] *= r; ax[2] *= r; }
+      const double PI = 3.14159265358979323846; double ang = 2*atan2(s, d[0]); if (ang > PI) ang -= 2*PI;
+      for (int c = 0; c < 3; c++) v[da+3+c] = ax[c]*ang; }
+    else v[da] = q2[qa] - q1[qa]; }
+}
+
 __device__ void phase_integrate(const DevModel& m, const Warp w, long long* cyc) {
   int n = m.nv; double h = m.timestep; long long tc = cyc ? clock64() : 0;
   // (M + h B) qacc' = M qacc  (= qfrc_smooth + qfrc_constraint at the solver optimum)

@@ -498,6 +498,67 @@ class MyoVecEnv:
                     fields=("jacp", "jacr", "site_xpos", "site_xmat"))
         return r["jacp"], r["jacr"], r["site_xpos"], r["site_xmat"]
 
+    FD_FIELDS = ("A", "B", "overflow")
+
+    def transition_fd(self, ctrl, eps=1e-6, centered=False, substeps=1, qfrc_applied=None, initial_state=None, fields=("A", "B")):
+        """MuJoCo's mjd_transitionFD for every env, over one interval of `substeps` mj_steps with ctrl held (substeps = 1 is
+        mjd_transitionFD itself; substeps = frame_skip linearises the env's control interval, whose B is not zero in qpos / qvel since ctrl
+        enters the muscles only through act_dot).  x' ~ x'0 + A dx + B du with x = [dq (nv, tangent space), qvel (nv), act (na)], nx =
+        2 nv + na: A [num_envs, nx, nx], B [num_envs, nx, nu], A[i][j] = d x'_i / d x_j.  Forward differences, or centred ones with
+        centered=True; ctrl columns at a ctrlrange end take the one side that stays in range (mjd_stepFD's rule, include/myo_b200.h).
+        ctrl [num_envs, nu] is mjData.ctrl (as rollout(): no action remap), qfrc_applied [num_envs, nv] or None, both float64 CUDA
+        tensors on this batch's device, contiguous.  initial_state: {"qpos", "qvel", "act", "qacc_warmstart": float64 tensor
+        [num_envs, width]}; a key left out is taken from the env's current state.  The nominal x'0 is exactly rollout(ctrl[:, None],
+        substeps=substeps) from the same start, and every perturbed interval starts with the start's warm start.
+        Returns {field: tensor} of FD_FIELDS (overflow [num_envs] int32: set where a substep of the nominal or a perturbed interval
+        dropped contacts).  The outputs are allocated per call: A takes num_envs * nx^2 * 8 bytes (359 MB for 2048 legs envs, 320 MB for
+        661 torso envs), B num_envs * nx * nu * 8.  Not a state change: the call advances nothing and writes no env buffer.  With the
+        iterative solver each column carries solver noise of order solver_tolerance / eps, as in MuJoCo; MyoVecEnv(...,
+        solver_tolerance=...) tightens it.  Two launches (the nominal interval, then one warp per (env, column))."""
+        torch = self.torch
+        fields = tuple(fields)
+        bad = [f for f in fields if f not in self.FD_FIELDS]
+        if bad:
+            raise KeyError("unknown transition_fd fields %s (available: %s)" % (bad, list(self.FD_FIELDS)))
+        if "A" not in fields and "B" not in fields:
+            raise ValueError("transition_fd needs at least one of the fields A and B")
+        m, n = self.mj_model, self.num_envs
+        substeps, eps = int(substeps), float(eps)
+        if substeps < 1:
+            raise ValueError("substeps must be >= 1, got %d" % substeps)
+        if not (np.isfinite(eps) and eps > 0):
+            raise ValueError("eps must be finite and > 0, got %r" % eps)
+        if centered not in (0, 1, False, True):
+            raise ValueError("centered must be a bool, got %r" % (centered,))
+
+        def check(name, x, shape):
+            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
+                    or not x.is_contiguous()):
+                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
+                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
+                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+        check("ctrl", ctrl, (n, m.nu))
+        bufs = {"ctrl": ctrl}
+        if qfrc_applied is not None:
+            check("qfrc_applied", qfrc_applied, (n, m.nv))
+            bufs["qfrc_applied"] = qfrc_applied
+        width = dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,))
+        for k, v in (initial_state or {}).items():
+            if k not in width:
+                raise KeyError("unknown initial_state key %r (available: %s)" % (k, list(width)))
+            if v is not None:
+                check("initial_state[%r]" % k, v, (n,) + width[k])
+                bufs[abi.ROLLOUT_STATE[k]] = v
+        nx = 2 * m.nv + m.na
+        shape = dict(A=(n, nx, nx), B=(n, nx, m.nu))
+        out = {}
+        for f in fields:
+            out[f] = (torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow"
+                      else torch.full(shape[f], float("nan"), dtype=torch.float64, device=self.device))
+        params = abi.MyoFdParams(eps=eps, centered=int(bool(centered)), substeps=substeps)
+        self.batch.transition_fd(params, stream=self._stream(), **bufs, **out)
+        return out
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -704,6 +765,20 @@ class MyoEnv:
         """mujoco.mj_jacSite at the current state: (jacp [3, nv], jacr [3, nv]) as numpy arrays."""
         jp, jr, _, _ = self.vec.jac_site([site])
         return jp[0, 0].cpu().numpy(), jr[0, 0].cpu().numpy()
+
+    def mjd_transitionFD(self, ctrl, eps=1e-6, flg_centered=False, substeps=1, qfrc_applied=None, initial_state=None):
+        """mujoco.mjd_transitionFD of this env (MyoVecEnv.transition_fd) over one interval of `substeps` mj_steps: ctrl [nu] is MuJoCo's
+        ctrl, qfrc_applied [nv] or None, initial_state {key: array} or None (the current state).  Returns numpy (A [nx, nx], B [nx, nu]),
+        nx = 2 nv + na.  Not a state change.  One device-to-host copy."""
+        v = self.vec
+        as_dev = lambda x, shape: v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        q = None if qfrc_applied is None else as_dev(qfrc_applied, (1, self.mj_model.nv))
+        st = None if initial_state is None else {k: as_dev(x, (1, -1)) for k, x in initial_state.items()}
+        out = v.transition_fd(as_dev(ctrl, (1, self.mj_model.nu)), eps=eps, centered=flg_centered, substeps=substeps, qfrc_applied=q,
+                              initial_state=st)
+        nx = out["A"].shape[1]
+        flat = v.torch.cat([out["A"][0].reshape(-1), out["B"][0].reshape(-1)]).cpu().numpy()
+        return flat[:nx * nx].reshape(nx, nx), flat[nx * nx:].reshape(nx, -1)
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)
     def get_obs_dict(self, *sim_args):

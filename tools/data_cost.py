@@ -13,7 +13,13 @@ The "ik" case (MyoVecEnv.ik, myo_batch_ik): the hand, 4096 envs, the five finger
 in-range configurations, start at qpos0, in alternating order with one env step: "ik" at the default parameters (per call, with the mean
 and largest number of iterations), "ik_10" (tol = 0, max_iter = 10: every env runs 10 iterations) and "jac_site" (max_iter = 0).  Per
 iteration = (ik_10 - jac_site) / 10.  Beside them, the C reference (tests/ik_oracle.c, oracle_ik) at the same defaults on one host core
-for the first --ref-envs targets.  --cases selects cases by name."""
+for the first --ref-envs targets.
+
+The "fd" case (MyoVecEnv.transition_fd, myo_batch_transition_fd): the hand, 4096 envs, in alternating order with one env step: forward
+and centred A and B at substeps 1 and frame_skip, and the host loop of rollout calls (one per column) that the rollout API alone allows
+for the same forward A and B at substeps 1; then the single env (MyoEnv.mjd_transitionFD, the device call alone, the host loop) on the
+hand and the legs, beside the C reference (tests/fd_oracle.c) on one host core.  --fd-reps rounds (x4 for the single env).
+--cases selects cases by name (the fd case runs only when named)."""
 import argparse
 import json
 import os
@@ -113,6 +119,114 @@ def ik_case(args):
     return dict(env_id=IK_ENV, n_env=n, sites=list(IK_SITES), **s)
 
 
+FD_ENV, FD_N, FD_SINGLE = "myoHandPoseRandom-v0", 4096, (("hand", "myoHandPoseRandom-v0"), ("legs", "myoLegWalk-v0"))
+
+
+def _fd_host_loop(env, ctrl, substeps):
+    """forward-difference A and B the way the rollout API alone allows: one rollout per column from a host-built perturbed start (hinge /
+    slide qpos, qvel, act and ctrl columns; a free joint's rotation would need its quaternion update on the host as well)"""
+    import numpy as np
+    import torch
+    m, eps = env.mj_model, 1e-6
+    nv, na = m.nv, m.na
+    S = {k: env.t[k].clone() for k in ("qpos", "qvel", "act", "qacc_warmstart")}
+    roll = lambda st, c: env.rollout(c[:, None].contiguous(), substeps=substeps, initial_state=st, fields=("qpos", "qvel", "act"))
+    R0 = roll(S, ctrl)
+    x0 = torch.cat([R0["qpos"][:, 0], R0["qvel"][:, 0], R0["act"][:, 0]], 1)
+    cols = []
+    for j in range(2 * nv + na + m.nu):
+        st, c = dict(S), ctrl
+        if j < nv:
+            q = S["qpos"].clone(); st["qpos"] = q
+            jn = int(np.nonzero(m.jnt_dofadr <= j)[0][-1]); qa, k = m.jnt_qposadr[jn], j - m.jnt_dofadr[jn]
+            if m.jnt_type[jn] != 0 or k < 3:
+                q[:, qa + k] += eps
+            else:           # a free joint's rotation: q <- q (cos eps/2, e_k sin eps/2), normalised (mj_integratePos)
+                w = q[:, qa + 3:qa + 7].clone(); r = torch.zeros(4, dtype=q.dtype, device=q.device)
+                r[0], r[k - 2] = np.cos(eps / 2), np.sin(eps / 2)
+                prod = torch.stack([w[:, 0] * r[0] - (w[:, 1:] * r[1:]).sum(1)] + [w[:, 0] * r[1 + i] + r[0] * w[:, 1 + i] for i in range(3)], 1)
+                prod[:, 1:] += torch.cross(w[:, 1:], r[1:].expand(len(w), 3), dim=1)
+                q[:, qa + 3:qa + 7] = prod / prod.norm(dim=1, keepdim=True)
+        elif j < 2 * nv:
+            v = S["qvel"].clone(); v[:, j - nv] += eps; st["qvel"] = v
+        elif j < 2 * nv + na:
+            a = S["act"].clone(); a[:, j - 2 * nv] += eps; st["act"] = a
+        else:
+            c = ctrl.clone(); c[:, j - 2 * nv - na] += eps
+        R = roll(st, c)
+        cols.append((torch.cat([R["qpos"][:, 0], R["qvel"][:, 0], R["act"][:, 0]], 1) - x0) * (1 / eps))
+    return torch.stack(cols, 2)
+
+
+def fd_case(args):
+    """transition_fd beside one env step: the hand batch (forward and centred, substeps 1 and frame_skip), the host loop of rollouts over
+    the columns, the single env on the hand and the legs, and the C reference (tests/fd_oracle.c) on one host core"""
+    import time
+    import numpy as np
+    import torch
+    from myosuite_b200 import vec_env
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from fd_oracle import FdOracle
+    out = {}
+    env = vec_env.MyoVecEnv(FD_ENV, FD_N, seed=0)
+    m, n, fs = env.mj_model, FD_N, env.frame_skip
+    env.reset(seed=0)
+    stream = torch.cuda.current_stream(env.device)
+    g = torch.Generator(device="cpu").manual_seed(0)
+    acts = [(torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device) for _ in range(8)]
+    for k in range(4):
+        env.step(acts[k])
+    ctrl = torch.rand(n, m.nu, generator=g, dtype=torch.float64).to(env.device)
+    calls = {"step": lambda k: env.step(acts[k % 8]),
+             "fd_fwd_1": lambda k: env.transition_fd(ctrl), "fd_ctr_1": lambda k: env.transition_fd(ctrl, centered=True),
+             "fd_fwd_fs": lambda k: env.transition_fd(ctrl, substeps=fs), "fd_ctr_fs": lambda k: env.transition_fd(ctrl, centered=True, substeps=fs),
+             "host_loop_fwd_1": lambda k: _fd_host_loop(env, ctrl, 1)}
+    for k in range(2):
+        for f in calls.values():
+            f(k)
+    torch.cuda.synchronize()
+    order = list(calls)
+    t = {k: [] for k in order}
+    for r in range(args.fd_reps):
+        for k in (order if r % 2 == 0 else order[::-1]):
+            t[k].append(_timed(stream, lambda: calls[k](r)))
+    s = {k: dict(median_us=float(np.median(v)), min_us=float(np.min(v)), max_us=float(np.max(v))) for k, v in t.items()}
+    for k in order[1:]:
+        s[k]["per_step"] = s[k]["median_us"] / s["step"]["median_us"]
+    out["batch"] = dict(env_id=FD_ENV, n_env=n, frame_skip=fs, columns=2 * m.nv + m.na + m.nu, **s)
+    print("fd batch      n %4d  step %8.1f us | " % (n, s["step"]["median_us"]) + "  ".join("%s %9.1f us (%.2f step)" % (k, s[k]["median_us"], s[k]["per_step"]) for k in order[1:]), flush=True)
+    del env, calls
+    torch.cuda.empty_cache()
+    for name, eid in FD_SINGLE:
+        one = vec_env.MyoEnv(eid, seed=0)
+        one.reset()
+        v = one.vec
+        c1 = torch.rand(1, v.mj_model.nu, generator=g, dtype=torch.float64).to(v.device)
+        st = torch.cuda.current_stream(v.device)
+        calls = {"mjd_transitionFD": lambda k: one.mjd_transitionFD(c1[0].cpu().numpy()), "fd_device": lambda k: v.transition_fd(c1),
+                 "host_loop": lambda k: _fd_host_loop(v, c1, 1)}
+        for k in range(2):
+            for f in calls.values():
+                f(k)
+        torch.cuda.synchronize()
+        t = {k: [] for k in calls}
+        for r in range(args.fd_reps * 4):
+            for k in (list(calls) if r % 2 == 0 else list(calls)[::-1]):
+                t[k].append(_timed(st, lambda: calls[k](r)))
+        s = {k: dict(median_us=float(np.median(x)), min_us=float(np.min(x)), max_us=float(np.max(x))) for k, x in t.items()}
+        o = FdOracle(v.I, v.D)
+        o.reset(); o.set(qpos=v.t["qpos"][0].cpu().numpy(), qvel=v.t["qvel"][0].cpu().numpy(), act=v.t["act"][0].cpu().numpy())
+        t0 = time.perf_counter()
+        for _ in range(3):
+            o.transition_fd(c1[0].cpu().numpy())
+        s["c_reference_us"] = (time.perf_counter() - t0) / 3 * 1e6
+        out["single_" + name] = dict(env_id=eid, **s)
+        print("fd single %-4s  mjd_transitionFD %8.1f us | device call %8.1f us | host loop of rollouts %9.1f us | C reference, one core %10.1f us"
+              % (name, s["mjd_transitionFD"]["median_us"], s["fd_device"]["median_us"], s["host_loop"]["median_us"], s["c_reference_us"]), flush=True)
+        del one, v
+    return out
+
+
 def main():
     import numpy as np
     import torch
@@ -123,6 +237,7 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--cases", default=",".join([c[0] for c in CASES] + ["ik"]))
     ap.add_argument("--ref-envs", type=int, default=64)
+    ap.add_argument("--fd-reps", type=int, default=5)
     args = ap.parse_args()
     want = set(args.cases.split(","))
     res = {"gpu_before": gpu_info(), "cases": {}}
@@ -176,6 +291,8 @@ def main():
         torch.cuda.empty_cache()
     if "ik" in want:
         res["cases"]["ik"] = ik_case(args)
+    if "fd" in want:
+        res["cases"]["fd"] = fd_case(args)
     res["gpu_after"] = gpu_info()
     print("GPU [name, power limit, SM clock, max SM clock, throttle reasons] before: %s after: %s" % (res["gpu_before"], res["gpu_after"]))
     if args.out:
