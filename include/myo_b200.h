@@ -18,9 +18,11 @@
  * Conventions: every function returns 0 on success, <0 on error (text via myo_last_error(), thread
  * local).  No exceptions cross the ABI, no torch types appear in it.  All per-env arrays are
  * CALLER-OWNED device buffers (e.g. torch CUDA tensors passed by data_ptr()), contiguous,
- * row-major [n_env, width], on the batch's device, and must outlive the batch.  A batch is
- * single-stream and not re-entrant; distinct batches (one per GPU) are independent; a model is
- * immutable and shareable.  `stream` arguments are `cudaStream_t` passed as void* (NULL = default).
+ * row-major [n_env, width], on the batch's device, and must outlive the batch.  Any number of
+ * batches, on one device or several, are independent: calls on one batch never change another
+ * batch's results or whether its launches succeed, in any order and from any stream or host
+ * thread.  Each batch itself is single-stream and not re-entrant.  A model is immutable and
+ * shareable.  `stream` arguments are `cudaStream_t` passed as void* (NULL = default).
  */
 #ifndef MYO_B200_H
 #define MYO_B200_H

@@ -1014,8 +1014,11 @@ static int warps_that_fit(const cudaDeviceProp& prop, int per_env_bytes, int con
 // Launch shape of kernel `fn`: as many env-warps per CTA as its thread limit and shared memory allow, at most one per env.  min_rounds (one
 // CTA per SM): the batch takes ceil(n_env / (SMs * warps)) rounds; among the warp counts that reach the minimal number of rounds take the
 // SMALLEST (same rounds, less issue contention and less lockstep imbalance per round).  want (tuning override, 0 = none) wins where it fits.
+// The dynamic shared-memory limit is an attribute of the kernel in the device context, shared by every batch: it is set to the most the
+// device allows that kernel, the same value from every batch and host thread, so that no batch's set-up can lower another batch's limit.
 static int launch_shape(const void* fn, const cudaDeviceProp& prop, int per_env_bytes, int const_bytes, int n_env, bool min_rounds, int want, LaunchShape& s) {
   cudaFuncAttributes fa; CUDA_OK(cudaFuncGetAttributes(&fa, fn));
+  const int smem_max = (int)prop.sharedMemPerBlockOptin - (int)fa.sharedSizeBytes;
   const int sms = prop.multiProcessorCount, fit = warps_that_fit(prop, per_env_bytes, const_bytes), maxw = fa.maxThreadsPerBlock/32;
   int wpc = fit < maxw ? fit : maxw; if (n_env < wpc) wpc = n_env;
   if (wpc < 1) return fail("model working set exceeds shared memory of one CTA");
@@ -1023,7 +1026,8 @@ static int launch_shape(const void* fn, const cudaDeviceProp& prop, int per_env_
     if ((size_t)per_env_bytes*best + const_bytes > 100*1024) wpc = best; }
   if (want >= 1 && want <= (maxw < fit ? maxw : fit)) wpc = want;
   s.warps = wpc; s.smem = const_bytes + wpc*per_env_bytes;
-  CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem));
+  if (s.smem > smem_max) return fail("launch shape needs more dynamic shared memory than the device allows the kernel");
+  CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
   int c = 1; CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, fn, wpc*32, s.smem)); if (c < 1) c = 1;
   const int need = (n_env + wpc - 1)/wpc, cap = sms*c; s.grid = need < cap ? need : cap;
   return 0;
@@ -1068,6 +1072,9 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
   CUDA_OK(cudaMalloc(&b->dCtrl, (size_t)n_env*imax(b->dm.nu, 1)*8)); CUDA_OK(cudaMemset(b->dCtrl, 0, (size_t)n_env*imax(b->dm.nu, 1)*8));
   b->dm.gI16 = b->dI; b->dm.gD = b->dD; b->dm.g_ctrl = b->dCtrl;
   if (b->regroup) { CUDA_OK(cudaMalloc(&b->dLoad, (size_t)n_env*4)); CUDA_OK(cudaMemset(b->dLoad, 0, (size_t)n_env*4)); CUDA_OK(cudaMalloc(&b->dPerm, (size_t)b->perm_slots*4)); }
+  // the uploads and memsets above run on the legacy stream (a pageable upload may return before its DMA lands): complete them here, so
+  // that a caller whose first launch goes to a non-blocking stream finds the model and the zeroed rows in place
+  CUDA_OK(cudaStreamSynchronize(cudaStreamLegacy));
   if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
     n_env, b->use_w14 ? "launch_bounds(448)" : "launch_bounds(320)", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
   return 0;
@@ -1213,6 +1220,7 @@ static int data_setup(myo_batch* b) {
   CUDA_OK(cudaMalloc(&b->dRI, ri.size()*4)); CUDA_OK(cudaMemcpy(b->dRI, ri.data(), ri.size()*4, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMalloc(&b->dRD, imax((int)rd.size(), 1)*8)); CUDA_OK(cudaMemcpy(b->dRD, rd.data(), rd.size()*8, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMalloc(&b->dPose, (size_t)b->n_env*2*nb*7*8));
+  CUDA_OK(cudaStreamSynchronize(cudaStreamLegacy));      // the tables are in place before a launch on any stream reads them (as batch_setup)
   a.nbody = nb; a.nsite = ns; a.nlevel = nlevel; a.lvl = b->dRI; a.parent = b->dRI + o_parent; a.jadr = b->dRI + o_jadr; a.jnum = b->dRI + o_jnum;
   a.jtype = b->dRI + o_jtype; a.jq = b->dRI + o_jq; a.site_body = b->dRI + o_sb; a.pair_geom = b->dRI + o_pg;
   a.bpos = b->dRD + od[0]; a.bquat = b->dRD + od[1]; a.jpos = b->dRD + od[2]; a.jaxis = b->dRD + od[3]; a.qpos0 = b->dRD + od[4]; a.site_pos = b->dRD + od[5];
@@ -1398,8 +1406,6 @@ extern "C" int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, co
   a.n_env = (int)items; a.dt = dm.timestep*p->substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset; a.balanced = 0;
   a.fd.A = d->A; a.fd.B = d->B; a.fd.nom = b->dCarry; a.fd.rows = b->dFdRows; a.fd.eps = p->eps; a.fd.rinv1 = 1.0/p->eps; a.fd.rinv2 = 1.0/(2.0*p->eps);
   a.fd.n_env = b->n_env; a.fd.ncol = ncol; a.fd.nxa = nxa; a.fd.npass = p->centered ? 2 : 1;
-  // (the dynamic shared-memory limit is an attribute of the kernel, not of the batch: a batch of another size may have lowered it since)
-  CUDA_OK(cudaFuncSetAttribute((const void*)myo_fd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem));
   myo_fd_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
