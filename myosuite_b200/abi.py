@@ -347,7 +347,7 @@ class Batch:
     def launches(self):
         return self.L.myo_batch_launch_count(self.handle)
 
-    LAUNCH_INFO_KEYS = ("use_w14", "warps_per_cta", "grid", "rounds", "regroup", "balanced", "smem_bytes", "perm_slots")
+    LAUNCH_INFO_KEYS = ("use_w14", "warps_per_cta", "grid", "rounds", "regroup", "balanced", "smem_bytes", "perm_slots", "hand_shape")
 
     def launch_info(self):
         """How env steps are launched: product kernel (use_w14), warps per CTA, grid, rounds per CTA, slot -> env map (regroup / balanced)."""

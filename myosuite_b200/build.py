@@ -4,8 +4,9 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "myo_b200.cu")
-DEPS = [SRC, os.path.join(HERE, "csrc", "myo_device.cuh"), os.path.join(HERE, "csrc", "myo_solver.cuh"),
-        os.path.join(HERE, "..", "include", "myo_b200.h"), os.path.join(HERE, "..", "include", "myo_blob_layout.h")]
+DEPS = [SRC, os.path.join(HERE, "csrc", "myo_device.cuh"), os.path.join(HERE, "csrc", "myo_solver.cuh"), os.path.join(HERE, "csrc", "myo_layout.cuh"),
+        os.path.join(HERE, "..", "include", "myo_b200.h"), os.path.join(HERE, "..", "include", "myo_blob_layout.h"),
+        os.path.join(HERE, "..", "include", "myo_hand_shape.h")]
 LIB = os.path.join(HERE, "libmyo_b200.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]

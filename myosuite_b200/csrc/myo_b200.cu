@@ -7,7 +7,7 @@
 #include <string>
 #include <vector>
 
-#include "myo_solver.cuh"
+#include "myo_layout.cuh"
 
 // ------------------------------------------------------------------ kernel arguments
 #define MYO_BMASK 0x40      /* phases of the product kernels that start with a CTA barrier (bit k = phase k).  0x40: only the solver entry, whose inner
@@ -67,7 +67,7 @@ __device__ __noinline__ double philox_uniform(Philox& p) {   // [0,1) with 53 ra
   return ((double)(((unsigned long long)(a >> 5) << 26) | (b >> 6))) * (1.0/9007199254740992.0); }
 
 // ------------------------------------------------------------------ parity taps
-__device__ void write_taps_solve(const DevModel& m, const Warp w, const StepArgs& a, int env) {   // after the Newton solve
+template <class MD> __device__ void write_taps_solve(const MD& m, const Warp w, const StepArgs& a, int env) {   // after the Newton solve
   const myo_buffers& b = a.b;
   if (b.tap_qacc) for (int i = w.lane; i < m.nv; i += 32) b.tap_qacc[(size_t)env*m.nv+i] = S_a[i];
   if (b.tap_qfrc_smooth) for (int i = w.lane; i < m.nv; i += 32) b.tap_qfrc_smooth[(size_t)env*m.nv+i] = W_(fsm)[i];
@@ -75,7 +75,7 @@ __device__ void write_taps_solve(const DevModel& m, const Warp w, const StepArgs
   if (b.tap_ncon && w.lane == 0) { int* t = b.tap_ncon + 4*(size_t)env; t[0] = WI_(ncon); t[1] = WI_(nefc); t[2] = WI_(niter); t[3] = WI_(overflow); }
   __syncwarp();
 }
-__device__ void write_taps_contacts(const DevModel& m, const Warp w, const StepArgs& a, int env) {   // after constraint assembly (con is overwritten by the solve)
+template <class MD> __device__ void write_taps_contacts(const MD& m, const Warp w, const StepArgs& a, int env) {   // after constraint assembly (con is overwritten by the solve)
   const myo_buffers& b = a.b; const int ncon = WI_(ncon);
   // reported in model pair order (the rank phase_constraints assigned), -1 / 0 padded
   if (b.tap_contact_pair) for (int c = w.lane; c < m.maxcon; c += 32) if (c >= ncon) b.tap_contact_pair[(size_t)env*m.maxcon+c] = -1;
@@ -87,7 +87,7 @@ __device__ void write_taps_contacts(const DevModel& m, const Warp w, const StepA
 }
 
 // ------------------------------------------------------------------ task logic: pose task (pose_v0.py:100-140,154-170,174-257)
-__device__ void env_reset(const DevModel& m, const Warp w, const StepArgs& a, int env) {
+template <class MD> __device__ void env_reset(const MD& m, const Warp w, const StepArgs& a, int env) {
   const myo_buffers& b = a.b; long long ep = b.episode_count ? b.episode_count[env] : 0;
   Philox rng; philox_init(rng, a.seed, (unsigned long long)(a.env_offset + env), (unsigned long long)ep, (uint32_t)w.lane);
   const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const double* jrange = CD(jnt_range); const double* qpos0 = CD(qpos0);
@@ -137,7 +137,7 @@ __device__ void env_reset(const DevModel& m, const Warp w, const StepArgs& a, in
   __syncwarp();
 }
 
-__device__ void write_obs_pose(const DevModel& m, const Warp w, const StepArgs& a, int env, double* dist_out, double* actmag_out) {
+template <class MD> __device__ void write_obs_pose(const MD& m, const Warp w, const StepArgs& a, int env, double* dist_out, double* actmag_out) {
   const myo_buffers& b = a.b; float* o = b.obs ? b.obs + (size_t)env*a.obs_dim : nullptr; double d2 = 0, a2 = 0;
   for (int i = w.lane; i < m.nq; i += 32) { double tgt = b.target ? b.target[(size_t)env*m.nq+i] : 0.0, err = tgt - W_(qpos)[i]; d2 += err*err;
     if (o) { o[i] = (float)W_(qpos)[i]; o[m.nq+m.nv+i] = (float)err; } }
@@ -147,14 +147,14 @@ __device__ void write_obs_pose(const DevModel& m, const Warp w, const StepArgs& 
 }
 
 // reward / done of the current state (pose_v0.py:113-140); lane 0 writes
-__device__ void pose_reward_done(const DevModel& m, const Warp w, const StepArgs& a, int env, double* rw_out, bool* done_out) {
+template <class MD> __device__ void pose_reward_done(const MD& m, const Warp w, const StepArgs& a, int env, double* rw_out, bool* done_out) {
   double dist, am; write_obs_pose(m, w, a, env, &dist, &am);
   const double far_th = a.cfg.task_d[0] > 0 ? a.cfg.task_d[0] : 4*3.14159265358979323846/2; double thd = a.cfg.pose_thd;      // PoseEnvV0: 2 pi (pose_v0.py:117); TorsoEnvV0: pi (torso_v0.py:104), passed in task_d[0]
   *rw_out = a.cfg.weights[0]*(-dist) + a.cfg.weights[1]*((dist < thd ? 1.0 : 0.0)+(dist < 1.5*thd ? 1.0 : 0.0)) + a.cfg.weights[2]*(-am) + a.cfg.weights[3]*(dist > far_th ? -1.0 : 0.0);
   *done_out = dist > far_th; }
 
 // spatial velocity [omega; v_origin] of dynamic body k from its dof chain
-__device__ __forceinline__ void body_velocity(const DevModel& m, const Warp w, int k, double* v) {
+template <class MD> __device__ __forceinline__ void body_velocity(const MD& m, const Warp w, int k, double* v) {
   const idx_t* cadr = CI(PCH_adr); const idx_t* ch = CI(PCH);
   for (int c = 0; c < 6; c++) v[c] = 0;
   #pragma unroll 1
@@ -162,7 +162,7 @@ __device__ __forceinline__ void body_velocity(const DevModel& m, const Warp w, i
 
 // WalkEnvV0 obs / reward / done (walk_v0.py:268-319,358-494) on the post-step state; needs kinematics + tendon + actuation of that
 // state in scratch (the reference's extra mj_forward, robot.py:607).  `steps` = WalkEnvV0.steps BEFORE its increment (walk_v0.py:339-342).
-__device__ void walk_observe(const DevModel& m, const Warp w, const StepArgs& a, int env, int steps, double* rw_out, bool* done_out) {
+template <class MD> __device__ void walk_observe(const MD& m, const Warp w, const StepArgs& a, int env, int steps, double* rw_out, bool* done_out) {
   const myo_buffers& b = a.b; const int* ti = a.cfg.task_i; const double* td = a.cfg.task_d;
   const double* PB = CD(PB_d); const double* xpos = SCR(s_xpos); const double* xmat = SCR(s_xmat);
   double acc[9] = {0,0,0,0,0,0,0,0,0};     // sum m*xipos, sum m*v_origin, sum m*omega
@@ -204,7 +204,7 @@ __device__ void walk_observe(const DevModel& m, const Warp w, const StepArgs& a,
 }
 
 // ObjHold obs / reward / done (obj_hold_v0.py:79-121): needs kinematics of the post-step state in scratch
-__device__ void hold_observe(const DevModel& m, const Warp w, const StepArgs& a, int env, double* rw_out, bool* done_out) {
+template <class MD> __device__ void hold_observe(const MD& m, const Warp w, const StepArgs& a, int env, double* rw_out, bool* done_out) {
   const myo_buffers& b = a.b; const int* ti = a.cfg.task_i; const double* td = a.cfg.task_d;
   int ob = ti[0]; const double* xp = SCR(s_xpos) + 3*ob; double op[3]; mat_vec(op, SCR(s_xmat) + 9*ob, td); op[0]+=xp[0]; op[1]+=xp[1]; op[2]+=xp[2];
   double err[3] = {W_(eprm)[0]-op[0], W_(eprm)[1]-op[1], W_(eprm)[2]-op[2]}, dist = sqrt(dot3(err, err));
@@ -219,12 +219,12 @@ __device__ void hold_observe(const DevModel& m, const Warp w, const StepArgs& a,
 }
 
 // |qvel dt| of the state in shared memory (the leg stand task's velocity term); out of line, so that the reach epilogue keeps its registers
-__device__ __noinline__ double qvel_dt_norm(const DevModel& m, const Warp w, const StepArgs& a) {
+template <class MD> __device__ __noinline__ double qvel_dt_norm(const MD& m, const Warp w, const StepArgs& a) {
   double v2 = 0; for (int i = w.lane; i < m.nv; i += 32) { const double v = W_(qvel)[i]*a.dt; v2 += v*v; }
   return sqrt(warp_sum(v2)); }
 
 // ReachEnvV0 obs / reward / done (reach_v0.py:98-160): needs kinematics of the post-step state in scratch.  tnow = mjData.time of that state
-__device__ void reach_observe(const DevModel& m, const Warp w, const StepArgs& a, int env, double tnow, double* rw_out, bool* done_out) {
+template <class MD> __device__ void reach_observe(const MD& m, const Warp w, const StepArgs& a, int env, double tnow, double* rw_out, bool* done_out) {
   const myo_buffers& b = a.b; const int* ti = a.cfg.task_i; const double* td = a.cfg.task_d; const int ntip = ti[0];
   float* o = b.obs ? b.obs + (size_t)env*a.obs_dim : nullptr; double d2 = 0, a2 = 0; const int base = m.nq + m.nv;
   if (w.lane < ntip) { int bd = ti[1+w.lane]; const double* lp = td + 3*w.lane; double tip[3] = {lp[0], lp[1], lp[2]};
@@ -246,7 +246,7 @@ __device__ void reach_observe(const DevModel& m, const Warp w, const StepArgs& a
 
 // obs / reward / done of the state held in shared memory, for any task (runs the extra forward stages the task needs)
 struct RwDone { double rw; int done; };   // returned by value (registers), not through pointers to the caller's stack
-__device__ __noinline__ RwDone task_observe(const DevModel& m, const Warp w, const StepArgs& a, int env, int steps, double tnow) {
+template <class MD> __device__ __noinline__ RwDone task_observe(const MD& m, const Warp w, const StepArgs& a, int env, int steps, double tnow) {
   double rw = 0; bool done = false;
   if (a.cfg.task == MYO_TASK_POSE) pose_reward_done(m, w, a, env, &rw, &done);
   else if (a.cfg.task == MYO_TASK_WALK) { phase_kinematics(m, w); phase_tendon_all(m, w); phase_actuation(m, w, false, m.g_ctrl + (size_t)env*m.nu, nullptr, nullptr); walk_observe(m, w, a, env, steps, &rw, &done); }
@@ -283,7 +283,7 @@ __device__ __forceinline__ void group_sync(int ngroups, int gid, int gthreads) {
 }
 
 // The stored state of `env` into this warp's slice (coalesced: one env's row per warp).  The inverse-wrap roots start cold.
-__device__ __forceinline__ void load_env_state(const DevModel& m, const Warp w, const myo_buffers& b, int env) {
+template <class MD> __device__ __forceinline__ void load_env_state(const MD& m, const Warp w, const myo_buffers& b, int env) {
   for (int i = w.lane; i < m.nq; i += 32) W_(qpos)[i] = b.qpos[(size_t)env*m.nq+i];
   for (int i = w.lane; i < m.nv; i += 32) { W_(qvel)[i] = b.qvel[(size_t)env*m.nv+i]; W_(qws)[i] = b.qacc_warmstart[(size_t)env*m.nv+i]; }
   for (int i = w.lane; i < m.na; i += 32) W_(act)[i] = b.act[(size_t)env*m.na+i];
@@ -296,7 +296,7 @@ __device__ __forceinline__ void load_env_state(const DevModel& m, const Warp w, 
 // The sides a column is perturbed to (mjd_stepFD): a state column always goes forward and goes back when centered; a ctrl column of an
 // actuator with ctrllimited goes forward when inRange(c, c + eps) and back when (centered || !fwd) && inRange(c - eps, c).
 struct FdCol { int col, ctrl; bool fwd, back; };      // ctrl: the actuator of a B column, -1 for an A column
-__device__ __forceinline__ FdCol fd_column(const DevModel& m, const StepArgs& a, int env, int col) {
+template <class MD> __device__ __forceinline__ FdCol fd_column(const MD& m, const StepArgs& a, int env, int col) {
   const bool centered = a.fd.npass == 2;
   FdCol c; c.col = col; c.ctrl = col < a.fd.nxa ? -1 : col - a.fd.nxa; c.fwd = true; c.back = centered;
   if (c.ctrl >= 0) { const double* __restrict__ pa = GD(PA_d) + CI(PA_cls)[c.ctrl]*PA_STRIDE;
@@ -309,7 +309,7 @@ __device__ __forceinline__ bool fd_minus(const StepArgs& a, const FdCol& c, int 
 __device__ __forceinline__ bool fd_runs(const StepArgs& a, const FdCol& c, int pass) { return fd_minus(a, c, pass) ? c.back : c.fwd; }
 
 // The perturbation of the start state already in the slice (load_env_state); a ctrl column's ctrl row goes to the slot's global row
-__device__ void fd_perturb(const DevModel& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, double* ctrl_row) {
+template <class MD> __device__ void fd_perturb(const MD& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, double* ctrl_row) {
   const double h = fd_minus(a, c, pass) ? -a.fd.eps : a.fd.eps;
   if (c.ctrl >= 0) { const double* src = a.roll.ctrl + (size_t)env*m.nu;
     for (int i = w.lane; i < m.nu; i += 32) ctrl_row[i] = i == c.ctrl ? src[i] + h : src[i]; }
@@ -324,7 +324,7 @@ __device__ void fd_perturb(const DevModel& m, const Warp w, const StepArgs& a, i
 // After a pass: the + pass of a centred column parks its result in the slot's row; the last pass writes the column of A or B
 //   both sides (x'+ (-) x'-) * rinv2, forward only (x'+ (-) x'0) * rinv1, back only (x'0 (-) x'-) * rinv1, neither 0
 // ((-): differentiate_pos on qpos, subtraction on qvel and act; x'0 from the nominal carry, the last pass's result in the slice).
-__device__ void fd_store(const DevModel& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, bool ran, double* prow) {
+template <class MD> __device__ void fd_store(const MD& m, const Warp w, const StepArgs& a, int env, const FdCol& c, int pass, bool ran, double* prow) {
   const int nq = m.nq, nv = m.nv, na = m.na, nx = 2*nv + na; const bool centered = a.fd.npass == 2;
   if (centered && pass == 0) {
     if (ran) { for (int i = w.lane; i < nq; i += 32) prow[i] = W_(qpos)[i];
@@ -362,8 +362,8 @@ __device__ void fd_store(const DevModel& m, const Warp w, const StepArgs& a, int
 // whose side the column does not take runs as an idle slot (live = false).  A pass loads the env's start state from a.b, perturbs it
 // (fd_perturb) and, after the substeps, parks or differences its result (fd_store); no state is stored back.
 // MAXT: launch bound (threads per CTA) -> register budget of the instantiation.
-template <bool DBG, int MAXT, bool ROLL = false, bool FD = false>
-__device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArgs& a) {
+template <bool DBG, int MAXT, bool ROLL = false, bool FD = false, class MD>
+__device__ __forceinline__ void env_kernel_body(const MD& m, const StepArgs& a) {
   __shared__ __align__(8) unsigned long long mbar;
   const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
   STAGE_MODEL(m, mbar)
@@ -483,7 +483,7 @@ __device__ __forceinline__ void env_kernel_body(const DevModel& m, const StepArg
       }
       __syncwarp();
       // ---- store state.  A forward pass without substeps runs the solve but not the integrator, so the warm start was not rewritten, and
-      // where it lives in the Hessian tail (fill_devmodel) the solve has overwritten it: the caller's warm start stays as it was.
+      // where it lives in the Hessian tail (model_layout) the solve has overwritten it: the caller's warm start stays as it was.
       const bool store_qws = !(DBG && a.mode == 1 && !integrate);
       for (int i = w.lane; i < m.nq; i += 32) b.qpos[(size_t)env*m.nq+i] = W_(qpos)[i];
       for (int i = w.lane; i < m.nv; i += 32) { b.qvel[(size_t)env*m.nv+i] = W_(qvel)[i]; if (store_qws) b.qacc_warmstart[(size_t)env*m.nv+i] = W_(qws)[i]; }
@@ -505,6 +505,9 @@ extern "C" __global__ void __launch_bounds__(320) myo_env_kernel(const __grid_co
 // the same product body under launch_bounds(448): 128 registers for the entry function, up to 14 env-warps per CTA.  Chosen when the model's
 // shared-memory footprint lets that many warps cut the number of rounds (hand, 4096 envs: 2 rounds of 14 instead of 3 of 10).
 extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
+// the same launch_bounds(448) product body on the hand's compile-time shape (HandShape): chosen instead of myo_env_kernel_w14 for a batch
+// whose DevModel matches that shape (batch_setup)
+extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14_hand(const __grid_constant__ HandShape m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
 // parity taps / forward-debug / profiling counters / tuning knobs
 extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<true, 320>(m, a); }
 // rollout (myo_batch_rollout): the product body's mode 0 with the caller's ctrl and applied forces, under the two product launch bounds
@@ -512,7 +515,7 @@ extern "C" __global__ void __launch_bounds__(320) myo_roll_kernel(const __grid_c
 extern "C" __global__ void __launch_bounds__(448) myo_roll_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448, true>(m, a); }
 // transition FD (myo_batch_transition_fd): the rollout body over (env, column) work items, under launch_bounds(320)
 extern "C" __global__ void __launch_bounds__(320) myo_fd_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320, true, true>(m, a); }
-static_assert(sizeof(DevModel) + sizeof(StepArgs) <= 4096, "the step kernels' arguments fit the 4 KB kernel parameter space");
+static_assert(sizeof(HandShape) + sizeof(StepArgs) <= 4096, "the step kernels' arguments fit the 4 KB kernel parameter space");
 
 // ------------------------------------------------------------------ mjData readout (myo_batch_data)
 // One forward pass over the stored state of every env, one env per warp on the balanced map (env = CTA + grid * slot).  Each field is
@@ -875,7 +878,7 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
 struct LaunchShape { int warps, smem, grid; };      // env-warps per CTA, dynamic shared memory (bytes), CTAs
 // Zero-initialised by myo_batch_create (new myo_batch()), so that myo_batch_destroy can free a partly built batch.
 struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
-  LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
+  LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14, use_hand; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
   int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
   LaunchShape inv_shape; bool inv_ready;      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
@@ -898,89 +901,19 @@ extern "C" int myo_model_from_blob(const int32_t* I, int64_t nI, const double* D
 }
 extern "C" void myo_model_destroy(myo_model* m) { delete m; }
 
-static int al2(int x) { return (x + 1) & ~1; }
-static int imax(int a, int b) { return a > b ? a : b; }
-// What fill_devmodel decided beyond the DevModel offsets (myo_model_layout): the size reserved for every persistent and scratch region
-// (slot orders of include/myo_b200.h) and the boundaries and flags of the scratch scheme, the latter relative to the scratch start.
-#define LP_ENUM(n) LP_##n,
-#define LS_ENUM(n) LS_##n,
-enum { MYO_LAYOUT_PERSISTENT(LP_ENUM) LP_N };
-enum { MYO_LAYOUT_SCRATCH(LS_ENUM) LS_N };
-#undef LP_ENUM
-#undef LS_ENUM
-struct Layout { int32_t psz[LP_N], ssz[LS_N], head, afterK, extNonSolve, solveEnd, arefInH, qwsInH; };
+// The DevModel of a model under a task configuration: its shape's dimensions and layout (model_layout), the staged tables and the scalars
 static void fill_devmodel(const myo_model* mm, const myo_task_cfg* cfg, DevModel& d, Layout* lay = nullptr) {
-  const int32_t* I = mm->I.data(); const double* D = mm->D.data(); memset(&d, 0, sizeof(d));
-  Layout L_; Layout& L = lay ? *lay : L_; memset(&L, 0, sizeof(L));
+  const int32_t* I = mm->I.data(); const double* D = mm->D.data(); const int32_t* P = MYO_ISEC(I, MYO_SEC_P_dims);
+  const bool hold = cfg && cfg->task == MYO_TASK_HOLD;
+  const ModelDims x = {MYO_DIM(I, MYO_DIM_nq), MYO_DIM(I, MYO_DIM_nv), MYO_DIM(I, MYO_DIM_nu), MYO_DIM(I, MYO_DIM_na), MYO_DIM(I, MYO_DIM_nM), MYO_DIM(I, MYO_DIM_njnt),
+    P[PD_NBD], P[PD_NLEVEL], P[PD_NSP], P[PD_NWE], P[PD_NTA], P[PD_NNZ], P[PD_NLIM], P[PD_NEQ], P[PD_NPAIR], P[PD_NPAIR_ANALYTIC], P[PD_MAXPATH], P[PD_NDEPTH],
+    P[PD_EQ_TREE], P[PD_NGC], P[PD_NWE_SPH_IN] + P[PD_NWE_CYL_IN], P[PD_NLIMROW], P[PD_SPLIT_SP], P[PD_SPLIT_WE], P[PD_SPLIT_TA], P[PD_SPLIT_NZ],
+    hold ? 8 : 0, hold ? cfg->task_i[1] : -1, cfg ? cfg->maxcon : 0};
+  const ModelLayout ml = model_layout(x); d = ml.d; if (lay) *lay = ml.L;
   const int32_t* hoff = MYO_ISEC(I, MYO_SEC_HOT_off);
   for (int s = 0; s < MYO_NSEC; s++) d.hoff[s] = hoff[s];
   d.nI16w = MYO_SEC_LEN(I, MYO_SEC_HOT_I16); d.nD = hoff[MYO_NSEC] >= 0 ? hoff[MYO_NSEC] : MYO_SEC_LEN(I, MYO_SEC_HOT_D);      // doubles staged to shared memory (the cold tables behind them stay in HBM)
-  d.nq = MYO_DIM(I, MYO_DIM_nq); d.nv = MYO_DIM(I, MYO_DIM_nv); d.nu = MYO_DIM(I, MYO_DIM_nu); d.na = MYO_DIM(I, MYO_DIM_na); d.nM = MYO_DIM(I, MYO_DIM_nM); d.njnt = MYO_DIM(I, MYO_DIM_njnt);
-  const int32_t* P = MYO_ISEC(I, MYO_SEC_P_dims);
-  d.nbd = P[PD_NBD]; d.nlevel = P[PD_NLEVEL]; d.nsp = P[PD_NSP]; d.nwe = P[PD_NWE]; d.nta = P[PD_NTA]; d.nnz = P[PD_NNZ]; d.nlim = P[PD_NLIM]; d.neq = P[PD_NEQ];
-  { const int sp_[3] = {0, P[PD_SPLIT_SP], d.nsp}, we_[3] = {0, P[PD_SPLIT_WE], d.nwe}, ta_[3] = {0, P[PD_SPLIT_TA], d.nta}, nz_[3] = {0, P[PD_SPLIT_NZ], d.nnz};
-    for (int k = 0; k < 3; k++) { d.tg_sp[k] = sp_[k]; d.tg_we[k] = we_[k]; d.tg_ta[k] = ta_[k]; d.tg_nz[k] = nz_[k]; } }
-  d.npair = P[PD_NPAIR]; d.npair_an = P[PD_NPAIR_ANALYTIC]; d.maxpath = P[PD_MAXPATH]; d.ndepth = P[PD_NDEPTH]; d.eq_tree = P[PD_EQ_TREE];
   const double* opt = MYO_DSEC(I, D, MYO_SEC_opt); d.timestep = opt[0]; d.gx = opt[1]; d.gy = opt[2]; d.gz = opt[3]; d.tolerance = opt[4]; d.meaninertia = opt[6];
-  d.ovr_geom = (cfg && cfg->task == MYO_TASK_HOLD) ? cfg->task_i[1] : -1;
-  int mc = cfg && cfg->maxcon > 0 ? cfg->maxcon : 32; if (mc > 64) mc = 64; if (mc > 2*d.npair) mc = 2*d.npair; /* (the contact-order merge handles up to 64) */ d.maxcon = mc; d.nlimrow = P[PD_NLIMROW] > 0 ? P[PD_NLIMROW] : 2*d.nlim; d.maxefc = d.neq + d.nlimrow + 4*mc;
-  int o = 0;
-  #define TAKE(field, n) d.o_##field = o; L.psz[LP_##field] = al2(n); o += al2(n)
-  // persistent per-env arrays.  ctrl is NOT here: it is written once per control step to a library-owned global row and re-read by the actuation
-  // phase of every substep (an L2 hit); the solver's warm start lives in the tail of the Hessian region when that tail is provably idle (below).
-  TAKE(qpos, d.nq); TAKE(qvel, d.nv); TAKE(act, d.na); TAKE(dax, 3*d.nv); TAKE(dan, 3*d.nv); TAKE(qM, d.nM); TAKE(fsm, d.nv);
-  d.neprm = (cfg && cfg->task == MYO_TASK_HOLD) ? 8 : 0; TAKE(eprm, d.neprm); d.nwz = P[PD_NWE_SPH_IN] + P[PD_NWE_CYL_IN]; TAKE(wz, d.nwz); TAKE(cnt, CNT_N/2);
-  d.nvp = chol_pad(d.nv); L.psz[LP_qws] = al2(d.nv);
-  const int o_qws_persistent = o;          // (claimed only if the warm start cannot alias the Hessian tail)
-  // ---- scratch, time-multiplexed by stage (offsets from d.o_scr, fixed up at the end).  Lifetimes:
-  //   head: icon (contact / row integer records), con (contact records)     collision .. constraints ; in the solve the con region holds jar, jv
-  //   K   (xpos, xmat)                                                      kinematics .. collision              -> right after the head
-  //   T   (U, PL, mom, tlen, tvel, tfrc)                                    tendon .. actuation                  -> around K
-  //   C   (cin, crb, bf)                                                    body inertia .. bias                 -> around K
-  //   G   (gpose, clist)                                                    collision                            -> after K
-  //   S   (conJ 48-bit, D, eqJ, a, g|p, Ma, Mp, H | Hs LD Dinv, aref->H)   constraints .. integrate             -> after the head (K is dead)
-  const int icon = al2(mc + (mc + 1)/2 + (2*(mc + d.nlimrow + 4) + d.maxefc + 7)/8);       // cmask u64[mc] | crown i32[mc] | cpair i16[mc] | lrow i16[nlimrow+4] | drow u8[maxefc]
-  const int rows = al2(d.maxefc), conReg = imax(al2(CON_STRIDE*mc), 2*rows), K = al2(3*d.nbd) + al2(9*d.nbd);
-  d.s_icon = 0; d.s_con = icon; d.s_efR = icon; d.s_efV = icon + rows; const int head = icon + conReg;
-  L.ssz[LS_icon] = icon; L.ssz[LS_con] = conReg; L.ssz[LS_efR] = rows; L.ssz[LS_efV] = rows;
-  d.s_xpos = head; d.s_xmat = head + al2(3*d.nbd); const int afterK = head + K; L.ssz[LS_xpos] = al2(3*d.nbd); L.ssz[LS_xmat] = al2(9*d.nbd);
-  int c0, c1, ext;      // two cursors: inside [0, head) and after K
-  #define PLACE(field, n) { const int n_ = al2(n); L.ssz[LS_##field] = n_; if (c0 + n_ <= head) { d.s_##field = c0; c0 += n_; } else { d.s_##field = c1; c1 += n_; } }
-  c0 = 0; c1 = afterK;
-  PLACE(mom, d.nnz); PLACE(tlen, d.nta); PLACE(tvel, d.nta); PLACE(tfrc, d.nta); { const int nsA = d.tg_sp[1], nsB = d.nsp - nsA, nwA = d.tg_we[1], nwB = d.nwe - nwA;      // one tendon group at a time lives in U / PL
-    PLACE(PL, imax(nsA + nwA, nsB + nwB)); PLACE(U, 3*imax(nsA + 2*nwA, nsB + 2*nwB)); }
-  ext = c1;
-  c0 = 0; c1 = afterK;
-  PLACE(cin, 10*d.nbd); PLACE(crb, 10*d.nbd); PLACE(bf, 6*d.nbd);
-  ext = imax(ext, c1);
-  d.kcand = d.npair - d.npair_an; d.ngc = P[PD_NGC];
-  d.s_gpose = afterK; d.s_clist = afterK + al2(6*d.ngc); ext = imax(ext, d.s_clist + al2((d.kcand + 1)/2)); L.ssz[LS_gpose] = al2(6*d.ngc); L.ssz[LS_clist] = al2((d.kcand + 1)/2);
-  ext = imax(ext, d.s_gpose + al2(2*d.njnt));      // the hinge sines / cosines of the kinematics phase (phase_kinematics)
-  const int extNonSolve = ext;
-  int t = head;
-  L.ssz[LS_conJ] = al2(imax((3*d.maxpath*mc*JAC_BYTES + 7)/8, (mc + 1)/2)); L.ssz[LS_efD] = al2(d.neq + d.nlimrow + mc); L.ssz[LS_eqJ] = al2(d.neq);
-  d.s_conJ = t; t += L.ssz[LS_conJ]; d.s_efD = t; t += L.ssz[LS_efD]; d.s_eqJ = t; t += L.ssz[LS_eqJ];      /* (the Jacobian region doubles as the int rank keys of the contact ordering) */
-  d.s_va = t; t += al2(d.nvp); d.s_vg = t; d.s_vp = t; t += al2(d.nvp); d.s_vMa = t; t += al2(d.nvp); d.s_vMp = t; t += al2(d.nvp);
-  L.ssz[LS_va] = L.ssz[LS_vg] = L.ssz[LS_vp] = L.ssz[LS_vMa] = L.ssz[LS_vMp] = al2(d.nvp);
-  const int hsize = imax(al2(d.nvp*(d.nvp+1)/2), 2*al2(d.nM) + al2(d.nv)); const bool arefInH = rows <= hsize;
-  d.s_efA = t; if (!arefInH) t += rows;      /* aref (constraints -> start of the solve) lives in the Hessian region when it fits: H is first written after its last read */
-  d.s_H = t; d.s_Hs = t; d.s_LD = t + al2(d.nM); d.s_Dinv = t + 2*al2(d.nM); if (arefInH) d.s_efA = t; t += hsize;
-  L.ssz[LS_efA] = rows; L.ssz[LS_H] = hsize; L.ssz[LS_Hs] = L.ssz[LS_LD] = al2(d.nM); L.ssz[LS_Dinv] = hsize - 2*al2(d.nM);
-  // warm start in the last nv slots of the Hessian region: read once at the start of the solve (before any write to H), rewritten at the end
-  // of the integrator (after the last read of H).  Requires that no other stage reaches that far and that aref (head of H) does not overlap it.
-  int qws = t - al2(d.nv);
-  const bool qwsInH = qws >= extNonSolve && (!arefInH || d.s_H + rows <= qws) && d.s_H + al2(d.nvp*(d.nvp+1)/2) <= t;
-  ext = imax(ext, t);
-  int scratch = ext;
-  if (qwsInH) { d.o_scr = o; d.o_qws = o + qws; } else { d.o_qws = o_qws_persistent; o += al2(d.nv); d.o_scr = o; }
-  L.psz[LP_scr] = scratch; L.head = head; L.afterK = afterK; L.extNonSolve = extNonSolve; L.solveEnd = t; L.arefInH = arefInH; L.qwsInH = qwsInH;
-  #undef PLACE
-  #undef TAKE
-  // scratch offsets are used relative to the warp base
-  #define TO_WARP(n) d.s_##n += d.o_scr;
-  MYO_LAYOUT_SCRATCH(TO_WARP)
-  #undef TO_WARP
-  d.n_per_warp = d.o_scr + scratch;
 }
 
 extern "C" int myo_model_dims(const myo_model* m, const myo_task_cfg* cfg, myo_dims* out) {
@@ -1057,8 +990,10 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
   if (launch_shape((const void*)myo_env_kernel, prop, per, b->const_bytes, n_env, big, 0, sp) || launch_shape((const void*)myo_env_kernel_w14, prop, per, b->const_bytes, n_env, big, 0, sw)) return -1;
   b->use_w14 = sw.warps > sp.warps && rounds_of(sw) < rounds_of(sp);      // (small models too: the elbow runs 4096 envs in 2 rounds of 14 warps instead of 3 of 10 -- registers, not shared memory, keep it at one CTA per SM)
   if (const char* e = getenv("MYO_B200_W14")) b->use_w14 = atoi(e) != 0 && fa_w.maxThreadsPerBlock > fa_p.maxThreadsPerBlock;      // tuning override
+  b->use_hand = b->use_w14 && HandShape::matches(b->dm);      // the w14 launch, compiled for this batch's shape
+  const void* prod_fn = b->use_hand ? (const void*)myo_env_kernel_w14_hand : b->use_w14 ? (const void*)myo_env_kernel_w14 : (const void*)myo_env_kernel;
   const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;      // tuning override (never above what fits)
-  if (launch_shape(b->use_w14 ? (const void*)myo_env_kernel_w14 : (const void*)myo_env_kernel, prop, per, b->const_bytes, n_env, big, want, b->prod) ||
+  if (launch_shape(prod_fn, prop, per, b->const_bytes, n_env, big, want, b->prod) ||
       launch_shape((const void*)myo_env_kernel_dbg, prop, per, b->const_bytes, n_env, big, want, b->dbg)) return -1;
   b->balanced = b->prod.smem > 100*1024; b->dbg_balanced = b->dbg.smem > 100*1024;      // the balanced slot map for CTAs that fill an SM
   // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
@@ -1076,7 +1011,7 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
   // that a caller whose first launch goes to a non-blocking stream finds the model and the zeroed rows in place
   CUDA_OK(cudaStreamSynchronize(cudaStreamLegacy));
   if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
-    n_env, b->use_w14 ? "launch_bounds(448)" : "launch_bounds(320)", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
+    n_env, b->use_hand ? "myo_env_kernel_w14_hand" : b->use_w14 ? "myo_env_kernel_w14" : "myo_env_kernel", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
   return 0;
 }
 
@@ -1098,15 +1033,16 @@ extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(
   cudaFree(b->dCarry); cudaFree(b->dFdRows); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
-// Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 8) written):
-// use_w14, warps_per_cta, grid, rounds per CTA, regroup, balanced, smem_bytes, perm_slots.
+// Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 9) written):
+// use_w14, warps_per_cta, grid, rounds per CTA, regroup, balanced, smem_bytes, perm_slots, hand_shape (1: the launch_bounds(448) kernel is
+// myo_env_kernel_w14_hand, compiled for the hand's shape).
 extern "C" int myo_batch_launch_info(const myo_batch* b, int32_t* out, int n) {
   if (!b || !out || n < 1) return fail("myo_batch_launch_info: bad arguments");
   const int nw = b->prod.warps, grid = b->prod.grid;
   // per_cta and the round loop of env_kernel_body (for j0 = 0; j0 < per_cta; j0 += nw)
   const int per_cta = b->regroup ? b->perm_rounds*nw : SLOTS_PER_CTA(b->balanced, b->n_env, grid, nw);
-  const int32_t v[8] = {b->use_w14 ? 1 : 0, nw, grid, (per_cta + nw - 1)/nw, b->regroup ? 1 : 0, b->balanced, b->prod.smem, b->perm_slots};
-  for (int i = 0; i < n && i < 8; i++) out[i] = v[i];
+  const int32_t v[9] = {b->use_w14 ? 1 : 0, nw, grid, (per_cta + nw - 1)/nw, b->regroup ? 1 : 0, b->balanced, b->prod.smem, b->perm_slots, b->use_hand ? 1 : 0};
+  for (int i = 0; i < n && i < 9; i++) out[i] = v[i];
   return 0;
 }
 // Slot -> env map (-1 = idle slot) the last env step ran with: slot blockIdx.x + grid*(round*warps_per_cta + warp).  Synchronises the device.
@@ -1169,7 +1105,8 @@ static int launch(myo_batch* b, StepArgs& a, void* stream) {
     if (a.mode == 0 && b->regroup) {      // env steps: regroup by last step's load first (same stream), then step through the permutation
       myo_regroup_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots);
       a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; b->perm_built = true; b->launches++; }
-    if (b->use_w14) myo_env_kernel_w14<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
+    if (b->use_hand) { HandShape hm; static_cast<DevModel&>(hm) = b->dm; myo_env_kernel_w14_hand<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(hm, a); }
+    else if (b->use_w14) myo_env_kernel_w14<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
     else myo_env_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a); }
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

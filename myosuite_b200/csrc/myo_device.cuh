@@ -47,7 +47,7 @@ struct DevModel {
   double timestep, gx, gy, gz, meaninertia, tolerance;
   // per-warp shared-memory layout, in doubles.  Persistent part:
   int32_t o_qpos, o_qvel, o_act, o_qws, o_dax, o_dan, o_qM, o_fsm, o_eprm, neprm, o_wz, nwz, o_cnt, o_scr, n_per_warp;
-  // scratch (time-multiplexed by stage; offsets relative to the warp base, i.e. o_scr included).  See fill_devmodel() for the overlap rules.
+  // scratch (time-multiplexed by stage; offsets relative to the warp base, i.e. o_scr included).  See model_layout() (myo_layout.cuh) for the overlap rules.
   int32_t s_xpos, s_xmat;                                  // K: body poses, alive kinematics .. constraints
   int32_t s_U, s_PL, s_mom, s_tlen, s_tvel, s_tfrc;  // stage 1: tendons + actuation
   int32_t s_cin, s_crb, s_bf;                              // stage 2: CRB / bias
@@ -113,18 +113,18 @@ __device__ __forceinline__ double m_sqrt(double x) { double y; asm("rsqrt.approx
 #define FDIV(a, b) ((a)*m_rcp(b))
 
 // world position of program point `pt`
-__device__ __forceinline__ void world_point(const DevModel& m, const Warp w, int pt, double* out) {
+template <class MD> __device__ __forceinline__ void world_point(const MD& m, const Warp w, int pt, double* out) {
   int b = CI(PPT_body)[pt]; const double* __restrict__ xg = GD(PPT_xyz) + 3*pt; const double x[3] = {LDC(xg), LDC(xg+1), LDC(xg+2)};
   if (b < 0) { out[0]=x[0]; out[1]=x[1]; out[2]=x[2]; }
   else { const double* xp = SCR(s_xpos) + 3*b; mat_vec(out, SCR(s_xmat) + 9*b, x); out[0]+=xp[0]; out[1]+=xp[1]; out[2]+=xp[2]; } }
 
 // spatial motion vector of dof d about the world origin: [omega ; velocity of the point at the origin]
-__device__ __forceinline__ void dof_motion(const DevModel& m, const Warp w, int d, double* S) {
+template <class MD> __device__ __forceinline__ void dof_motion(const MD& m, const Warp w, int d, double* S) {
   const double* ax = W_(dax) + 3*d;
   if (CI(PD_lin)[d]) { S[0]=S[1]=S[2]=0; S[3]=ax[0]; S[4]=ax[1]; S[5]=ax[2]; }
   else { S[0]=ax[0]; S[1]=ax[1]; S[2]=ax[2]; cross3(S+3, W_(dan) + 3*d, ax); } }
 // velocity of world point p due to unit rate of dof d
-__device__ __forceinline__ void dof_point_vel(const DevModel& m, const Warp w, int d, const double* p, double* c) {
+template <class MD> __device__ __forceinline__ void dof_point_vel(const MD& m, const Warp w, int d, const double* p, double* c) {
   const double* ax = W_(dax) + 3*d;
   if (CI(PD_lin)[d]) { c[0]=ax[0]; c[1]=ax[1]; c[2]=ax[2]; }
   else { double r[3] = {p[0]-W_(dan)[3*d], p[1]-W_(dan)[3*d+1], p[2]-W_(dan)[3*d+2]}; cross3(c, ax, r); } }
@@ -137,7 +137,7 @@ __device__ __forceinline__ void inert_mul(double* f, const double* ic, const dou
 
 // ------------------------------------------------------------------ phase 1: kinematics (rotation matrices, level by level)
 // also writes each dynamic body's spatial inertia about the world origin (cin) into the stage-2 scratch
-__device__ void phase_kinematics(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_kinematics(const MD& m, const Warp w) {
   const idx_t* level = CI(PB_level_adr); const idx_t* par = CI(PB_parent); const idx_t* jadr = CI(PB_jadr); const idx_t* jnum = CI(PB_jnum);
   const double* PB = CD(PB_d);
   const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr);
@@ -192,7 +192,7 @@ __device__ void phase_kinematics(const DevModel& m, const Warp w) {
 }
 
 // spatial inertia of every dynamic body about the world origin (needs final poses; writes stage-2 scratch)
-__device__ void phase_body_inertia(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_body_inertia(const MD& m, const Warp w) {
   const double* PB = CD(PB_d); const double* xpos = SCR(s_xpos); const double* xmat = SCR(s_xmat); double* cin = SCR(s_cin);
   for (int k = w.lane; k < m.nbd; k += 32) { const double* bd = PB + k*PB_STRIDE; const double* R = xmat + 9*k;
     double c3[3]; mat_vec(c3, R, bd + 12); c3[0]+=xpos[3*k]; c3[1]+=xpos[3*k+1]; c3[2]+=xpos[3*k+2];
@@ -279,7 +279,7 @@ __device__ __forceinline__ double wrap2d_inside(double* pnt, const double* d, do
   pnt[0] = rad*(c*vx - s*vy); pnt[1] = rad*(s*vx + c*vy); pnt[2] = pnt[0]; pnt[3] = pnt[1];
   return 0; }
 
-__device__ void wrap_element(const DevModel& m, const Warp w, int k, int g, double* U, double* PL) {
+template <class MD> __device__ void wrap_element(const MD& m, const Warp w, int k, int g, double* U, double* PL) {
   const idx_t* we = CI(PWE) + 6*k; const double* __restrict__ wdg = GD(PWE_d) + k*PWE_STRIDE;      // (cold table: 16 independent read-only loads per element)
   double wd[12]; for (int c = 0; c < 12; c++) wd[c] = LDC(wdg + c);
   double x0[3], x1[3]; world_point(m, w, we[0], x0); world_point(m, w, we[1], x1);
@@ -326,7 +326,7 @@ __device__ void wrap_element(const DevModel& m, const Warp w, int k, int g, doub
 }
 
 // One tendon group (pass): straight segments and wrap elements of the group into the group-local unit-vector / piece-length scratch
-__device__ void phase_tendon(const DevModel& m, const Warp w, int g) {
+template <class MD> __device__ void phase_tendon(const MD& m, const Warp w, int g) {
   double* U = SCR(s_U); double* PL = SCR(s_PL);
   const idx_t* sp = CI(PSP); const int s0 = m.tg_sp[g], s1 = m.tg_sp[g+1];
   for (int k = s0 + w.lane; k < s1; k += 32) { double a[3], b[3]; world_point(m, w, sp[2*k], a); world_point(m, w, sp[2*k+1], b); const int kl = k - s0;
@@ -338,7 +338,7 @@ __device__ void phase_tendon(const DevModel& m, const Warp w, int g) {
   __syncwarp();
 }
 // second half of a pass: moments per structural non-zero and tendon lengths of the group
-__device__ void phase_tendon_moments(const DevModel& m, const Warp w, int g) {
+template <class MD> __device__ void phase_tendon_moments(const MD& m, const Warp w, int g) {
   double* U = SCR(s_U); double* PL = SCR(s_PL); double* mom = SCR(s_mom); double* tlen = SCR(s_tlen);
   const idx_t* nzd = CI(PNZ_dof); const idx_t* tadr = CI(PNZ_term_adr); const idx_t* term = CI(PTERM);
   for (int z = m.tg_nz[g] + w.lane; z < m.tg_nz[g+1]; z += 32) { int d = nzd[z]; double acc = 0;
@@ -355,7 +355,7 @@ __device__ void phase_tendon_moments(const DevModel& m, const Warp w, int g) {
   __syncwarp();
 }
 // after both passes: tendon velocities (moment . qvel); tendon forces start at zero
-__device__ void phase_tendon_velocity(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_tendon_velocity(const MD& m, const Warp w) {
   const double* mom = SCR(s_mom); double* tvel = SCR(s_tvel); double* tfrc = SCR(s_tfrc);
   const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof);
   for (int t = w.lane; t < m.nta; t += 32) { double v = 0;
@@ -365,7 +365,7 @@ __device__ void phase_tendon_velocity(const DevModel& m, const Warp w) {
   __syncwarp();
 }
 // both passes (groups A, B) + velocities: the whole tendon stage
-__device__ __forceinline__ void phase_tendon_all(const DevModel& m, const Warp w) {
+template <class MD> __device__ __forceinline__ void phase_tendon_all(const MD& m, const Warp w) {
   #pragma unroll 1
   for (int g = 0; g < 2; g++) if (m.tg_ta[g+1] > m.tg_ta[g]) { phase_tendon(m, w, g); phase_tendon_moments(m, w, g); }
   phase_tendon_velocity(m, w);
@@ -381,7 +381,7 @@ __device__ __forceinline__ double muscle_FL(double L, double lmin, double lmax) 
   return 0; }
 
 // tap_force / tap_len: nullable global rows for the parity taps (values before the activation is advanced)
-__device__ void phase_actuation(const DevModel& m, const Warp w, bool integrate, const double* ctrl_row, double* tap_force, double* tap_len) {
+template <class MD> __device__ void phase_actuation(const MD& m, const Warp w, bool integrate, const double* ctrl_row, double* tap_force, double* tap_len) {
   const idx_t* atend = CI(PA_tendon); const idx_t* acls = CI(PA_cls); const double* __restrict__ PAc = GD(PA_d); const double* __restrict__ PAm = GD(PAM_d);      // (cold tables: 17 + 5 independent read-only loads per actuator)
   double* tlen = SCR(s_tlen); double* tvel = SCR(s_tvel); double* tfrc = SCR(s_tfrc); double* mom = SCR(s_mom);
   for (int i = w.lane; i < m.nu; i += 32) { double a[PA_STRIDE]; { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; for (int c = 0; c < 16; c++) a[c] = LDC(ag + c); } double am[5]; for (int c = 0; c < 5; c++) am[c] = LDC(PAm + i*PAM_STRIDE + c); int t = atend[i];
@@ -418,7 +418,7 @@ __device__ void phase_actuation(const DevModel& m, const Warp w, bool integrate,
 }
 
 // ------------------------------------------------------------------ phase 4: composite inertia -> joint-space mass matrix
-__device__ void phase_crb(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_crb(const MD& m, const Warp w) {
   double* crb = SCR(s_crb); const double* cin = SCR(s_cin); const idx_t* sadr = CI(PSUB_adr); const idx_t* sub = CI(PSUB);
   for (int k = w.lane; k < m.nbd; k += 32) { double acc[10] = {0,0,0,0,0,0,0,0,0,0};
     #pragma unroll 1
@@ -438,7 +438,7 @@ __device__ void phase_crb(const DevModel& m, const Warp w) {
 }
 
 // ------------------------------------------------------------------ phase 5: Coriolis/centrifugal/gravity bias (subtracts from fsm)
-__device__ void phase_bias(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_bias(const MD& m, const Warp w) {
   double* bf = SCR(s_bf); const double* cin = SCR(s_cin); const idx_t* cadr = CI(PCH_adr); const idx_t* ch = CI(PCH);
   for (int k = w.lane; k < m.nbd; k += 32) {
     double v[6] = {0,0,0,0,0,0}, vh[6] = {0,0,0,0,0,0}, a[6] = {0,0,0,-m.gx,-m.gy,-m.gz};
@@ -464,19 +464,19 @@ __device__ void phase_bias(const DevModel& m, const Warp w) {
 
 // ------------------------------------------------------------------ phase 6: collision (analytic primitives)
 // world position and z axis of every collision geom, once per substep (each geom takes part in ~20 pairs)
-__device__ __forceinline__ void geom_pose_all(const DevModel& m, const Warp w) {
+template <class MD> __device__ __forceinline__ void geom_pose_all(const MD& m, const Warp w) {
   double* GP = SCR(s_gpose);
   for (int g = w.lane; g < m.ngc; g += 32) { int b = CI(PG_body)[g]; const double* gd = CD(PG_d) + g*PG_STRIDE; double* o = GP + 6*g;
     if (b < 0) { o[0]=gd[0]; o[1]=gd[1]; o[2]=gd[2]; o[3]=gd[5]; o[4]=gd[8]; o[5]=gd[11]; }
     else { const double* X = SCR(s_xmat) + 9*b; const double* xp = SCR(s_xpos) + 3*b; mat_vec(o, X, gd); o[0]+=xp[0]; o[1]+=xp[1]; o[2]+=xp[2];
       double z[3] = {gd[5], gd[8], gd[11]}; mat_vec(o+3, X, z); } }
   __syncwarp(); }
-__device__ __forceinline__ void geom_pose(const DevModel& m, const Warp w, int g, double* pos, double* axis /* z column */) {
+template <class MD> __device__ __forceinline__ void geom_pose(const MD& m, const Warp w, int g, double* pos, double* axis /* z column */) {
   const double* o = SCR(s_gpose) + 6*g; pos[0]=o[0]; pos[1]=o[1]; pos[2]=o[2]; axis[0]=o[3]; axis[1]=o[4]; axis[2]=o[5]; }
 
-__device__ __forceinline__ const double* geom_size(const DevModel& m, const Warp w, int g) { return g == m.ovr_geom ? W_(eprm) + 3 : CD(PG_d) + g*PG_STRIDE + 12; }
+template <class MD> __device__ __forceinline__ const double* geom_size(const MD& m, const Warp w, int g) { return g == m.ovr_geom ? W_(eprm) + 3 : CD(PG_d) + g*PG_STRIDE + 12; }
 // full world rotation of a collision geom (ellipsoids need it)
-__device__ __forceinline__ void geom_mat(const DevModel& m, const Warp w, int g, double* mat) {
+template <class MD> __device__ __forceinline__ void geom_mat(const MD& m, const Warp w, int g, double* mat) {
   int b = CI(PG_body)[g]; const double* gd = CD(PG_d) + g*PG_STRIDE;
   if (b < 0) {
     #pragma unroll
@@ -551,7 +551,7 @@ __device__ __forceinline__ void plane_sph(ConOut& o, double margin, const double
   double off = r+0.5*dist;
   con_put(o, dist, sp[0]-pn[0]*off, sp[1]-pn[1]*off, sp[2]-pn[2]*off, pn[0], pn[1], pn[2]); }
 
-__device__ __forceinline__ void collide_analytic(const DevModel& m, const Warp w, int p, ConOut& o) {
+template <class MD> __device__ __forceinline__ void collide_analytic(const MD& m, const Warp w, int p, ConOut& o) {
   const idx_t* pr = CI(PPAIR) + PPAIR_ISTRIDE*p; const double* pd = CD(PPAIR_d) + pr[6]*PPAIR_STRIDE;
   int g1 = pr[0], g2 = pr[1], ct = pr[5]; double margin = pd[0]; o.n = 0; o.has_y = false;
   const double* s1 = geom_size(m, w, g1); const double* s2 = geom_size(m, w, g2);
@@ -591,7 +591,7 @@ __device__ __forceinline__ void collide_analytic(const DevModel& m, const Warp w
   }
 }
 
-__device__ __forceinline__ void collide_ellipsoid(const DevModel& m, const Warp w, int p, ConOut& o) {
+template <class MD> __device__ __forceinline__ void collide_ellipsoid(const MD& m, const Warp w, int p, ConOut& o) {
   const idx_t* pr = CI(PPAIR) + PPAIR_ISTRIDE*p; const double* pd = CD(PPAIR_d) + pr[6]*PPAIR_STRIDE;
   int g1 = pr[0], g2 = pr[1], ct = pr[5]; double margin = pd[0]; o.n = 0; o.has_y = false;
   const double* s1 = geom_size(m, w, g1); const double* s2 = geom_size(m, w, g2);
@@ -646,7 +646,7 @@ __device__ __forceinline__ void collide_ellipsoid(const DevModel& m, const Warp 
 }
 
 // cheap conservative test for the iterative (ellipsoid) colliders: can this pair be within its margin at all?
-__device__ __forceinline__ bool expensive_candidate(const DevModel& m, const Warp w, int p) {
+template <class MD> __device__ __forceinline__ bool expensive_candidate(const MD& m, const Warp w, int p) {
   const idx_t* pr = CI(PPAIR) + PPAIR_ISTRIDE*p; const double* pd = CD(PPAIR_d) + pr[6]*PPAIR_STRIDE;
   int g1 = pr[0], g2 = pr[1]; const double* s1 = geom_size(m, w, g1); const double* s2 = geom_size(m, w, g2); double margin = pd[0];
   double x1[3], a1[3], x2[3], a2[3]; geom_pose(m, w, g1, x1, a1); geom_pose(m, w, g2, x2, a2);
@@ -664,7 +664,7 @@ __device__ __forceinline__ bool expensive_candidate(const DevModel& m, const War
   double R1[9], R2[9], b[3], c[3], icd = m_rcp(cd), d[3] = {dv[0]*icd, dv[1]*icd, dv[2]*icd}; geom_mat(m, w, g1, R1); geom_mat(m, w, g2, R2); matT_vec(b, R1, d); matT_vec(c, R2, d);
   return cd - m_sqrt(s1[0]*s1[0]*b[0]*b[0]+s1[1]*s1[1]*b[1]*b[1]+s1[2]*s1[2]*b[2]*b[2]) - m_sqrt(s2[0]*s2[0]*c[0]*c[0]+s2[1]*s2[1]*c[1]*c[1]+s2[2]*s2[2]*c[2]*c[2]) <= margin; }
 
-__device__ __forceinline__ void store_contact(const DevModel& m, double* con, idx_t* icon, int ci, int p, const Con1& c, const ConOut& o) {
+template <class MD> __device__ __forceinline__ void store_contact(const MD& m, double* con, idx_t* icon, int ci, int p, const Con1& c, const ConOut& o) {
   if (ci >= m.maxcon) return;
   double* cd = con + ci*CON_STRIDE; cd[0] = c.dist; cd[1] = c.px; cd[2] = c.py; cd[3] = c.pz;
   double* f = cd + 4; f[0] = c.nx; f[1] = c.ny; f[2] = c.nz;
@@ -681,7 +681,7 @@ __device__ __forceinline__ void store_contact(const DevModel& m, double* con, id
 // order; phase_constraints ranks them into ONE model-pair order (contact reporting, numbering of the constraint rows) without moving records.
 // Overflow (more contacts than maxcon, or more surviving ellipsoid candidates than kcand): the extra ones are dropped first-come and
 // CNT_overflow is set; the step kernel ORs it into the caller's sticky per-env `overflow` buffer.
-__device__ void phase_collision(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_collision(const MD& m, const Warp w) {
   double* con = SCR(s_con); idx_t* icon = S_cpair;
   int ncon = 0, overflow = 0;
   geom_pose_all(m, w);

@@ -71,12 +71,12 @@ __device__ __forceinline__ double impedance(const double* si, double pos, double
   return si[0]+y*(si[1]-si[0]); }
 
 // y = M x using the per-row non-zero lists
-__device__ __forceinline__ void mul_M(const DevModel& m, const Warp w, double* y, const double* x) {
+template <class MD> __device__ __forceinline__ void mul_M(const MD& m, const Warp w, double* y, const double* x) {
   const idx_t* radr = CI(PROW_adr); const idx_t* rcol = CI(PROW_col); const idx_t* ridx = CI(PROW_idx);
   for (int i = w.lane; i < m.nv; i += 32) { double s = 0; for (int e = radr[i]; e < radr[i+1]; e++) s += W_(qM)[ridx[e]]*x[rcol[e]]; y[i] = s; } }
 
 // out[r] = (J x)_r for every constraint row
-__device__ void rows_apply(const DevModel& m, const Warp w, const double* x, double* out) {
+template <class MD> __device__ void rows_apply(const MD& m, const Warp w, const double* x, double* out) {
   SHARED_PTR(x); SHARED_PTR(out);
   const idx_t* eq = CI(PEQ); const int nlimrow = WI_(nlimrow), ncon = WI_(ncon);
   for (int e = w.lane; e < m.neq; e += 32) { double v = x[eq[PEQ_ISTRIDE*e+1]]; if (eq[PEQ_ISTRIDE*e+3] >= 0) v += S_eqJ[e]*x[eq[PEQ_ISTRIDE*e+3]]; out[e] = v; }
@@ -94,7 +94,7 @@ __device__ void rows_apply(const DevModel& m, const Warp w, const double* x, dou
 // normal / tangent weights in place).  Contacts are GATHERED: lane d owns vec[d] and walks the contact list, testing its bit in each contact's
 // path mask; the position of d in the contact's Jacobian is the number of lower bits set (paths list dofs in ascending order).  No lane
 // waits for another contact's rows: round 1 looped over the contacts with a warp sync and <= 8 busy lanes per contact.
-__device__ void rows_applyT_add(const DevModel& m, const Warp w, double* wgt, double* vec) {
+template <class MD> __device__ void rows_applyT_add(const MD& m, const Warp w, double* wgt, double* vec) {
   SHARED_PTR(wgt); SHARED_PTR(vec);
   const idx_t* eq = CI(PEQ); const int nlimrow = WI_(nlimrow), ncon = WI_(ncon);
   if (w.lane == 0) for (int e = 0; e < m.neq; e++) { vec[eq[PEQ_ISTRIDE*e+1]] += wgt[e]; if (eq[PEQ_ISTRIDE*e+3] >= 0) vec[eq[PEQ_ISTRIDE*e+3]] += S_eqJ[e]*wgt[e]; }
@@ -124,7 +124,7 @@ __device__ __forceinline__ double eq_residual(const double* c, const double* qpo
   if (q2 >= 0) { double x = qpos[q2]-c[6]; deriv = c[1]+x*(2*c[2]+x*(3*c[3]+x*4*c[4])); return pos0-(c[0]+x*(c[1]+x*(c[2]+x*(c[3]+x*c[4])))); }
   deriv = 0; return pos0-c[0]; }
 
-__device__ void phase_constraints(const DevModel& m, const Warp w) {
+template <class MD> __device__ void phase_constraints(const MD& m, const Warp w) {
   // joint equalities (always active)
   const idx_t* eq = CI(PEQ); const double* eqd = CD(PEQ_d);
   for (int e = w.lane; e < m.neq; e += 32) { const double* c = eqd + e*PEQ_STRIDE; int q1 = eq[PEQ_ISTRIDE*e], d1 = eq[PEQ_ISTRIDE*e+1], q2 = eq[PEQ_ISTRIDE*e+2], d2 = eq[PEQ_ISTRIDE*e+3];
@@ -349,7 +349,7 @@ __device__ __noinline__ void chol_rs32b(double* H, double* x, int n, int lane) {
 }
 
 // padded order of the dense solver for an n x n system (the order of the chol_rs instance that solves it; H and the solver vectors are laid out for it)
-__host__ __device__ __forceinline__ int chol_pad(int n) { return n > 32 ? n : (n <= 8 ? 8 : (n == 23 || n == 29 ? n : (n + 3) & ~3)); }
+__host__ __device__ __forceinline__ constexpr int chol_pad(int n) { return n > 32 ? n : (n <= 8 ? 8 : (n == 23 || n == 29 ? n : (n + 3) & ~3)); }
 // x <- H^-1 x for a dense SPD H (packed lower triangle in shared memory); H is destroyed
 __device__ __forceinline__ void chol_dense(double* H, int n, double* x, int lane) {
   if (n > 36) { chol_factor_rows(H, n, lane); chol_solve(H, n, x, lane); return; }
@@ -361,7 +361,7 @@ __device__ __forceinline__ void chol_dense(double* H, int n, double* x, int lane
 }
 
 // H <- M (+ diag_scale * damping on the diagonal), dense packed lower triangle padded with identity rows up to chol_pad(nv)
-__device__ __forceinline__ void load_M_dense(const DevModel& m, const Warp w, double* H, double diag_scale /* h */) {
+template <class MD> __device__ __forceinline__ void load_M_dense(const MD& m, const Warp w, double* H, double diag_scale /* h */) {
   const int n = m.nv, np = chol_pad(n), nt = n*(n+1)/2; for (int i = w.lane; i < np*(np+1)/2; i += 32) H[i] = 0; __syncwarp();
   if (w.lane >= n && w.lane < np) H[TRI(w.lane, w.lane)] = 1.0;
   for (int i = 32 + w.lane; i < np; i += 32) if (i >= n) H[TRI(i, i)] = 1.0;
@@ -372,7 +372,7 @@ __device__ __forceinline__ void load_M_dense(const DevModel& m, const Warp w, do
 
 // ------------------------------------------------------------------ tree-sparse L'DL (level-scheduled, left-looking) on the qM layout
 // Hs (nM, input) -> LD (nM: D on the diagonal slots, unit-L off-diagonals), Dinv (nv)
-__device__ void ldl_factor(const DevModel& m, const Warp w, const double* Hs, double* LD, double* Dinv) {
+template <class MD> __device__ void ldl_factor(const MD& m, const Warp w, const double* Hs, double* LD, double* Dinv) {
   SHARED_PTR(Hs); SHARED_PTR(LD); SHARED_PTR(Dinv);
   const idx_t* fadr = CI(PFE_adr); const idx_t* fe = CI(PFE); const idx_t* tadr = CI(PFT_adr); const idx_t* ft = CI(PFT);
   const idx_t* mi = CI(PM_i); const idx_t* mj = CI(PM_j); const idx_t* madr = CI(dof_Madr);
@@ -386,7 +386,7 @@ __device__ void ldl_factor(const DevModel& m, const Warp w, const double* Hs, do
     __syncwarp(); }
 }
 // x <- (L'DL)^-1 x
-__device__ void ldl_solve(const DevModel& m, const Warp w, const double* LD, const double* Dinv, double* x) {
+template <class MD> __device__ void ldl_solve(const MD& m, const Warp w, const double* LD, const double* Dinv, double* x) {
   SHARED_PTR(LD); SHARED_PTR(Dinv); SHARED_PTR(x);
   const idx_t* ladr = CI(PLV_adr); const idx_t* lv = CI(PLV); const idx_t* dadr = CI(PDS_adr); const idx_t* ds = CI(PDS);
   const idx_t* madr = CI(dof_Madr); const idx_t* mj = CI(PM_j);
@@ -409,7 +409,7 @@ __device__ void ldl_solve(const DevModel& m, const Warp w, const double* LD, con
 // warps only take part in the barriers.  The total wait is unchanged: the CTA leaves the phase with its slowest env either way.
 // __forceinline__: as a real call the function receives the DevModel by address and every m.field becomes a generic load that is repeated
 // after each shared-memory store (measured round 2: 310 LD.E in the solver of the launch_bounds(448) kernel, which had not inlined it).
-__device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, double tol, long long* cyc, bool live, bool cta_sync) {
+template <class MD> __device__ __forceinline__ void phase_solve(const MD& m, const Warp w, double tol, long long* cyc, bool live, bool cta_sync) {
   long long tc = cyc ? clock64() : 0;
   #define LAP(k) if (cyc) { long long t_ = clock64(); cyc[k] += t_ - tc; tc = t_; }
   int n = m.nv, nefc = live ? WI_(nefc) : 0; const int ncon = live ? WI_(ncon) : 0, nlimrow = live ? WI_(nlimrow) : 0; int niter = 0;
@@ -509,7 +509,7 @@ __device__ __forceinline__ void phase_solve(const DevModel& m, const Warp w, dou
 // qpos <- qpos (+) h v (mj_integratePos): hinge and slide joints add; a free joint adds the position and turns its quaternion by
 // exp(h omega / 2) in the body frame, then normalises it.  Lanes over the joints; the caller syncs.  phase_integrate keeps its own
 // inline copy of this loop over qpos / qvel, for the same reason as phase_constraints' equality rows.
-__device__ __forceinline__ void integrate_pos(const DevModel& m, const Warp w, double* qpos, const double* v, double h) {
+template <class MD> __device__ __forceinline__ void integrate_pos(const MD& m, const Warp w, double* qpos, const double* v, double h) {
   const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr);
   for (int j = w.lane; j < m.njnt; j += 32) { int qa = jq[j], da = jd[j];
     if (jtype[j] == 0) { for (int c = 0; c < 3; c++) qpos[qa+c] += h*v[da+c];
@@ -525,7 +525,7 @@ __device__ __forceinline__ void integrate_pos(const DevModel& m, const Warp w, d
 // The vector part of q1^-1 q2 is formed without fused multiply-adds, so that equal quaternions give exactly 0 (a contracted
 // a0 b1 - b0 a1 leaves the rounding error of one product, which divided by eps would put ~1e-11 into columns that are exactly 0).
 // Lanes over the joints; the caller syncs.
-__device__ __forceinline__ void differentiate_pos(const DevModel& m, const Warp w, double* v, const double* q1, const double* q2) {
+template <class MD> __device__ __forceinline__ void differentiate_pos(const MD& m, const Warp w, double* v, const double* q1, const double* q2) {
   const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr);
   for (int j = w.lane; j < m.njnt; j += 32) { int qa = jq[j], da = jd[j];
     if (jtype[j] == 0) { for (int c = 0; c < 3; c++) v[da+c] = q2[qa+c] - q1[qa+c];
@@ -543,7 +543,7 @@ __device__ __forceinline__ void differentiate_pos(const DevModel& m, const Warp 
     else v[da] = q2[qa] - q1[qa]; }
 }
 
-__device__ void phase_integrate(const DevModel& m, const Warp w, long long* cyc) {
+template <class MD> __device__ void phase_integrate(const MD& m, const Warp w, long long* cyc) {
   int n = m.nv; double h = m.timestep; long long tc = cyc ? clock64() : 0;
   // (M + h B) qacc' = M qacc  (= qfrc_smooth + qfrc_constraint at the solver optimum)
   for (int i = w.lane; i < n; i += 32) S_g[i] = S_Ma[i];     // M qacc, maintained by the solver
