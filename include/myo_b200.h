@@ -347,7 +347,8 @@ int64_t myo_batch_launch_count(const myo_batch* b);
  * launch_info writes the first min(n, 9) of: use_w14 (1: the launch_bounds(448) kernel, 0: launch_bounds(320)), warps_per_cta,
  * grid, rounds of warps each CTA walks, regroup (1: load-sorted slot -> env map), balanced (1: env e on CTA e % grid when not
  * regrouped, 0: contiguous groups of warps), smem_bytes, perm_slots (entries of the slot -> env map, 0 without regroup), hand_shape
- * (1: the launch_bounds(448) kernel is the one compiled for the hand's shape, myo_env_kernel_w14_hand).
+ * (1: the env steps run myo_env_kernel_w14_hand, the launch_bounds(352) kernel compiled for the hand's shape, in place of the launch_bounds(448) one;
+ * smem_bytes then includes its cold-table region).
  * debug_perm copies the slot -> env map of the last env step to HOST memory (n >= perm_slots entries; slot
  * cta + grid*(round*warps_per_cta + warp), -1 = idle slot); it synchronises the device and fails when regroup is off or no step has run. */
 int myo_batch_launch_info(const myo_batch* b, int32_t* out, int n);

@@ -505,9 +505,9 @@ extern "C" __global__ void __launch_bounds__(320) myo_env_kernel(const __grid_co
 // the same product body under launch_bounds(448): 128 registers for the entry function, up to 14 env-warps per CTA.  Chosen when the model's
 // shared-memory footprint lets that many warps cut the number of rounds (hand, 4096 envs: 2 rounds of 14 instead of 3 of 10).
 extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
-// the same launch_bounds(448) product body on the hand's compile-time shape (HandShape): chosen instead of myo_env_kernel_w14 for a batch
-// whose DevModel matches that shape (batch_setup)
-extern "C" __global__ void __launch_bounds__(448) myo_env_kernel_w14_hand(const __grid_constant__ HandShape m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 448>(m, a); }
+// the same product body on the hand's compile-time shape (HandShape), sized for its H100 launch of 11 warps per CTA: 168 registers under launch_bounds(352, 1), and
+// the cold tables in shared memory.  Chosen instead of myo_env_kernel_w14 for a batch of that shape whose launch fits its thread limit and shared memory (batch_setup)
+extern "C" __global__ void __launch_bounds__(352, 1) myo_env_kernel_w14_hand(const __grid_constant__ HandShape m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 352>(m, a); }
 // parity taps / forward-debug / profiling counters / tuning knobs
 extern "C" __global__ void __launch_bounds__(320) myo_env_kernel_dbg(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<true, 320>(m, a); }
 // rollout (myo_batch_rollout): the product body's mode 0 with the caller's ctrl and applied forces, under the two product launch bounds
@@ -877,7 +877,7 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
 
 struct LaunchShape { int warps, smem, grid; };      // env-warps per CTA, dynamic shared memory (bytes), CTAs
 // Zero-initialised by myo_batch_create (new myo_batch()), so that myo_batch_destroy can free a partly built batch.
-struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes;
+struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes, cold_bytes;
   LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14, use_hand; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
   int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
@@ -984,18 +984,25 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
   if (b->dm.neq + b->dm.nlimrow + b->dm.maxcon > 255) return fail("equality + limit rows + contact capacity exceed the 255 regulariser slots of the row map");
   // Launch configurations.  Product: the launch_bounds(320) kernel (168 registers, <= 10 warps) unless more warps fit in shared memory AND cut the
   // number of rounds, then the launch_bounds(448) kernel (128 registers, <= 14 warps).  Debug kernel: its own configuration (<= 10 warps).
-  cudaFuncAttributes fa_p, fa_w, fa_d; CUDA_OK(cudaFuncGetAttributes(&fa_p, myo_env_kernel)); CUDA_OK(cudaFuncGetAttributes(&fa_w, myo_env_kernel_w14)); CUDA_OK(cudaFuncGetAttributes(&fa_d, myo_env_kernel_dbg));
+  cudaFuncAttributes fa_p, fa_w, fa_h, fa_d; CUDA_OK(cudaFuncGetAttributes(&fa_p, myo_env_kernel)); CUDA_OK(cudaFuncGetAttributes(&fa_w, myo_env_kernel_w14));
+  CUDA_OK(cudaFuncGetAttributes(&fa_h, myo_env_kernel_w14_hand)); CUDA_OK(cudaFuncGetAttributes(&fa_d, myo_env_kernel_dbg));
   const bool big = (size_t)per*(fit < 4 ? fit : 4) + b->const_bytes > 50*1024;      // a 4-warp CTA already takes > 50 KB: one CTA per SM, sized by the round count (small models run several CTAs per SM instead)
   auto rounds_of = [&](const LaunchShape& s) { const int sms = prop.multiProcessorCount; return (n_env + sms*s.warps - 1)/(sms*s.warps); }; LaunchShape sp, sw;
   if (launch_shape((const void*)myo_env_kernel, prop, per, b->const_bytes, n_env, big, 0, sp) || launch_shape((const void*)myo_env_kernel_w14, prop, per, b->const_bytes, n_env, big, 0, sw)) return -1;
   b->use_w14 = sw.warps > sp.warps && rounds_of(sw) < rounds_of(sp);      // (small models too: the elbow runs 4096 envs in 2 rounds of 14 warps instead of 3 of 10 -- registers, not shared memory, keep it at one CTA per SM)
   if (const char* e = getenv("MYO_B200_W14")) b->use_w14 = atoi(e) != 0 && fa_w.maxThreadsPerBlock > fa_p.maxThreadsPerBlock;      // tuning override
-  b->use_hand = b->use_w14 && HandShape::matches(b->dm);      // the w14 launch, compiled for this batch's shape
-  const void* prod_fn = b->use_hand ? (const void*)myo_env_kernel_w14_hand : b->use_w14 ? (const void*)myo_env_kernel_w14 : (const void*)myo_env_kernel;
+  const void* prod_fn = b->use_w14 ? (const void*)myo_env_kernel_w14 : (const void*)myo_env_kernel;
   const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;      // tuning override (never above what fits)
   if (launch_shape(prod_fn, prop, per, b->const_bytes, n_env, big, want, b->prod) ||
       launch_shape((const void*)myo_env_kernel_dbg, prop, per, b->const_bytes, n_env, big, want, b->dbg)) return -1;
   b->balanced = b->prod.smem > 100*1024; b->dbg_balanced = b->dbg.smem > 100*1024;      // the balanced slot map for CTAs that fill an SM
+  // The w14 launch on the kernel compiled for this batch's shape, where that launch fits it: the same warps per CTA within its thread
+  // limit and, with its cold-table region, within the device's shared memory.  It then runs the same grid and slot map.
+  if (b->use_w14 && HandShape::matches(b->dm)) {
+    const int cold = HandShape::cold_bytes(b->dm, MYO_SEC_LEN(m->I.data(), MYO_SEC_HOT_D)); LaunchShape sh;
+    if (b->prod.warps <= fa_h.maxThreadsPerBlock/32 && b->prod.warps <= warps_that_fit(prop, per, b->const_bytes + cold)) {
+      if (launch_shape((const void*)myo_env_kernel_w14_hand, prop, per, b->const_bytes + cold, n_env, big, b->prod.warps, sh)) return -1;
+      if (sh.warps == b->prod.warps && sh.grid == b->prod.grid) { b->use_hand = true; b->cold_bytes = cold; b->prod = sh; } } }
   // load-sorted env -> round map (one-CTA-per-SM models only; MYO_B200_REGROUP=0 switches it off)
   b->big = big; b->regroup = big; if (const char* e = getenv("MYO_B200_REGROUP")) b->regroup = big && atoi(e) != 0;
   if (b->regroup) { b->perm_rounds = (SLOTS_PER_CTA(1, n_env, b->prod.grid, b->prod.warps) + b->prod.warps - 1)/b->prod.warps; b->perm_slots = b->prod.grid*b->prod.warps*b->perm_rounds; }
@@ -1010,8 +1017,8 @@ static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg
   // the uploads and memsets above run on the legacy stream (a pageable upload may return before its DMA lands): complete them here, so
   // that a caller whose first launch goes to a non-blocking stream finds the model and the zeroed rows in place
   CUDA_OK(cudaStreamSynchronize(cudaStreamLegacy));
-  if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, debug %d / %d\n",
-    n_env, b->use_hand ? "myo_env_kernel_w14_hand" : b->use_w14 ? "myo_env_kernel_w14" : "myo_env_kernel", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
+  if (getenv("MYO_B200_VERBOSE")) fprintf(stderr, "[myo_b200] n_env %d: %s kernel, %d warps/CTA, grid %d, smem %d B (const %d + cold tables %d + %d/env, %d fit); debug kernel %d warps, grid %d; max threads / regs: product %d / %d, w14 %d / %d, w14_hand %d / %d, debug %d / %d\n",
+    n_env, b->use_hand ? "myo_env_kernel_w14_hand" : b->use_w14 ? "myo_env_kernel_w14" : "myo_env_kernel", b->prod.warps, b->prod.grid, b->prod.smem, b->const_bytes, b->cold_bytes, per, fit, b->dbg.warps, b->dbg.grid, fa_p.maxThreadsPerBlock, fa_p.numRegs, fa_w.maxThreadsPerBlock, fa_w.numRegs, fa_h.maxThreadsPerBlock, fa_h.numRegs, fa_d.maxThreadsPerBlock, fa_d.numRegs);
   return 0;
 }
 
@@ -1105,7 +1112,8 @@ static int launch(myo_batch* b, StepArgs& a, void* stream) {
     if (a.mode == 0 && b->regroup) {      // env steps: regroup by last step's load first (same stream), then step through the permutation
       myo_regroup_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots);
       a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; b->perm_built = true; b->launches++; }
-    if (b->use_hand) { HandShape hm; static_cast<DevModel&>(hm) = b->dm; myo_env_kernel_w14_hand<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(hm, a); }
+    if (b->use_hand) { HandShape hm; static_cast<DevModel&>(hm) = b->dm; hm.nD += b->cold_bytes/8;      // the cold tables staged too
+      myo_env_kernel_w14_hand<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(hm, a); }
     else if (b->use_w14) myo_env_kernel_w14<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
     else myo_env_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a); }
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
@@ -1202,7 +1210,7 @@ static int roll_setup(myo_batch* b) {
   cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
   const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;
   if (launch_shape(b->use_w14 ? (const void*)myo_roll_kernel_w14 : (const void*)myo_roll_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, b->big, want, b->roll_shape)) return -1;
-  const bool same = b->roll_shape.warps == b->prod.warps && b->roll_shape.grid == b->prod.grid && b->roll_shape.smem == b->prod.smem;
+  const bool same = b->roll_shape.warps == b->prod.warps && b->roll_shape.grid == b->prod.grid && b->roll_shape.smem == b->prod.smem - b->cold_bytes;      // (less the hand kernel's cold tables)
   b->roll_regroup = same && b->regroup; b->roll_balanced = same ? b->balanced : 1;
   const DevModel& d = b->dm;
   CUDA_OK(cudaMalloc(&b->dCarry, (size_t)b->n_env*(d.nq + 2*d.nv + d.na + 1)*8));

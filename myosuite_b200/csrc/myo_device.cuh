@@ -54,20 +54,20 @@ struct DevModel {
   int32_t s_conJ, s_efD, s_efA, s_eqJ, s_icon, s_con;      // stage 3 -> 4: contacts / constraint rows
   int32_t s_clist, kcand;                                  // collision only: list of the expensive (ellipsoid) candidates that survived the cull
   int32_t s_efR, s_efV, s_va, s_vg, s_vp, s_vMa, s_vMp, s_H, s_Hs, s_LD, s_Dinv;   // stage 4: Newton
+  static constexpr bool cold_in_smem = false;              // the cold f64 tables stay in HBM (GD(); HandShape stages them, myo_layout.cuh)
 };
 
-// The whole dynamic shared-memory window, declared at file scope so that every pointer derived from it is PROVABLY in the
-// shared address space: the working-set and constant accesses compile to LDS/STS with 32-bit address arithmetic instead of
-// generic 64-bit loads (round 1: 4 048 generic LD.E vs 127 LDS in the kernel's SASS).
-// Layout: [hot f64 tables (m.nD)] [hot int16 lists] [per-warp regions of m.n_per_warp doubles]
+// The whole dynamic shared-memory window, declared at file scope so that every pointer derived from it is PROVABLY in the shared address space: the working-set
+// and constant accesses compile to LDS/STS with 32-bit address arithmetic instead of generic 64-bit loads (round 1: 4 048 generic LD.E vs 127 LDS in the kernel's SASS).
+// Layout: [hot f64 tables (m.nD)] [hot int16 lists] [per-warp regions of m.n_per_warp doubles]; the hand kernel's m.nD also covers the cold f64 tables (HandShape)
 extern __shared__ __align__(16) double smem[];
 
 struct Warp { int base, lane; };   // by value: offset (doubles) of this warp's region in smem, lane id.  Everything else lives in shared memory.
 enum { CNT_ncon, CNT_nefc, CNT_nlimrow, CNT_niter, CNT_overflow, CNT_ncand, CNT_na, CNT_N = 8 };   // per-warp int counters (m.o_cnt)
 #define CI(name) ((const idx_t*)(smem + m.nD) + m.hoff[MYO_SEC_##name])
 #define CD(name) ((const double*)smem + m.hoff[MYO_SEC_##name])
-#define LDC(p) __ldg(p)
-#define GD(name) (m.gD + m.hoff[MYO_SEC_##name])              // cold f64 tables (blob.py COLD_D): read from HBM / L2 through the read-only path (__ldg)
+#define LDC(p) (m.cold_in_smem ? *(p) : __ldg(p))      // (a constant condition in a macro, not a helper function: one more inline layer reorders the inlining of the kernels' callees, and with it their machine code)
+#define GD(name) (m.cold_in_smem ? (const double*)smem + m.hoff[MYO_SEC_##name] : m.gD + m.hoff[MYO_SEC_##name])   // cold f64 tables (blob.py COLD_D): read from HBM / L2 through the read-only path (__ldg), or from shared memory where the launch stages them behind the hot tables (HandShape)
 #define W_(f) (smem + w.base + m.o_##f)                       // persistent per-env arrays
 #define WI_(f) (((int*)(smem + w.base + m.o_cnt))[CNT_##f])   // per-env counters
 #define SCR(field) (smem + w.base + m.field)                  // scratch (m.s_* are offsets from the warp base)

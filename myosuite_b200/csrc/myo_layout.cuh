@@ -138,4 +138,12 @@ template <class Dims> struct StaticShape : DevModel {
 #include "../../include/myo_hand_shape.h"
 struct HandDims { static constexpr ModelDims value = MYO_HAND_SHAPE_DIMS; };
 static_assert(sizeof(ModelDims) == MYO_HAND_SHAPE_NDIMS*sizeof(int32_t), "include/myo_hand_shape.h lists every ModelDims field");
-typedef StaticShape<HandDims> HandShape;
+// The hand kernel's launch adds one region to the generic launch: the cold f64 tables (blob.py COLD_D), which sit behind the staged
+// doubles in the blob.  It passes nD = every hot double, so that the same bulk copy stages them and they land right behind the staged
+// tables ([hot f64 | cold f64 | int16 lists | per-warp regions]); GD() / LDC() then read shared memory instead of HBM.  The model layout,
+// the DevModel of the batch and every other kernel's launch are those of the generic kernel.
+struct HandShape : StaticShape<HandDims> {
+  static constexpr bool cold_in_smem = true;
+  // bytes of the region for a batch whose blob holds nD_all hot doubles, of which its DevModel d stages d.nD
+  static int cold_bytes(const DevModel& d, int nD_all) { return (nD_all - d.nD)*8; }
+};
