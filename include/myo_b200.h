@@ -249,6 +249,40 @@ typedef struct {
 } myo_fd_buffers;
 typedef struct { double eps; int32_t centered, substeps; } myo_fd_params;
 
+/* Caller-owned device buffers of myo_batch_static_opt: muscle static optimisation with reserve actuators at each env's current (qpos, qvel,
+ * act).  With tau = qfrc_inverse(qacc) (myo_batch_inverse with the same flags), AM [nu, nv] the actuator moments (gear x the tendon
+ * moment), and g <= 0, b the muscle gain and bias at the current actuator length and velocity (actuator_force = g act + b), let
+ * t = tau - AM' b and G = AM' diag(g) [nv, nu].  The solution of the strictly convex problem
+ *   min_{a, r}  1/2 sum_m w_m a_m^2 + 1/2 sum_i (r_i / rho_i)^2   s.t.   G a + r = t,   0 <= a_m <= 1
+ * (w: weight, rho: reserve; r is the reserve generalized force, exactly t on dofs no muscle crosses) comes from semismooth Newton on the
+ * dual in nv space: a(l) = clip((G' l)_m / w_m, 0, 1), r(l) = rho^2 l, F(l) = G a(l) + rho^2 l - t; the step solves
+ * (G_F W_F^-1 G_F' + diag rho^2) d = -F over the muscles F strictly inside the box and those at the kink (G'l)_m = 0 (the generalized
+ * Jacobian's choice there; at l = 0 it is every muscle, which keeps the first step from overshooting), with Armijo backtracking (halving, slope 1e-4) on the
+ * concave dual psi(l) = l't - 1/2 sum rho_i^2 l_i^2 - sum_m max_{a in [0, 1]} (a (G'l)_m - 1/2 w_m a^2).  From l = lambda0 (or 0) it stops
+ * with converged = 1 at the first iterate where |F|_inf <= tol max(1, |t|_inf), else with converged = 0 after max_iter steps; every
+ * output describes the returned l.  ctrl is the excitation that takes the current act to a in one mj_step of the muscle activation
+ * dynamics (act' = act + h (clip(ctrl, 0, 1) - act) / tau(ctrl, act)): closed form with tausmooth = 0, bisection over the range to machine
+ * precision otherwise; it is clipped to ctrlrange intersected with [0, 1] ([0, 1] without ctrllimited), where act moves toward a but does
+ * not reach it.  Only the non-null outputs are written. */
+typedef struct {
+  const double* qacc;          /* [n, nv] in, required */
+  const double* weight;        /* [nu] nullable (1): w > 0 */
+  const double* reserve;       /* [nv] in, required: rho > 0 */
+  const double* lambda0;       /* [n, nv] nullable (0): warm start of the dual */
+  double* act;                 /* [n, nu] out, required: the optimal activations a */
+  double* reserve_force;       /* [n, nv] nullable: r = rho^2 lambda */
+  double* ctrl;                /* [n, nu] nullable: excitation reaching a in one mj_step */
+  double* actuator_force;      /* [n, nu] nullable: g a + b */
+  double* muscle_gain;         /* [n, nu] nullable: g */
+  double* muscle_bias;         /* [n, nu] nullable: b */
+  double* qfrc_inverse;        /* [n, nv] nullable: tau */
+  double* lambda;              /* [n, nv] nullable: the dual solution */
+  int32_t* niter;              /* [n] nullable: Newton steps taken */
+  int32_t* converged;          /* [n] nullable */
+  double* residual;            /* [n] nullable: |F|_inf at the returned lambda */
+} myo_static_opt_buffers;
+typedef struct { int32_t max_iter; double tol; } myo_static_opt_params;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -339,6 +373,14 @@ int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_params* p, 
  * unbound batch, eps not finite or not > 0, substeps < 1 or centered not in {0, 1}.  Replaces mujoco.mjd_transitionFD (iLQR / DDP, LQR
  * about a reference pose, MPC warm starts, controllability and sensitivity studies). */
 int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, const myo_fd_params* p, void* stream);
+
+/* Muscle static optimisation of every env (myo_static_opt_buffers, myo_static_opt_params), one launch on `stream`; flags: MYO_INV_* as
+ * myo_batch_inverse's; each env iterates until its own stop test.  No bound buffer is written.  Fails before any launch on a null batch,
+ * buffers, params, qacc, reserve or act, an unbound batch, unknown flag bits, tol < 0, max_iter < 0, a non-finite tol, a model with more
+ * than 64 dofs, or a per-env slice without room for the iteration's arrays (the legs at maxcon 4); the device does not check the values of
+ * weight and reserve.  Replaces the per-frame SLSQP / OSQP solves of MyoSuite
+ * tutorials 6_Inverse_Dynamics (get_ctrl) and 9_Computed_muscle_control. */
+int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* d, const myo_static_opt_params* p, int flags, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

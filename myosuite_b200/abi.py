@@ -111,11 +111,27 @@ class MyoFdParams(ctypes.Structure):
     _fields_ = [("eps", c_f64), ("centered", c_i32), ("substeps", c_i32)]
 
 
+# myo_static_opt_buffers / myo_static_opt_params (include/myo_b200.h): muscle static optimisation of myo_batch_static_opt.  Inputs, then
+# the outputs -> trailing shape after [n] in the model's sizes
+STATIC_OPT_FIELDS = ["qacc", "weight", "reserve", "lambda0", "act", "reserve_force", "ctrl", "actuator_force", "muscle_gain", "muscle_bias",
+                     "qfrc_inverse", "lambda", "niter", "converged", "residual"]
+STATIC_OPT_SHAPES = {"act": ("nu",), "reserve_force": ("nv",), "ctrl": ("nu",), "actuator_force": ("nu",), "muscle_gain": ("nu",),
+                     "muscle_bias": ("nu",), "qfrc_inverse": ("nv",), "lambda": ("nv",), "niter": (), "converged": (), "residual": ()}
+
+
+class MyoStaticOptBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in STATIC_OPT_FIELDS]
+
+
+class MyoStaticOptParams(ctypes.Structure):
+    _fields_ = [("max_iter", c_i32), ("tol", c_f64)]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
            "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout",
-           "myo_batch_ik", "myo_batch_transition_fd"]
+           "myo_batch_ik", "myo_batch_transition_fd", "myo_batch_static_opt"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -177,6 +193,7 @@ def _bind(L):
     L.myo_batch_rollout.argtypes = [c_vp, ctypes.POINTER(MyoRolloutBuffers), ctypes.c_int, ctypes.c_int, c_vp]
     L.myo_batch_ik.argtypes = [c_vp, ctypes.POINTER(MyoIkBuffers), ctypes.POINTER(MyoIkParams), c_vp]
     L.myo_batch_transition_fd.argtypes = [c_vp, ctypes.POINTER(MyoFdBuffers), ctypes.POINTER(MyoFdParams), c_vp]
+    L.myo_batch_static_opt.argtypes = [c_vp, ctypes.POINTER(MyoStaticOptBuffers), ctypes.POINTER(MyoStaticOptParams), ctypes.c_int, c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -342,6 +359,20 @@ class Batch:
                 raise ValueError("%s must be contiguous" % k)
             setattr(d, k, t.data_ptr())
         _check(self.L.myo_batch_transition_fd(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
+
+    def static_opt(self, params, stream=None, flags=0, **tensors):
+        """Muscle static optimisation (myo_batch_static_opt) with the given torch CUDA tensors (names of STATIC_OPT_FIELDS: qacc, reserve
+        and act are required), a MyoStaticOptParams and MYO_INV_* flags."""
+        d = MyoStaticOptBuffers()
+        for k, t in tensors.items():
+            if k not in STATIC_OPT_FIELDS:
+                raise KeyError(k)
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % k)
+            setattr(d, k, t.data_ptr())
+        _check(self.L.myo_batch_static_opt(self.handle, ctypes.byref(d), ctypes.byref(params), flags, stream), self.L)
 
     @property
     def launches(self):

@@ -664,6 +664,42 @@ extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_c
 //   vg / vp      vg holds B qacc, then M^-1 B qacc, then qfrc_constraint; vp is not used
 //   efR, efV     jar (read again by the contact-force decoding); efV: aref, then the row forces -D jar (folded by rows_applyT_add)
 struct InvArgs { myo_inverse_buffers d; myo_buffers b; int n_env, flags; };
+// One env's inverse up to its outputs (myo_inverse_kernel, myo_static_opt_kernel): leaves M qacc in S_Ma, qfrc_passive - qfrc_bias in fsm
+// and qfrc_constraint in S_g, so that qfrc_inverse = S_Ma - fsm - S_g; qacc and actuator_moment (nullable) are the whole batch's rows
+__device__ __forceinline__ void inverse_pass(const DevModel& m, const Warp w, const myo_buffers& b, int env, const double* qacc, double* actuator_moment, bool constraints, bool discrete) {
+  if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
+  load_env_state(m, w, b, env);
+  phase_kinematics(m, w);
+  if (actuator_moment) { phase_tendon_all(m, w);      // dense [nu, nv]: gear x the tendon moment
+    const idx_t* at = CI(PA_tendon); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof); const double* __restrict__ PAm = GD(PAM_d); const double* mom = SCR(s_mom);
+    for (int i = w.lane; i < m.nu; i += 32) { double* row = actuator_moment + ((size_t)env*m.nu + i)*m.nv; const double gear = LDC(PAm + i*PAM_STRIDE + 4); const int t = at[i];
+      for (int k = 0; k < m.nv; k++) row[k] = 0;
+      for (int z = nadr[t]; z < nadr[t+1]; z++) row[nzd[z]] += gear*mom[z]; }
+    __syncwarp(); }
+  { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; }
+  __syncwarp();
+  phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w);       // fsm = qfrc_passive - qfrc_bias
+  if (constraints) { phase_collision(m, w); phase_constraints(m, w); }
+  const int nefc = WI_(nefc);
+  for (int r = w.lane; r < nefc; r += 32) S_jv[r] = S_aref[r];
+  for (int i = w.lane; i < m.nv; i += 32) S_a[i] = qacc[(size_t)env*m.nv + i];
+  __syncwarp();
+  if (discrete) {      // (M + h B) qacc = M qacc_c: qacc_c = qacc + h M^-1 B qacc, with the integrator's choice of solver
+    const double* dofp = CD(PDOF_d);      // (the program drops the tree-sparse lists where that choice is dense and no Newton step is sparse)
+    for (int i = w.lane; i < m.nv; i += 32) S_g[i] = dofp[2*i+1]*S_a[i];
+    if (m.nv >= 8 && m.nv <= 36) { load_M_dense(m, w, S_H, 0.0); chol_dense(S_H, m.nv, S_g, w.lane); }
+    else { ldl_factor(m, w, W_(qM), S_LD, S_Dinv); ldl_solve(m, w, S_LD, S_Dinv, S_g); }
+    for (int i = w.lane; i < m.nv; i += 32) S_a[i] += m.timestep*S_g[i];
+    __syncwarp(); }
+  mul_M(m, w, S_Ma, S_a);
+  for (int i = w.lane; i < m.nv; i += 32) S_g[i] = 0;
+  __syncwarp();
+  if (constraints) {      // (the row operators walk the equality rows whether or not the constraint phase ran)
+    rows_apply(m, w, S_a, S_jar); __syncwarp();
+    for (int r = w.lane; r < nefc; r += 32) { const double x = S_jar[r] - S_jv[r]; S_jar[r] = x; S_jv[r] = (r < m.neq || x < 0) ? -S_D[S_drow[r]]*x : 0.0; }
+    __syncwarp();
+    rows_applyT_add(m, w, S_jv, S_g); }      // qfrc_constraint
+}
 
 extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __grid_constant__ DevModel m, const __grid_constant__ InvArgs a) {
   __shared__ __align__(8) unsigned long long mbar;
@@ -675,38 +711,7 @@ extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __gri
   for (int j = wid; j < per_cta; j += nw) {
     const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
     if (env >= a.n_env) break;
-    if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
-    load_env_state(m, w, a.b, env);
-    phase_kinematics(m, w);
-    if (d.actuator_moment) { phase_tendon_all(m, w);      // dense [nu, nv]: gear x the tendon moment
-      const idx_t* at = CI(PA_tendon); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof); const double* __restrict__ PAm = GD(PAM_d); const double* mom = SCR(s_mom);
-      for (int i = w.lane; i < m.nu; i += 32) { double* row = d.actuator_moment + ((size_t)env*m.nu + i)*m.nv; const double gear = LDC(PAm + i*PAM_STRIDE + 4); const int t = at[i];
-        for (int k = 0; k < m.nv; k++) row[k] = 0;
-        for (int z = nadr[t]; z < nadr[t+1]; z++) row[nzd[z]] += gear*mom[z]; }
-      __syncwarp(); }
-    { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; }
-    __syncwarp();
-    phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w);       // fsm = qfrc_passive - qfrc_bias
-    if (constraints) { phase_collision(m, w); phase_constraints(m, w); }
-    const int nefc = WI_(nefc);
-    for (int r = w.lane; r < nefc; r += 32) S_jv[r] = S_aref[r];
-    for (int i = w.lane; i < m.nv; i += 32) S_a[i] = d.qacc[(size_t)env*m.nv + i];
-    __syncwarp();
-    if (discrete) {      // (M + h B) qacc = M qacc_c: qacc_c = qacc + h M^-1 B qacc, with the integrator's choice of solver
-      const double* dofp = CD(PDOF_d);      // (the program drops the tree-sparse lists where that choice is dense and no Newton step is sparse)
-      for (int i = w.lane; i < m.nv; i += 32) S_g[i] = dofp[2*i+1]*S_a[i];
-      if (m.nv >= 8 && m.nv <= 36) { load_M_dense(m, w, S_H, 0.0); chol_dense(S_H, m.nv, S_g, w.lane); }
-      else { ldl_factor(m, w, W_(qM), S_LD, S_Dinv); ldl_solve(m, w, S_LD, S_Dinv, S_g); }
-      for (int i = w.lane; i < m.nv; i += 32) S_a[i] += m.timestep*S_g[i];
-      __syncwarp(); }
-    mul_M(m, w, S_Ma, S_a);
-    for (int i = w.lane; i < m.nv; i += 32) S_g[i] = 0;
-    __syncwarp();
-    if (constraints) {      // (the row operators walk the equality rows whether or not the constraint phase ran)
-      rows_apply(m, w, S_a, S_jar); __syncwarp();
-      for (int r = w.lane; r < nefc; r += 32) { const double x = S_jar[r] - S_jv[r]; S_jar[r] = x; S_jv[r] = (r < m.neq || x < 0) ? -S_D[S_drow[r]]*x : 0.0; }
-      __syncwarp();
-      rows_applyT_add(m, w, S_jv, S_g); }      // qfrc_constraint
+    inverse_pass(m, w, a.b, env, d.qacc, d.actuator_moment, constraints, discrete);
     for (int i = w.lane; i < m.nv; i += 32) { const size_t o = (size_t)env*m.nv + i;
       d.qfrc_inverse[o] = S_Ma[i] - W_(fsm)[i] - S_g[i];
       if (d.qfrc_constraint) d.qfrc_constraint[o] = S_g[i]; }
@@ -852,6 +857,145 @@ extern "C" __global__ void __launch_bounds__(320) myo_ik_kernel(const __grid_con
   }
 }
 
+// ------------------------------------------------------------------ muscle static optimisation (myo_batch_static_opt)
+// The dual Newton of include/myo_b200.h (myo_static_opt_buffers), one env per warp on the balanced map; each warp leaves on its own stop test
+// and nothing is stored back.  The inverse pass gives t; a second kinematics and tendon pass gives the moments, lengths and velocities (the
+// inverse's CRB stage overwrites them).  G is never formed: (G' l)_m = gear g (mom . l) over the muscle's moment non-zeros, and (G a)_i sums
+// mom x (gear g a) of its tendon over dof i's column list, as phase_actuation sums the tendon forces.  Lane i owns rows i and i + 32 of the
+// packed H (the dense solver's padded order, identity padding) and adds each free muscle's outer product from its non-zeros: no atomics,
+// one summation order whatever the batch.  Scratch lifetimes:
+//   everything      the inverse pass (its own lifetimes, above), then the kinematics and tendon passes, as in a forward pass
+//   fsm             qfrc_passive - qfrc_bias, then t from the end of the inverse pass to the last iteration
+//   T (mom)         from the tendon pass to the end: read by every product with G; T (tlen, tvel): read by the gain and bias only
+//   gm, bm          gain and bias per muscle, from the gain pass to the outputs; placed outside mom, tlen and tvel
+//   H, x, l, cg, tf, s   written after the gain pass, so they may overlap tlen, tvel, the rest of the scratch and the dead persistent
+//                   dof axes and mass matrix (dax, dan, qM); cg: gear g per tendon, tf: gear b, then gear g a per tendon; s: (G' l)_m
+//   F               in registers (lane i: F_i and F_{i+32})
+// The host places the arrays (so_plan), first fit by decreasing size, and refuses a model whose slice has no room.
+struct SoArgs { myo_static_opt_buffers d; myo_static_opt_params p; myo_buffers b; int n_env, flags;
+  int o_H, o_x, o_l, o_cg, o_tf, o_s, o_gm, o_bm; };      // offsets from the warp base (doubles)
+
+// phi(s + ds) - phi(s) of a muscle's conjugate term phi(s) = max_{a in [0, 1]} (a s - w a^2 / 2), without cancellation inside one piece
+__device__ __forceinline__ double so_phi_diff(double s, double ds, double wm) {
+  const double s1 = s + ds; const int k0 = s <= 0 ? 0 : (s < wm ? 1 : 2), k1 = s1 <= 0 ? 0 : (s1 < wm ? 1 : 2);
+  if (k0 == k1) return k0 == 0 ? 0.0 : (k0 == 1 ? ds*(s + 0.5*ds)/wm : ds);
+  const double p0 = k0 == 0 ? 0.0 : (k0 == 1 ? 0.5*s*s/wm : s - 0.5*wm), p1 = k1 == 0 ? 0.0 : (k1 == 1 ? 0.5*s1*s1/wm : s1 - 0.5*wm);
+  return p1 - p0;
+}
+
+// act after one mj_step of the activation dynamics with ctrl c (phase_actuation's update; c already inside ctrlrange)
+__device__ __forceinline__ double so_act_next(const double* dyn, double c, double act, double h) {
+  const double dctrl = clipd(c, 0, 1) - act; return act + h*(dctrl*m_rcp(fmax(MYO_MINVAL, muscle_tau(dyn, dctrl, act)))); }
+
+// the excitation that takes act to a in one step, inside [lo, hi]
+__device__ __forceinline__ double so_excitation(const double* dyn, double act, double a, double h, double lo, double hi) {
+  if (dyn[2] < MYO_MINVAL) { const double dd = a - act; return clipd(act + dd*muscle_tau(dyn, dd, act)/h, lo, hi); }
+  if (so_act_next(dyn, hi, act, h) <= a) return hi;
+  if (so_act_next(dyn, lo, act, h) >= a) return lo;
+  for (int k = 0; k < 200; k++) { const double mid = 0.5*(lo + hi); if (!(mid > lo && mid < hi)) break;
+    if (so_act_next(dyn, mid, act, h) < a) lo = mid; else hi = mid; }
+  return fabs(so_act_next(dyn, lo, act, h) - a) <= fabs(so_act_next(dyn, hi, act, h) - a) ? lo : hi;
+}
+
+extern "C" __global__ void __launch_bounds__(320) myo_static_opt_kernel(const __grid_constant__ DevModel m, const __grid_constant__ SoArgs a) {
+  __shared__ __align__(8) unsigned long long mbar;
+  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  STAGE_MODEL(m, mbar)
+  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  const myo_static_opt_buffers& d = a.d; const bool constraints = !(a.flags & MYO_INV_NOCONSTRAINT), discrete = a.flags & MYO_INV_DISCRETE;
+  const int nv = m.nv, nu = m.nu, np = m.nvp, lane = w.lane;
+  double* t = W_(fsm); double* H = smem + w.base + a.o_H; double* x = smem + w.base + a.o_x; double* lam = smem + w.base + a.o_l;
+  double* cg = smem + w.base + a.o_cg; double* tf = smem + w.base + a.o_tf; double* sm = smem + w.base + a.o_s;
+  double* gm = smem + w.base + a.o_gm; double* bm = smem + w.base + a.o_bm; const double* mom = SCR(s_mom);
+  const idx_t* at = CI(PA_tendon); const idx_t* acls = CI(PA_cls); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof);
+  const idx_t* cadr = CI(PCOL_adr); const idx_t* col = CI(PCOL); const idx_t* nzt = CI(PNZ_tendon);
+  const double* __restrict__ PAc = GD(PA_d); const double* __restrict__ PAm = GD(PAM_d);
+  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
+  for (int j = wid; j < per_cta; j += nw) {
+    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
+    if (env >= a.n_env) break;
+    inverse_pass(m, w, a.b, env, d.qacc, nullptr, constraints, discrete);
+    for (int i = lane; i < nv; i += 32) { const double v = S_Ma[i] - W_(fsm)[i] - S_g[i]; t[i] = v; if (d.qfrc_inverse) d.qfrc_inverse[(size_t)env*nv + i] = v; }
+    __syncwarp();
+    phase_kinematics(m, w); phase_tendon_all(m, w);
+    // gain and bias of every muscle (phase_actuation's), then gear g and gear b per tendon (0 on tendons without a muscle)
+    for (int i = lane; i < nu; i += 32) { double ag[16], am[5]; for (int c = 0; c < 16; c++) ag[c] = LDC(PAc + acls[i]*PA_STRIDE + c); for (int c = 0; c < 5; c++) am[c] = LDC(PAm + i*PAM_STRIDE + c);
+      const int tt = at[i]; double g, b; muscle_gain_bias(ag + 3, ag + 9, am, am[4]*SCR(s_tlen)[tt], am[4]*SCR(s_tvel)[tt], g, b); gm[i] = g; bm[i] = b;
+      if (d.muscle_gain) d.muscle_gain[(size_t)env*nu + i] = g;
+      if (d.muscle_bias) d.muscle_bias[(size_t)env*nu + i] = b; }
+    __syncwarp();
+    for (int k = lane; k < m.nta; k += 32) { cg[k] = 0; tf[k] = 0; }
+    __syncwarp();
+    for (int i = lane; i < nu; i += 32) { const double gear = LDC(PAm + i*PAM_STRIDE + 4); cg[at[i]] = gear*gm[i]; tf[at[i]] = gear*bm[i]; }
+    __syncwarp();
+    double tmax = 0;      // t = tau - AM' b
+    for (int i = lane; i < nv; i += 32) { double s = 0; for (int e = cadr[i]; e < cadr[i+1]; e++) { const int z = col[e]; s += mom[z]*tf[nzt[z]]; }
+      t[i] -= s; tmax = fmax(tmax, fabs(t[i])); lam[i] = d.lambda0 ? d.lambda0[(size_t)env*nv + i] : 0.0; }
+    for (int o = 16; o > 0; o >>= 1) tmax = fmax(tmax, __shfl_xor_sync(FULL, tmax, o));
+    const double thr = a.p.tol*fmax(1.0, tmax);
+    __syncwarp();
+    int it = 0; bool conv = false; double fnorm = 0, F[2] = {0, 0};
+    for (;; it++) {
+      // muscle duals s = G' l, the activations a(l) and gear g a per tendon
+      for (int i = lane; i < nu; i += 32) { const int tt = at[i]; double acc = 0; for (int z = nadr[tt]; z < nadr[tt+1]; z++) acc += mom[z]*lam[nzd[z]];
+        const double s = cg[tt]*acc, wm = d.weight ? d.weight[i] : 1.0; sm[i] = s; tf[tt] = cg[tt]*clipd(s/wm, 0, 1); }
+      __syncwarp();
+      fnorm = 0;      // F = G a + rho^2 l - t
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; F[c] = 0; if (i >= nv) continue;
+        double s = 0; for (int e = cadr[i]; e < cadr[i+1]; e++) { const int z = col[e]; s += mom[z]*tf[nzt[z]]; }
+        const double rho = d.reserve[i]; F[c] = s + rho*rho*lam[i] - t[i]; fnorm = fmax(fnorm, fabs(F[c])); }
+      for (int o = 16; o > 0; o >>= 1) fnorm = fmax(fnorm, __shfl_xor_sync(FULL, fnorm, o));
+      conv = fnorm <= thr;
+      if (conv || it >= a.p.max_iter) break;
+      // H = G_F W_F^-1 G_F' + diag rho^2 over the free muscles and those at the kink s = 0 (every muscle at l = 0), rows owned by lanes
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i < np) { for (int k = 0; k < i; k++) H[TRI(i,k)] = 0; H[TRI(i,i)] = i < nv ? d.reserve[i]*d.reserve[i] : 1.0; } }
+      for (int mu = 0; mu < nu; mu++) { const double wm = d.weight ? d.weight[mu] : 1.0, q = sm[mu]/wm; if (!((q > 0 || sm[mu] == 0) && q < 1)) continue;
+        const int tt = at[mu], z0 = nadr[tt], z1 = nadr[tt+1]; const double c = cg[tt];
+        #pragma unroll
+        for (int cc = 0; cc < 2; cc++) { const int i = lane + 32*cc; if (i >= nv) continue;
+          double gi = 0; for (int z = z0; z < z1; z++) if (nzd[z] == i) gi += mom[z];
+          if (gi == 0) continue;
+          gi *= c*c/wm;
+          for (int z = z0; z < z1; z++) { const int k = nzd[z]; if (k <= i) H[TRI(i,k)] += gi*mom[z]; } } }
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i < np) x[i] = -F[c]; }      // (F = 0 on the padding rows)
+      __syncwarp();
+      chol_dense(H, nv, x, lane);
+      __syncwarp();
+      // Armijo backtracking on psi along x: psi(l + al x) - psi(l) = al x'(t - rho^2 l) - al^2/2 x' rho^2 x - sum_m [phi_m(s + al sd) - phi_m(s)]
+      // with sd = G' x, and slope x' grad psi = -F' x
+      double A1 = 0, A2 = 0, slope = 0;
+      #pragma unroll
+      for (int c = 0; c < 2; c++) { const int i = lane + 32*c; if (i >= nv) continue; const double r2 = d.reserve[i]*d.reserve[i];
+        A1 += x[i]*(t[i] - r2*lam[i]); A2 += r2*x[i]*x[i]; slope -= F[c]*x[i]; }
+      A1 = warp_sum(A1); A2 = warp_sum(A2); slope = warp_sum(slope);
+      double al = 1;
+      for (int ls = 0; ls < 60; ls++) { double ph = 0;
+        for (int i = lane; i < nu; i += 32) { const int tt = at[i]; double acc = 0; for (int z = nadr[tt]; z < nadr[tt+1]; z++) acc += mom[z]*x[nzd[z]];
+          ph += so_phi_diff(sm[i], al*(cg[tt]*acc), d.weight ? d.weight[i] : 1.0); }
+        const double dpsi = al*A1 - 0.5*al*al*A2 - warp_sum(ph);
+        if (dpsi >= 1e-4*al*slope) break;
+        al *= 0.5; }
+      for (int i = lane; i < nv; i += 32) lam[i] += al*x[i];
+      __syncwarp();
+    }
+    // outputs at the returned l: a(l), r, the excitation, the forces
+    if (lane == 0) { if (d.niter) d.niter[env] = it; if (d.converged) d.converged[env] = conv; if (d.residual) d.residual[env] = fnorm; }
+    for (int i = lane; i < nv; i += 32) { const size_t o = (size_t)env*nv + i; const double rho = d.reserve[i];
+      if (d.reserve_force) d.reserve_force[o] = rho*rho*lam[i];
+      if (d.lambda) d.lambda[o] = lam[i]; }
+    for (int i = lane; i < nu; i += 32) { const size_t o = (size_t)env*nu + i; const double act = clipd(sm[i]/(d.weight ? d.weight[i] : 1.0), 0, 1);
+      d.act[o] = act;
+      if (d.actuator_force) d.actuator_force[o] = gm[i]*act + bm[i];
+      if (d.ctrl) { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; const double dyn[3] = {LDC(ag), LDC(ag + 1), LDC(ag + 2)};
+        const bool lim = LDC(ag + 15) != 0; const double lo = lim ? fmax(LDC(ag + 13), 0.0) : 0.0, hi = lim ? fmin(LDC(ag + 14), 1.0) : 1.0;
+        d.ctrl[o] = so_excitation(dyn, W_(act)[i], act, m.timestep, lo, hi); } }
+    __syncwarp();
+  }
+}
+
 // ================================================================== host side (C-ABI)
 static thread_local std::string g_err;
 static int fail(const std::string& s) { g_err = s; return -1; }
@@ -886,7 +1030,8 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced;
   LaunchShape ik_shape; bool ik_ready;      // launch shape of myo_ik_kernel, set by the first myo_batch_ik
   // transition FD (myo_batch_transition_fd): launch shape of myo_fd_kernel for fd_items work items, and its per-slot rows
-  LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes; };
+  LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes;
+  LaunchShape so_shape; bool so_ready; int so_off[8]; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1352,5 +1497,53 @@ extern "C" int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, co
   a.fd.A = d->A; a.fd.B = d->B; a.fd.nom = b->dCarry; a.fd.rows = b->dFdRows; a.fd.eps = p->eps; a.fd.rinv1 = 1.0/p->eps; a.fd.rinv2 = 1.0/(2.0*p->eps);
   a.fd.n_env = b->n_env; a.fd.ncol = ncol; a.fd.nxa = nxa; a.fd.npass = p->centered ? 2 : 1;
   myo_fd_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+// Placement of myo_static_opt_kernel's arrays (SoArgs order: H, x, l, cg, tf, s, gm, bm), first fit by decreasing size in the per-env
+// scratch and the persistent dof axes and mass matrix (dead after the tendon pass).  gm and bm go first, outside the tendon moments, lengths
+// and velocities (the gain pass reads those while it writes them); the rest outside mom, gm and bm.  Offsets from the warp base, in doubles.
+static int so_plan(const DevModel& d, int* off) {
+  const int np = d.nvp, size[8] = {al2(np*(np + 1)/2), al2(np), al2(d.nv), al2(d.nta), al2(d.nta), al2(d.nu), al2(d.nu), al2(d.nu)};
+  int lo[16] = {d.s_mom, d.s_tlen, d.s_tvel}, hi[16] = {d.s_mom + al2(d.nnz), d.s_tlen + al2(d.nta), d.s_tvel + al2(d.nta)}, nused = 3;
+  const int room[2][2] = {{d.o_scr, d.n_per_warp}, {d.o_dax, d.o_fsm}};      // (dax, dan, qM are consecutive)
+  const int order[8] = {6, 7, 0, 1, 2, 3, 4, 5};
+  bool done[8] = {};
+  for (int r = 0; r < 8; r++) {
+    int k = -1;
+    if (r < 2) k = order[r];
+    else { if (r == 2) { lo[1] = lo[2] = hi[1] = hi[2] = 0; }      // tlen and tvel are dead after the gain pass
+      for (int q = 0; q < 6; q++) if (!done[q] && (k < 0 || size[q] > size[k])) k = q; }
+    int at = -1;
+    for (int g = 0; g < 2 && at < 0; g++) {
+      int c = room[g][0];      // the lowest start in this room that overlaps no used interval
+      for (bool moved = true; moved; ) { moved = false;
+        for (int u = 0; u < nused; u++) if (c < hi[u] && lo[u] < c + size[k]) { c = hi[u]; moved = true; } }
+      if (c + size[k] <= room[g][1]) at = c; }
+    if (at < 0) return fail("myo_batch_static_opt: the model's per-env scratch has no room for the dual Newton's arrays");
+    off[k] = at; lo[nused] = at; hi[nused] = at + size[k]; nused++; done[k] = true; }
+  return 0;
+}
+
+static_assert(sizeof(DevModel) + sizeof(SoArgs) <= 4096, "myo_static_opt_kernel's arguments fit the 4 KB kernel parameter space");
+
+extern "C" int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* d, const myo_static_opt_params* p, int flags, void* stream) {
+  if (!b || !d || !p) return fail("myo_batch_static_opt: null");
+  if (!d->qacc || !d->reserve || !d->act) return fail("myo_batch_static_opt: qacc, reserve and act are required");
+  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_static_opt: unknown flag bits");
+  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (!std::isfinite(p->tol)) return fail("myo_batch_static_opt: non-finite parameter");
+  if (p->tol < 0 || p->max_iter < 0) return fail("myo_batch_static_opt: needs tol >= 0 and max_iter >= 0");
+  if (b->dm.nv > 64) return fail("myo_batch_static_opt: models with more than 64 dofs are not supported");
+  CUDA_OK(cudaSetDevice(b->device));
+  if (!b->so_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+    if (so_plan(b->dm, b->so_off)) return -1;
+    if (launch_shape((const void*)myo_static_opt_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->so_shape)) return -1;
+    b->so_ready = true; }
+  SoArgs a; memset(&a, 0, sizeof(a));
+  a.d = *d; a.p = *p; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags;
+  a.o_H = b->so_off[0]; a.o_x = b->so_off[1]; a.o_l = b->so_off[2]; a.o_cg = b->so_off[3]; a.o_tf = b->so_off[4]; a.o_s = b->so_off[5]; a.o_gm = b->so_off[6]; a.o_bm = b->so_off[7];
+  const LaunchShape& s = b->so_shape;
+  myo_static_opt_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

@@ -379,29 +379,33 @@ __device__ __forceinline__ double muscle_FL(double L, double lmin, double lmax) 
     else if (L <= b) { x = (L-1)*m_rcp(fmax(MYO_MINVAL, b-1)); return 1-0.5*x*x; }
     else { x = (lmax-L)*m_rcp(fmax(MYO_MINVAL, lmax-b)); return 0.5*x*x; } }
   return 0; }
+// activation time constant of the step from act toward cc = clip(ctrl, 0, 1), dctrl = cc - act (mju_muscleDynamics)
+__device__ __forceinline__ double muscle_tau(const double* dyn, double dctrl, double act) {
+  double ac = clipd(act, 0, 1), ta = dyn[0]*(0.5+1.5*ac), td = dyn[1]*m_rcp(0.5+1.5*ac), tau;
+  if (dyn[2] < MYO_MINVAL) tau = dctrl > 0 ? ta : td;
+  else { double x = clipd(dctrl/dyn[2]+0.5, 0, 1), s = x*x*x*(3*x*(2*x-5)+10); tau = td+(ta-td)*s; }
+  return tau; }
+// gain (active force-length-velocity) and bias (passive force) at actuator length len and velocity vel: force = gain act + bias
+__device__ __forceinline__ void muscle_gain_bias(const double* gp, const double* bp, const double* am, double len, double vel, double& gain, double& bias) {
+  const double g_lmin = gp[2], g_lmax = gp[3], g_vmax = gp[4], g_fvmax = gp[5], b_lmax = bp[2], b_fpmax = bp[3], lr0 = am[2], lr1 = am[3];
+  double F = am[0], L0 = (lr1-lr0)*m_rcp(fmax(MYO_MINVAL, gp[1]-gp[0])), L = gp[0]+(len-lr0)*m_rcp(fmax(MYO_MINVAL, L0)), V = vel*m_rcp(fmax(MYO_MINVAL, L0*g_vmax));
+  double FL = muscle_FL(L, g_lmin, g_lmax), y = g_fvmax-1, FV;
+  if (V <= -1) FV = 0; else if (V <= 0) FV = (V+1)*(V+1); else if (V <= y) FV = g_fvmax-(y-V)*(y-V)*m_rcp(fmax(MYO_MINVAL, y)); else FV = g_fvmax;
+  gain = -F*FL*FV;
+  double Fb = am[1], L0b = (lr1-lr0)*m_rcp(fmax(MYO_MINVAL, bp[1]-bp[0])), Lb = bp[0]+(len-lr0)*m_rcp(fmax(MYO_MINVAL, L0b)), b = 0.5*(1+b_lmax);
+  if (Lb <= 1) bias = 0; else if (Lb <= b) { double x = (Lb-1)*m_rcp(fmax(MYO_MINVAL, b-1)); bias = -Fb*b_fpmax*0.5*x*x; }
+  else { double x = (Lb-b)*m_rcp(fmax(MYO_MINVAL, b-1)); bias = -Fb*b_fpmax*(0.5+x); } }
 
 // tap_force / tap_len: nullable global rows for the parity taps (values before the activation is advanced)
 template <class MD> __device__ void phase_actuation(const MD& m, const Warp w, bool integrate, const double* ctrl_row, double* tap_force, double* tap_len) {
   const idx_t* atend = CI(PA_tendon); const idx_t* acls = CI(PA_cls); const double* __restrict__ PAc = GD(PA_d); const double* __restrict__ PAm = GD(PAM_d);      // (cold tables: 17 + 5 independent read-only loads per actuator)
   double* tlen = SCR(s_tlen); double* tvel = SCR(s_tvel); double* tfrc = SCR(s_tfrc); double* mom = SCR(s_mom);
   for (int i = w.lane; i < m.nu; i += 32) { double a[PA_STRIDE]; { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; for (int c = 0; c < 16; c++) a[c] = LDC(ag + c); } double am[5]; for (int c = 0; c < 5; c++) am[c] = LDC(PAm + i*PAM_STRIDE + c); int t = atend[i];
-    const double *dyn = a, *gp = a+3, *bp = a+9, *cr = a+13; double gear = am[4], lr0 = am[2], lr1 = am[3];
+    const double *dyn = a, *gp = a+3, *bp = a+9, *cr = a+13; double gear = am[4];
     double len = gear*tlen[t], vel = gear*tvel[t], ctrl = ctrl_row[i], act = W_(act)[i];
     if (a[15] != 0) ctrl = clipd(ctrl, cr[0], cr[1]);
-    // activation dynamics
-    double cc = clipd(ctrl, 0, 1), ac = clipd(act, 0, 1), ta = dyn[0]*(0.5+1.5*ac), td = dyn[1]*m_rcp(0.5+1.5*ac), dctrl = cc - act, tau;
-    if (dyn[2] < MYO_MINVAL) tau = dctrl > 0 ? ta : td;
-    else { double x = clipd(dctrl/dyn[2]+0.5, 0, 1), s = x*x*x*(3*x*(2*x-5)+10); tau = td+(ta-td)*s; }
-    double actdot = dctrl*m_rcp(fmax(MYO_MINVAL, tau));
-    // gain (active force-length-velocity) and bias (passive force)
-    const double g_lmin = gp[2], g_lmax = gp[3], g_vmax = gp[4], g_fvmax = gp[5], b_lmax = bp[2], b_fpmax = bp[3];
-    double F = am[0], L0 = (lr1-lr0)*m_rcp(fmax(MYO_MINVAL, gp[1]-gp[0])), L = gp[0]+(len-lr0)*m_rcp(fmax(MYO_MINVAL, L0)), V = vel*m_rcp(fmax(MYO_MINVAL, L0*g_vmax));
-    double FL = muscle_FL(L, g_lmin, g_lmax), y = g_fvmax-1, FV;
-    if (V <= -1) FV = 0; else if (V <= 0) FV = (V+1)*(V+1); else if (V <= y) FV = g_fvmax-(y-V)*(y-V)*m_rcp(fmax(MYO_MINVAL, y)); else FV = g_fvmax;
-    double gain = -F*FL*FV;
-    double Fb = am[1], L0b = (lr1-lr0)*m_rcp(fmax(MYO_MINVAL, bp[1]-bp[0])), Lb = bp[0]+(len-lr0)*m_rcp(fmax(MYO_MINVAL, L0b)), b = 0.5*(1+b_lmax), bias;
-    if (Lb <= 1) bias = 0; else if (Lb <= b) { double x = (Lb-1)*m_rcp(fmax(MYO_MINVAL, b-1)); bias = -Fb*b_fpmax*0.5*x*x; }
-    else { double x = (Lb-b)*m_rcp(fmax(MYO_MINVAL, b-1)); bias = -Fb*b_fpmax*(0.5+x); }
+    double cc = clipd(ctrl, 0, 1), dctrl = cc - act, actdot = dctrl*m_rcp(fmax(MYO_MINVAL, muscle_tau(dyn, dctrl, act)));      // activation dynamics
+    double gain, bias; muscle_gain_bias(gp, bp, am, len, vel, gain, bias);
     double force = gain*act + bias;
     tfrc[t] = gear*force;   // one actuator per tendon (checked on the host)
     if (tap_force) tap_force[i] = force;

@@ -559,6 +559,65 @@ class MyoVecEnv:
         self.batch.transition_fd(params, stream=self._stream(), **bufs, **out)
         return out
 
+    STATIC_OPT_FIELDS = tuple(abi.STATIC_OPT_SHAPES)
+    STATIC_OPT_DEFAULTS = dict(max_iter=50, tol=1e-12)
+
+    def static_opt(self, qacc, reserve, weight=None, constraints=True, discrete=False, warmstart=None, max_iter=STATIC_OPT_DEFAULTS["max_iter"],
+                   tol=STATIC_OPT_DEFAULTS["tol"], fields=("act", "reserve_force", "ctrl")):
+        """Muscle static optimisation of every env at its current (qpos, qvel, act) (myo_batch_static_opt; include/myo_b200.h states the
+        problem and the solver): the activations a in [0, 1] and reserve generalized forces r of least 1/2 sum w a^2 + 1/2 sum (r / reserve)^2
+        whose muscle and reserve forces produce the acceleration qacc, i.e. G a + r = qfrc_inverse(qacc) - AM' bias.  qacc [num_envs, nv]
+        as inverse() takes it, with its constraints and discrete flags; reserve: the reserve strengths rho > 0, a scalar or [nv] (no
+        default: the right scale differs by orders of magnitude between models); weight: muscle weights [nu] > 0 (None: 1); warmstart:
+        the dual lambda [num_envs, nv] of an earlier call (None: 0).  Tensors are contiguous float64 CUDA tensors on this batch's device.
+        Returns {field: tensor [num_envs, ...]} of STATIC_OPT_FIELDS: act, reserve_force [nv], ctrl (the excitation that takes the current
+        act to a in one mj_step, clipped to ctrlrange), actuator_force, muscle_gain, muscle_bias [nu], qfrc_inverse, lambda [nv], niter,
+        converged (int32) and residual (|G a + r - t|_inf, converged when <= tol max(1, |t|_inf)); allocated per call.  One launch; not a
+        state change."""
+        torch, m, n = self.torch, self.mj_model, self.num_envs
+        fields = tuple(fields)
+        bad = [f for f in fields if f not in self.STATIC_OPT_FIELDS]
+        if bad:
+            raise KeyError("unknown static_opt fields %s (available: %s)" % (bad, list(self.STATIC_OPT_FIELDS)))
+
+        def check(name, x, shape):
+            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
+                    or not x.is_contiguous()):
+                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
+                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
+                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+
+        def positive(name, x, width):
+            if isinstance(x, torch.Tensor):
+                check(name, x, (width,))
+            else:
+                v = np.asarray(x, dtype=np.float64)
+                if v.shape not in ((), (width,)):
+                    raise ValueError("%s must be a scalar or of shape (%d,), got %s" % (name, width, v.shape))
+                x = torch.as_tensor(np.broadcast_to(v, (width,)).copy(), device=self.device)
+            if not bool(torch.all(torch.isfinite(x) & (x > 0))):
+                raise ValueError("%s must be finite and > 0" % name)
+            return x
+        check("qacc", qacc, (n, m.nv))
+        bufs = {"qacc": qacc, "reserve": positive("reserve", reserve, m.nv)}
+        if weight is not None:
+            bufs["weight"] = positive("weight", weight, m.nu)
+        if warmstart is not None:
+            check("warmstart", warmstart, (n, m.nv))
+            bufs["lambda0"] = warmstart
+        params = abi.MyoStaticOptParams(max_iter=int(max_iter), tol=float(tol))
+        if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
+            raise ValueError("static_opt needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (max_iter, tol))
+        size = dict(nu=m.nu, nv=m.nv)
+        out = {}
+        for f in set(fields) | {"act"}:
+            shape = (n,) + tuple(size[x] for x in abi.STATIC_OPT_SHAPES[f])
+            out[f] = (torch.full(shape, -1, dtype=torch.int32, device=self.device) if f in ("niter", "converged")
+                      else torch.full(shape, float("nan"), dtype=torch.float64, device=self.device))
+        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
+        self.batch.static_opt(params, stream=self._stream(), flags=flags, **bufs, **out)
+        return {f: out[f] for f in fields}
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -760,6 +819,17 @@ class MyoEnv:
         out = v.ik(sites, as_dev(target_pos, (1, ns, 3)), target_quat=as_dev(target_quat, (1, ns, 4)), qpos_init=as_dev(qpos_init, (1, -1)),
                    qpos_ref=as_dev(qpos_ref, (1, -1)), dofs=dofs, site_weight=as_dev(site_weight, (ns, 2)), fields=fields, **params)
         return {k: (int(x[0]) if k in ("niter", "converged") else x[0].cpu().numpy()) for k, x in out.items()}
+
+    def static_opt(self, qacc, reserve, weight=None, constraints=True, discrete=False, warmstart=None, fields=("act", "reserve_force", "ctrl"),
+                   **params):
+        """Muscle static optimisation of this env at its current state (MyoVecEnv.static_opt): qacc [nv], reserve (scalar or [nv]),
+        weight [nu] or None, warmstart [nv] or None; params: max_iter, tol.  Returns {field: numpy array} (niter and converged as ints).
+        Not a state change.  One device-to-host copy per field."""
+        v = self.vec
+        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        out = v.static_opt(as_dev(qacc, (1, -1)), reserve if np.ndim(reserve) == 0 else as_dev(reserve, (-1,)), weight=as_dev(weight, (-1,)),
+                           constraints=constraints, discrete=discrete, warmstart=as_dev(warmstart, (1, -1)), fields=fields, **params)
+        return {k: (int(x[0]) if k in ("niter", "converged") else (float(x[0]) if k == "residual" else x[0].cpu().numpy())) for k, x in out.items()}
 
     def mj_jacSite(self, site):
         """mujoco.mj_jacSite at the current state: (jacp [3, nv], jacr [3, nv]) as numpy arrays."""
