@@ -204,6 +204,21 @@ def _bind(L):
     return L
 
 
+def _buffers(cls, tensors):
+    """A cls (a struct of device pointers) with each tensor's data pointer in the field of its name; None leaves the field null."""
+    s = cls()
+    names = {n for n, _ in cls._fields_}
+    for k, t in tensors.items():
+        if k not in names:
+            raise KeyError(k)
+        if t is None:
+            continue
+        if not t.is_contiguous():
+            raise ValueError("%s must be contiguous" % k)
+        setattr(s, k, t.data_ptr())
+    return s
+
+
 def _check(rc, L=None):
     if rc != 0:
         raise MyoError((L or lib()).myo_last_error().decode())
@@ -260,15 +275,7 @@ class Batch:
     def bind(self, **tensors):
         """tensors: name -> torch CUDA tensor (contiguous) for the fields of myo_buffers."""
         self.tensors.update(tensors)
-        b = MyoBuffers()
-        for k, t in self.tensors.items():
-            if k not in BUFFER_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(b, k, t.data_ptr())
+        b = _buffers(MyoBuffers, self.tensors)
         _check(self.L.myo_batch_bind(self.handle, ctypes.byref(b)), self.L)
 
     def reset(self, mask=None, seed=0, env_offset=0, stream=None):
@@ -293,85 +300,37 @@ class Batch:
 
     def data(self, stream=None, **tensors):
         """mjData readout (myo_batch_data) into the given torch CUDA tensors (names of DATA_FIELDS; only these are computed)."""
-        d = MyoDataBuffers()
-        for k, t in tensors.items():
-            if k not in DATA_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoDataBuffers, tensors)
         _check(self.L.myo_batch_data(self.handle, ctypes.byref(d), stream), self.L)
 
     def inverse(self, stream=None, flags=0, **tensors):
         """Inverse dynamics (myo_batch_inverse) into the given torch CUDA tensors (names of INVERSE_FIELDS: qacc in, the others out; qacc and
         qfrc_inverse are required).  flags: INV_NOCONSTRAINT | INV_DISCRETE."""
-        d = MyoInverseBuffers()
-        for k, t in tensors.items():
-            if k not in INVERSE_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoInverseBuffers, tensors)
         _check(self.L.myo_batch_inverse(self.handle, ctypes.byref(d), flags, stream), self.L)
 
     def rollout(self, nstep, substeps, stream=None, **tensors):
         """mj_step rollout (myo_batch_rollout) of nstep intervals of `substeps` mj_steps with the given torch CUDA tensors (names of
         ROLLOUT_FIELDS: ctrl [n, nstep, nu] required, qfrc_applied and the start state *0 in, the others out)."""
-        d = MyoRolloutBuffers()
-        for k, t in tensors.items():
-            if k not in ROLLOUT_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoRolloutBuffers, tensors)
         _check(self.L.myo_batch_rollout(self.handle, ctypes.byref(d), nstep, substeps, stream), self.L)
 
     def ik(self, params, stream=None, **tensors):
         """Inverse kinematics (myo_batch_ik) with the given torch CUDA tensors (names of IK_FIELDS: site_id, target_pos and qpos are
         required) and a MyoIkParams."""
-        d = MyoIkBuffers()
-        for k, t in tensors.items():
-            if k not in IK_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoIkBuffers, tensors)
         _check(self.L.myo_batch_ik(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
 
     def transition_fd(self, params, stream=None, **tensors):
         """Finite-difference transition Jacobians (myo_batch_transition_fd) with the given torch CUDA tensors (names of FD_FIELDS: ctrl
         [n, nu] and at least one of A, B are required) and a MyoFdParams."""
-        d = MyoFdBuffers()
-        for k, t in tensors.items():
-            if k not in FD_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoFdBuffers, tensors)
         _check(self.L.myo_batch_transition_fd(self.handle, ctypes.byref(d), ctypes.byref(params), stream), self.L)
 
     def static_opt(self, params, stream=None, flags=0, **tensors):
         """Muscle static optimisation (myo_batch_static_opt) with the given torch CUDA tensors (names of STATIC_OPT_FIELDS: qacc, reserve
         and act are required), a MyoStaticOptParams and MYO_INV_* flags."""
-        d = MyoStaticOptBuffers()
-        for k, t in tensors.items():
-            if k not in STATIC_OPT_FIELDS:
-                raise KeyError(k)
-            if t is None:
-                continue
-            if not t.is_contiguous():
-                raise ValueError("%s must be contiguous" % k)
-            setattr(d, k, t.data_ptr())
+        d = _buffers(MyoStaticOptBuffers, tensors)
         _check(self.L.myo_batch_static_opt(self.handle, ctypes.byref(d), ctypes.byref(params), flags, stream), self.L)
 
     @property

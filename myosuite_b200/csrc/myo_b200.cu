@@ -517,6 +517,20 @@ extern "C" __global__ void __launch_bounds__(448) myo_roll_kernel_w14(const __gr
 extern "C" __global__ void __launch_bounds__(320) myo_fd_kernel(const __grid_constant__ DevModel m, const __grid_constant__ StepArgs a) { env_kernel_body<false, 320, true, true>(m, a); }
 static_assert(sizeof(HandShape) + sizeof(StepArgs) <= 4096, "the step kernels' arguments fit the 4 KB kernel parameter space");
 
+// ------------------------------------------------------------------ the one-env-per-warp analysis kernels
+// Their prologue: the model staged into shared memory when `stage` holds, then this warp's index `wid`, the CTA's warp count `nw` and its
+// slice `w`.  Macros for the reason STAGE_MODEL is one: the same statements written out in each kernel give the same machine code.
+#define WARP_KERNEL_PROLOGUE(m, stage) \
+  __shared__ __align__(8) unsigned long long mbar; \
+  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5; \
+  if (stage) STAGE_MODEL(m, mbar) \
+  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+// `FOR_EACH_WARP_ENV(env, n_env) body`: this warp's envs on the balanced map (env = CTA + grid * slot), in slot order; the body may
+// `continue` to the next env or `break` out of the walk
+#define FOR_EACH_WARP_ENV(env, n_env) \
+  for (int per_cta_ = SLOTS_PER_CTA(1, (n_env), (int)gridDim.x, nw), j_ = wid; j_ < per_cta_; j_ += nw) \
+    if (const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j_ - wid, wid); env >= (n_env)) break; else
+
 // ------------------------------------------------------------------ mjData readout (myo_batch_data)
 // One forward pass over the stored state of every env, one env per warp on the balanced map (env = CTA + grid * slot).  Each field is
 // written while the scratch region holding it is live; nothing is stored back (the Newton warm start is read, the inverse-wrap roots
@@ -622,15 +636,9 @@ __device__ void data_solve(const DevModel& m, const Warp w, const DataArgs& a, i
 }
 
 extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DataArgs a) {
-  __shared__ __align__(8) unsigned long long mbar;
-  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (a.depth != DATA_NONE) STAGE_MODEL(m, mbar)
-  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  WARP_KERNEL_PROLOGUE(m, a.depth != DATA_NONE)
   const myo_data_buffers& d = a.d; const myo_buffers& b = a.b;
-  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
-  for (int j = wid; j < per_cta; j += nw) {
-    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
-    if (env >= a.n_env) break;
+  FOR_EACH_WARP_ENV(env, a.n_env) {
     if (a.pose) data_poses(m, a, env, w.lane);
     if (a.depth == DATA_NONE) continue;
     if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
@@ -702,15 +710,9 @@ __device__ __forceinline__ void inverse_pass(const DevModel& m, const Warp w, co
 }
 
 extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __grid_constant__ DevModel m, const __grid_constant__ InvArgs a) {
-  __shared__ __align__(8) unsigned long long mbar;
-  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  STAGE_MODEL(m, mbar)
-  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  WARP_KERNEL_PROLOGUE(m, true)
   const myo_inverse_buffers& d = a.d; const bool constraints = !(a.flags & MYO_INV_NOCONSTRAINT), discrete = a.flags & MYO_INV_DISCRETE;
-  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
-  for (int j = wid; j < per_cta; j += nw) {
-    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
-    if (env >= a.n_env) break;
+  FOR_EACH_WARP_ENV(env, a.n_env) {
     inverse_pass(m, w, a.b, env, d.qacc, d.actuator_moment, constraints, discrete);
     for (int i = w.lane; i < m.nv; i += 32) { const size_t o = (size_t)env*m.nv + i;
       d.qfrc_inverse[o] = S_Ma[i] - W_(fsm)[i] - S_g[i];
@@ -754,19 +756,13 @@ __device__ __forceinline__ void ik_rotvec(const double* Q, const double* R, doub
 }
 
 extern "C" __global__ void __launch_bounds__(320) myo_ik_kernel(const __grid_constant__ DevModel m, const __grid_constant__ IkArgs a) {
-  __shared__ __align__(8) unsigned long long mbar;
-  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  STAGE_MODEL(m, mbar)
-  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  WARP_KERNEL_PROLOGUE(m, true)
   const myo_ik_buffers& d = a.d; const int ns = a.p.nsite, nv = m.nv, np = m.nvp, lane = w.lane; const bool rot = d.target_quat != nullptr;
   unsigned long long keep = ~0ull;      // dofs that may move
   if (d.dof_mask) keep = (unsigned long long)__ballot_sync(FULL, lane < nv && d.dof_mask[lane]) | (unsigned long long)__ballot_sync(FULL, lane + 32 < nv && d.dof_mask[lane + 32]) << 32;
   double* H = S_H; double* g = S_g; double* bx = S_a; double* by = S_Ma; double* bz = S_Mp;
   const idx_t* jtype = CI(jnt_type); const idx_t* jq = CI(jnt_qposadr); const idx_t* jd = CI(jnt_dofadr); const idx_t* lin = CI(PD_lin);
-  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
-  for (int jslot = wid; jslot < per_cta; jslot += nw) {
-    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, jslot - wid, wid);
-    if (env >= a.n_env) break;
+  FOR_EACH_WARP_ENV(env, a.n_env) {
     const double* q0 = (d.qpos0 ? d.qpos0 : a.bound_qpos) + (size_t)env*m.nq; const double* ref = d.qpos_ref ? d.qpos_ref + (size_t)env*m.nq : q0;
     for (int i = lane; i < m.nq; i += 32) W_(qpos)[i] = q0[i];
     __syncwarp();
@@ -898,10 +894,7 @@ __device__ __forceinline__ double so_excitation(const double* dyn, double act, d
 }
 
 extern "C" __global__ void __launch_bounds__(320) myo_static_opt_kernel(const __grid_constant__ DevModel m, const __grid_constant__ SoArgs a) {
-  __shared__ __align__(8) unsigned long long mbar;
-  const int wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  STAGE_MODEL(m, mbar)
-  const Warp w = { m.nD + (m.nI16w + 1)/2 + wid*m.n_per_warp, (int)(threadIdx.x & 31) };
+  WARP_KERNEL_PROLOGUE(m, true)
   const myo_static_opt_buffers& d = a.d; const bool constraints = !(a.flags & MYO_INV_NOCONSTRAINT), discrete = a.flags & MYO_INV_DISCRETE;
   const int nv = m.nv, nu = m.nu, np = m.nvp, lane = w.lane;
   double* t = W_(fsm); double* H = smem + w.base + a.o_H; double* x = smem + w.base + a.o_x; double* lam = smem + w.base + a.o_l;
@@ -910,10 +903,7 @@ extern "C" __global__ void __launch_bounds__(320) myo_static_opt_kernel(const __
   const idx_t* at = CI(PA_tendon); const idx_t* acls = CI(PA_cls); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof);
   const idx_t* cadr = CI(PCOL_adr); const idx_t* col = CI(PCOL); const idx_t* nzt = CI(PNZ_tendon);
   const double* __restrict__ PAc = GD(PA_d); const double* __restrict__ PAm = GD(PAM_d);
-  const int per_cta = SLOTS_PER_CTA(1, a.n_env, (int)gridDim.x, nw);
-  for (int j = wid; j < per_cta; j += nw) {
-    const int env = slot_env(1, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid);
-    if (env >= a.n_env) break;
+  FOR_EACH_WARP_ENV(env, a.n_env) {
     inverse_pass(m, w, a.b, env, d.qacc, nullptr, constraints, discrete);
     for (int i = lane; i < nv; i += 32) { const double v = S_Ma[i] - W_(fsm)[i] - S_g[i]; t[i] = v; if (d.qfrc_inverse) d.qfrc_inverse[(size_t)env*nv + i] = v; }
     __syncwarp();
@@ -1020,18 +1010,18 @@ __global__ void __launch_bounds__(1024) myo_regroup_kernel(const int* __restrict
 }
 
 struct LaunchShape { int warps, smem, grid; };      // env-warps per CTA, dynamic shared memory (bytes), CTAs
+struct LazyShape { LaunchShape s; bool ready; };    // a launch shape sized by the first call that launches its kernel
 // Zero-initialised by myo_batch_create (new myo_batch()), so that myo_batch_destroy can free a partly built batch.
 struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; double tol; myo_buffers bufs; bool bound; DevModel dm; int32_t* dI; double* dD; double* dCtrl; int const_bytes, cold_bytes;
   LaunchShape prod, dbg; int balanced, dbg_balanced, obs_dim; bool use_w14, use_hand; bool regroup; int* dLoad; int* dPerm; int perm_rounds, perm_slots; bool perm_built; long long launches; unsigned long long seed; long long env_offset;
   // mjData readout (myo_batch_data), set up by its first call: model tables in HBM, the pose scratch and the launch shape of myo_data_kernel
-  int32_t* dRI; double* dRD; double* dPose; DataArgs data; LaunchShape data_shape; bool data_ready;
-  LaunchShape inv_shape; bool inv_ready;      // launch shape of myo_inverse_kernel, set by the first myo_batch_inverse
+  int32_t* dRI; double* dRD; double* dPose; DataArgs data; LazyShape data_shape;
+  LazyShape inv_shape, ik_shape;      // launch shapes of myo_inverse_kernel and myo_ik_kernel
   // rollout (myo_batch_rollout), set up by its first call: carry state [n, nq + 2 nv + na + 1] (qpos | qvel | act | warm start | time)
-  bool big; double* dCarry; LaunchShape roll_shape; bool roll_ready, roll_regroup, roll_balanced;
-  LaunchShape ik_shape; bool ik_ready;      // launch shape of myo_ik_kernel, set by the first myo_batch_ik
+  bool big; double* dCarry; LazyShape roll_shape; bool roll_regroup, roll_balanced;
   // transition FD (myo_batch_transition_fd): launch shape of myo_fd_kernel for fd_items work items, and its per-slot rows
   LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes;
-  LaunchShape so_shape; bool so_ready; int so_off[8]; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt
+  LazyShape so_shape; int so_off[8]; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1110,6 +1100,14 @@ static int launch_shape(const void* fn, const cudaDeviceProp& prop, int per_env_
   const int need = (n_env + wpc - 1)/wpc, cap = sms*c; s.grid = need < cap ? need : cap;
   return 0;
 }
+// The launch shape of a one-env-per-warp analysis kernel `fn` over the batch, sized from the kernel's own register and thread limits at
+// the first call that launches it
+static int analysis_shape(const myo_batch* b, const void* fn, LazyShape& l) {
+  if (l.ready) return 0;
+  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+  if (launch_shape(fn, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, l.s)) return -1;
+  l.ready = true; return 0;
+}
 
 // Everything myo_batch_create does after allocating the batch; on failure the caller destroys the partly built batch.
 static int batch_setup(myo_batch* b, const myo_model* m, const myo_task_cfg* cfg) {
@@ -1180,7 +1178,7 @@ extern "C" int myo_batch_create(const myo_model* m, int device, int n_env, const
 // The readout's device memory and set-up (also on a failed data_setup, which leaves the batch as if it had not run)
 static void data_release(myo_batch* b) {
   cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
-  memset(&b->data, 0, sizeof(b->data)); b->data_shape = LaunchShape(); b->data_ready = false; }
+  memset(&b->data, 0, sizeof(b->data)); b->data_shape = LazyShape(); }
 extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
   cudaFree(b->dCarry); cudaFree(b->dFdRows); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
@@ -1232,6 +1230,8 @@ extern "C" int myo_debug_chol_solve(int device, const double* H_host, double* x_
   cudaFree(dH); cudaFree(dx); return 0;
 }
 
+static int require_bound(const myo_batch* b) { return b->bound ? 0 : fail("batch has no bound buffers (call myo_batch_bind)"); }
+
 extern "C" int myo_batch_bind(myo_batch* b, const myo_buffers* bufs) {
   if (!b || !bufs) return fail("myo_batch_bind: null");
   if (!bufs->qpos || !bufs->qvel || !bufs->qacc_warmstart || (b->dm.na && !bufs->act)) return fail("myo_batch_bind: qpos/qvel/act/qacc_warmstart are required");
@@ -1243,7 +1243,7 @@ extern "C" int myo_batch_bind(myo_batch* b, const myo_buffers* bufs) {
 }
 
 static int launch(myo_batch* b, StepArgs& a, void* stream) {
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   CUDA_OK(cudaSetDevice(b->device));
   a.b = b->bufs; a.cfg = b->cfg; a.n_env = b->n_env; a.obs_dim = b->obs_dim; a.dt = b->dm.timestep*b->cfg.frame_skip;
   a.seed = b->seed; a.env_offset = b->env_offset;
@@ -1315,21 +1315,19 @@ static int data_setup(myo_batch* b) {
   a.jtype = b->dRI + o_jtype; a.jq = b->dRI + o_jq; a.site_body = b->dRI + o_sb; a.pair_geom = b->dRI + o_pg;
   a.bpos = b->dRD + od[0]; a.bquat = b->dRD + od[1]; a.jpos = b->dRD + od[2]; a.jaxis = b->dRD + od[3]; a.qpos0 = b->dRD + od[4]; a.site_pos = b->dRD + od[5];
   a.pose_buf = b->dPose; a.n_env = b->n_env; a.tol = b->tol;
-  cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
-  if (launch_shape((const void*)myo_data_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->data_shape)) return -1;
-  b->data_ready = true; return 0;
+  return analysis_shape(b, (const void*)myo_data_kernel, b->data_shape);
 }
 
 extern "C" int myo_batch_data(myo_batch* b, const myo_data_buffers* d, void* stream) {
   if (!b || !d) return fail("myo_batch_data: null");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   const bool pose = d->xpos || d->xquat || d->xmat || d->site_xpos;
   const bool act = d->actuator_length || d->actuator_velocity || d->actuator_force || d->qfrc_actuator;
   const bool dyn = d->qacc || d->ncon || d->contact_geom || d->contact_dist || d->contact_pos || d->contact_frame || d->contact_force;
   if (!pose && !act && !dyn) return 0;
   CUDA_OK(cudaSetDevice(b->device));
-  if (!b->data_ready) { if (const int rc = data_setup(b)) { data_release(b); return rc; } }
-  DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE); const LaunchShape& s = b->data_shape;
+  if (!b->data_shape.ready) { if (const int rc = data_setup(b)) { data_release(b); return rc; } }
+  DataArgs a = b->data; a.d = *d; a.b = b->bufs; a.pose = pose; a.depth = dyn ? DATA_DYN : (act ? DATA_ACT : DATA_NONE); const LaunchShape& s = b->data_shape.s;
   myo_data_kernel<<<s.grid, s.warps*32, a.depth == DATA_NONE ? 0 : s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
@@ -1338,12 +1336,10 @@ extern "C" int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int
   if (!b || !d) return fail("myo_batch_inverse: null");
   if (!d->qacc || !d->qfrc_inverse) return fail("myo_batch_inverse: qacc and qfrc_inverse are required");
   if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_inverse: unknown flag bits");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   CUDA_OK(cudaSetDevice(b->device));
-  if (!b->inv_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
-    if (launch_shape((const void*)myo_inverse_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->inv_shape)) return -1;
-    b->inv_ready = true; }
-  InvArgs a; a.d = *d; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags; const LaunchShape& s = b->inv_shape;
+  if (analysis_shape(b, (const void*)myo_inverse_kernel, b->inv_shape)) return -1;
+  InvArgs a; a.d = *d; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags; const LaunchShape& s = b->inv_shape.s;
   myo_inverse_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
@@ -1354,19 +1350,28 @@ extern "C" int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int
 static int roll_setup(myo_batch* b) {
   cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
   const char* want_env = getenv("MYO_B200_WARPS_PER_CTA"); const int want = want_env ? atoi(want_env) : 0;
-  if (launch_shape(b->use_w14 ? (const void*)myo_roll_kernel_w14 : (const void*)myo_roll_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, b->big, want, b->roll_shape)) return -1;
-  const bool same = b->roll_shape.warps == b->prod.warps && b->roll_shape.grid == b->prod.grid && b->roll_shape.smem == b->prod.smem - b->cold_bytes;      // (less the hand kernel's cold tables)
+  LaunchShape& s = b->roll_shape.s;
+  if (launch_shape(b->use_w14 ? (const void*)myo_roll_kernel_w14 : (const void*)myo_roll_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, b->big, want, s)) return -1;
+  const bool same = s.warps == b->prod.warps && s.grid == b->prod.grid && s.smem == b->prod.smem - b->cold_bytes;      // (less the hand kernel's cold tables)
   b->roll_regroup = same && b->regroup; b->roll_balanced = same ? b->balanced : 1;
   const DevModel& d = b->dm;
   CUDA_OK(cudaMalloc(&b->dCarry, (size_t)b->n_env*(d.nq + 2*d.nv + d.na + 1)*8));
-  b->roll_ready = true; return 0;
+  b->roll_shape.ready = true; return 0;
 }
 
 static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream);
+// The StepArgs of a physics-only interval of `substeps` substeps (rollout and transition FD): the batch's model and solver with no task,
+// fatigue, reafferentation or auto-reset; the caller sets the state buffers, the roll / fd blocks, the slot map and the slot count
+static StepArgs physics_args(const myo_batch* b, int substeps) {
+  StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 0;
+  a.cfg = b->cfg; a.cfg.task = MYO_TASK_NONE; a.cfg.muscle_condition = MYO_COND_NONE; a.cfg.reaf_dst = a.cfg.reaf_src = 0; a.cfg.auto_reset = 0; a.cfg.frame_skip = substeps;
+  a.dt = b->dm.timestep*substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset;
+  return a;
+}
 extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
   if (!b || !r) return fail("myo_batch_rollout: null");
   if (!r->ctrl) return fail("myo_batch_rollout: ctrl is required");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   if (nstep < 1 || substeps < 1) return fail("myo_batch_rollout: nstep and substeps must be >= 1");
   CUDA_OK(cudaSetDevice(b->device));
   return roll_run(b, r, nstep, substeps, stream);
@@ -1374,7 +1379,7 @@ extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int
 
 // The launches of a checked rollout, on the current device: the carry from the start state, then one launch per interval
 static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
-  if (!b->roll_ready) { if (const int rc = roll_setup(b)) { cudaFree(b->dCarry); b->dCarry = nullptr; return rc; } }
+  if (!b->roll_shape.ready) { if (const int rc = roll_setup(b)) { cudaFree(b->dCarry); b->dCarry = nullptr; return rc; } }
   const DevModel& d = b->dm; const size_t n = b->n_env; cudaStream_t st = (cudaStream_t)stream;
   // the carry: the start state, from the caller's rows or the bound buffers
   myo_buffers c; memset(&c, 0, sizeof(c));
@@ -1388,10 +1393,8 @@ static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int s
     else CUDA_OK(cudaMemsetAsync(f.dst, 0, n*f.width*8, st)); }      // (an unbound time buffer: the rollout starts at 0)
   if (r->overflow) CUDA_OK(cudaMemsetAsync(r->overflow, 0, n*4, st));
   c.env_prm = q.env_prm; c.overflow = r->overflow;
-  StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 0; a.b = c; a.roll = *r; a.roll_nstep = nstep;
-  a.cfg = b->cfg; a.cfg.task = MYO_TASK_NONE; a.cfg.muscle_condition = MYO_COND_NONE; a.cfg.reaf_dst = a.cfg.reaf_src = 0; a.cfg.auto_reset = 0; a.cfg.frame_skip = substeps;
-  a.n_env = b->n_env; a.dt = d.timestep*substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset; a.balanced = b->roll_balanced;
-  const LaunchShape& s = b->roll_shape;
+  StepArgs a = physics_args(b, substeps); a.b = c; a.roll = *r; a.roll_nstep = nstep; a.n_env = b->n_env; a.balanced = b->roll_balanced;
+  const LaunchShape& s = b->roll_shape.s;
   if (b->roll_regroup) { a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; }
   for (int t = 0; t < nstep; t++) {
     a.roll_t = t;
@@ -1441,7 +1444,7 @@ static_assert(sizeof(DevModel) + sizeof(IkArgs) <= 4096, "myo_ik_kernel's argume
 extern "C" int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_params* p, void* stream) {
   if (!b || !d || !p) return fail("myo_batch_ik: null");
   if (!d->site_id || !d->site_quat || !d->target_pos || !d->qpos) return fail("myo_batch_ik: site_id, site_quat, target_pos and qpos are required");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   const int ns = p->nsite;
   if (ns < 1 || ns > MYO_IK_MAXSITE) return fail("myo_batch_ik: nsite must be in [1, " + std::to_string(MYO_IK_MAXSITE) + "]");
   if (!std::isfinite(p->tol) || !std::isfinite(p->damping) || !std::isfinite(p->max_step) || !std::isfinite(p->posture_weight) || !std::isfinite(p->eq_weight))
@@ -1454,10 +1457,8 @@ extern "C" int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_
   CUDA_OK(cudaMemcpyAsync(sid, d->site_id, (size_t)ns*4, cudaMemcpyDeviceToHost, st)); CUDA_OK(cudaStreamSynchronize(st));
   IkArgs a; memset(&a, 0, sizeof(a));
   if (const int rc = ik_sites(b, sid, ns, a)) return rc;
-  if (!b->ik_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
-    if (launch_shape((const void*)myo_ik_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->ik_shape)) return -1;
-    b->ik_ready = true; }
-  a.d = *d; a.p = *p; a.bound_qpos = b->bufs.qpos; a.n_env = b->n_env; const LaunchShape& s = b->ik_shape;
+  if (analysis_shape(b, (const void*)myo_ik_kernel, b->ik_shape)) return -1;
+  a.d = *d; a.p = *p; a.bound_qpos = b->bufs.qpos; a.n_env = b->n_env; const LaunchShape& s = b->ik_shape.s;
   myo_ik_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
@@ -1468,7 +1469,7 @@ extern "C" int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, co
   if (!b || !d || !p) return fail("myo_batch_transition_fd: null");
   if (!d->ctrl) return fail("myo_batch_transition_fd: ctrl is required");
   if (!d->A && !d->B) return fail("myo_batch_transition_fd: at least one of A and B is required");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   if (!std::isfinite(p->eps) || !(p->eps > 0)) return fail("myo_batch_transition_fd: eps must be finite and > 0");
   if (p->substeps < 1) return fail("myo_batch_transition_fd: substeps must be >= 1");
   if (p->centered != 0 && p->centered != 1) return fail("myo_batch_transition_fd: centered must be 0 or 1");
@@ -1491,9 +1492,8 @@ extern "C" int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, co
   myo_buffers c; memset(&c, 0, sizeof(c));      // the start state, read only: no state is stored back in this kernel
   c.qpos = d->qpos0 ? (double*)d->qpos0 : q.qpos; c.qvel = d->qvel0 ? (double*)d->qvel0 : q.qvel; c.act = d->act0 ? (double*)d->act0 : q.act;
   c.qacc_warmstart = d->qacc_warmstart0 ? (double*)d->qacc_warmstart0 : q.qacc_warmstart; c.env_prm = q.env_prm; c.overflow = d->overflow;
-  StepArgs a; memset(&a, 0, sizeof(a)); a.mode = 0; a.b = c; a.roll.ctrl = d->ctrl; a.roll.qfrc_applied = d->qfrc_applied; a.roll_nstep = 1; a.roll_t = 0;
-  a.cfg = b->cfg; a.cfg.task = MYO_TASK_NONE; a.cfg.muscle_condition = MYO_COND_NONE; a.cfg.reaf_dst = a.cfg.reaf_src = 0; a.cfg.auto_reset = 0; a.cfg.frame_skip = p->substeps;
-  a.n_env = (int)items; a.dt = dm.timestep*p->substeps; a.tol = b->tol; a.seed = b->seed; a.env_offset = b->env_offset; a.balanced = 0;
+  StepArgs a = physics_args(b, p->substeps); a.b = c; a.roll.ctrl = d->ctrl; a.roll.qfrc_applied = d->qfrc_applied; a.roll_nstep = 1; a.roll_t = 0;
+  a.n_env = (int)items; a.balanced = 0;
   a.fd.A = d->A; a.fd.B = d->B; a.fd.nom = b->dCarry; a.fd.rows = b->dFdRows; a.fd.eps = p->eps; a.fd.rinv1 = 1.0/p->eps; a.fd.rinv2 = 1.0/(2.0*p->eps);
   a.fd.n_env = b->n_env; a.fd.ncol = ncol; a.fd.nxa = nxa; a.fd.npass = p->centered ? 2 : 1;
   myo_fd_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
@@ -1531,19 +1531,17 @@ extern "C" int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* 
   if (!b || !d || !p) return fail("myo_batch_static_opt: null");
   if (!d->qacc || !d->reserve || !d->act) return fail("myo_batch_static_opt: qacc, reserve and act are required");
   if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_static_opt: unknown flag bits");
-  if (!b->bound) return fail("batch has no bound buffers (call myo_batch_bind)");
+  if (const int rc = require_bound(b)) return rc;
   if (!std::isfinite(p->tol)) return fail("myo_batch_static_opt: non-finite parameter");
   if (p->tol < 0 || p->max_iter < 0) return fail("myo_batch_static_opt: needs tol >= 0 and max_iter >= 0");
   if (b->dm.nv > 64) return fail("myo_batch_static_opt: models with more than 64 dofs are not supported");
   CUDA_OK(cudaSetDevice(b->device));
-  if (!b->so_ready) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
-    if (so_plan(b->dm, b->so_off)) return -1;
-    if (launch_shape((const void*)myo_static_opt_kernel, prop, b->dm.n_per_warp*8, b->const_bytes, b->n_env, false, 0, b->so_shape)) return -1;
-    b->so_ready = true; }
+  if (!b->so_shape.ready && so_plan(b->dm, b->so_off)) return -1;
+  if (analysis_shape(b, (const void*)myo_static_opt_kernel, b->so_shape)) return -1;
   SoArgs a; memset(&a, 0, sizeof(a));
   a.d = *d; a.p = *p; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags;
   a.o_H = b->so_off[0]; a.o_x = b->so_off[1]; a.o_l = b->so_off[2]; a.o_cg = b->so_off[3]; a.o_tf = b->so_off[4]; a.o_s = b->so_off[5]; a.o_gm = b->so_off[6]; a.o_bm = b->so_off[7];
-  const LaunchShape& s = b->so_shape;
+  const LaunchShape& s = b->so_shape.s;
   myo_static_opt_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }

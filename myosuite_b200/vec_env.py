@@ -18,6 +18,46 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _REG = None
 
 
+def _check_f64(name, x, shape, device):
+    """Raise ValueError unless x is a contiguous float64 tensor of `shape` on `device` (the analysis calls' input tensors)."""
+    import torch
+    if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != device or tuple(x.shape) != tuple(shape)
+            or not x.is_contiguous()):
+        raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), device, (
+            type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
+            x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+
+
+def _check_fields(kind, fields, available):
+    """The requested output fields as a tuple; KeyError names those not in `available`."""
+    fields = tuple(fields)
+    bad = [f for f in fields if f not in available]
+    if bad:
+        raise KeyError("unknown %s fields %s (available: %s)" % (kind, bad, list(available)))
+    return fields
+
+
+def _output(device, lead, trailing, size, int32=False):
+    """An output tensor of shape lead + trailing, with the model-size names in `trailing` looked up in `size`, filled with NaN (float64)
+    or -1 (int32) so that an entry the launch does not write stands out."""
+    import torch
+    shape = tuple(lead) + tuple(size[x] if isinstance(x, str) else x for x in trailing)
+    return torch.full(shape, -1, dtype=torch.int32, device=device) if int32 else torch.full(shape, float("nan"), dtype=torch.float64, device=device)
+
+
+def _initial_state(initial_state, width, n, device):
+    """The start-state fields (abi.ROLLOUT_STATE) of an `initial_state` dict: KeyError for a key not in `width` (key -> trailing shape
+    after [n]), ValueError for a tensor that is not a contiguous float64 [n, width] on `device`; a None value is left out."""
+    bufs = {}
+    for k, v in (initial_state or {}).items():
+        if k not in width:
+            raise KeyError("unknown initial_state key %r (available: %s)" % (k, list(width)))
+        if v is not None:
+            _check_f64("initial_state[%r]" % k, v, (n,) + width[k], device)
+            bufs[abi.ROLLOUT_STATE[k]] = v
+    return bufs
+
+
 def registry():
     global _REG
     if _REG is None:
@@ -320,19 +360,13 @@ class MyoVecEnv:
         One launch computes only what the deepest requested group needs (pose < actuation < dynamics; myo_batch_data).  The tensors
         are allocated on first request (NaN / -1 until first written) and reused: a result is valid until the next state change.
         ctrl is the last step's ctrl (zeros before the first step); after an auto-reset the values describe the new episode's state."""
-        torch = self.torch
-        fields = tuple(fields) or self.DATA_FIELDS
-        bad = [f for f in fields if f not in self.DATA_FIELDS]
-        if bad:
-            raise KeyError("unknown mjData fields %s (available: %s)" % (bad, list(self.DATA_FIELDS)))
+        fields = _check_fields("mjData", tuple(fields) or self.DATA_FIELDS, self.DATA_FIELDS)
         m, n = self.mj_model, self.num_envs
         size = dict(nbody=m.nbody, nsite=m.nsite, nu=m.nu, nv=m.nv, maxcon=self.dims.maxcon)
         for f in fields:
             if f not in self._data:
                 _, dt, shape = abi.DATA_SHAPES[f]
-                shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in shape)
-                self._data[f] = (torch.full(shape, float("nan"), dtype=torch.float64, device=self.device) if dt == "f64"
-                                 else torch.full(shape, -1, dtype=torch.int32, device=self.device))
+                self._data[f] = _output(self.device, (n,), shape, size, dt == "i32")
         bufs = {f: self._data[f] for f in fields}
         if "site_xpos" in bufs:
             bufs["site_source"] = self._site_source
@@ -349,10 +383,7 @@ class MyoVecEnv:
         Euler substep (mjENBL_INVDISCRETE).  act, ctrl and the warm start do not enter.  One launch; the tensors are allocated on first
         request and reused, like data()'s.  Not a state change."""
         torch = self.torch
-        fields = tuple(fields)
-        bad = [f for f in fields if f not in self.INVERSE_FIELDS]
-        if bad:
-            raise KeyError("unknown inverse fields %s (available: %s)" % (bad, list(self.INVERSE_FIELDS)))
+        fields = _check_fields("inverse", fields, self.INVERSE_FIELDS)
         m, n = self.mj_model, self.num_envs
         if not isinstance(qacc, torch.Tensor) or qacc.dtype != torch.float64 or qacc.device != self.device or tuple(qacc.shape) != (n, m.nv):
             raise ValueError("qacc must be a float64 tensor of shape (%d, %d) on %s, got %s" % (
@@ -361,8 +392,7 @@ class MyoVecEnv:
         outs = set(fields) | {"qfrc_inverse"}
         for f in outs:
             if f not in self._inv:
-                shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in abi.INVERSE_SHAPES[f])
-                self._inv[f] = torch.full(shape, float("nan"), dtype=torch.float64, device=self.device)
+                self._inv[f] = _output(self.device, (n,), abi.INVERSE_SHAPES[f], size)
         flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
         self.batch.inverse(stream=self._stream(), flags=flags, qacc=qacc.contiguous(), **{f: self._inv[f] for f in outs})
         return {f: self._inv[f] for f in fields}
@@ -382,43 +412,23 @@ class MyoVecEnv:
         dropped contacts.  The tensors are allocated per call.  Per-env overrides (env_prm) apply; the task layer, counters and auto-reset
         do not run, and the env's own state and episode are left as they were: not a state change.  One launch per interval."""
         torch = self.torch
-        fields = tuple(fields)
-        bad = [f for f in fields if f not in self.ROLLOUT_FIELDS]
-        if bad:
-            raise KeyError("unknown rollout fields %s (available: %s)" % (bad, list(self.ROLLOUT_FIELDS)))
+        fields = _check_fields("rollout", fields, self.ROLLOUT_FIELDS)
         m, n = self.mj_model, self.num_envs
         substeps = int(substeps)
         if substeps < 1:
             raise ValueError("substeps must be >= 1, got %d" % substeps)
-
-        def check(name, x, shape):
-            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
-                    or not x.is_contiguous()):
-                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
-                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
-                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
         nstep = int(ctrl.shape[1]) if isinstance(ctrl, torch.Tensor) and ctrl.dim() == 3 else 0
         if nstep < 1:
             raise ValueError("ctrl must be a float64 tensor [num_envs, nstep >= 1, nu], got %s" % (tuple(getattr(ctrl, "shape", ())),))
-        check("ctrl", ctrl, (n, nstep, m.nu))
+        _check_f64("ctrl", ctrl, (n, nstep, m.nu), self.device)
         bufs = {"ctrl": ctrl}
         if qfrc_applied is not None:
-            check("qfrc_applied", qfrc_applied, (n, nstep, m.nv))
+            _check_f64("qfrc_applied", qfrc_applied, (n, nstep, m.nv), self.device)
             bufs["qfrc_applied"] = qfrc_applied
-        width = dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=())
-        for k, v in (initial_state or {}).items():
-            if k not in abi.ROLLOUT_STATE:
-                raise KeyError("unknown initial_state key %r (available: %s)" % (k, list(abi.ROLLOUT_STATE)))
-            if v is not None:
-                check("initial_state[%r]" % k, v, (n,) + width[k])
-                bufs[abi.ROLLOUT_STATE[k]] = v
+        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=()), n, self.device))
         size = dict(nq=m.nq, nv=m.nv, na=m.na)
-        out = {}
-        for f in fields:
-            if f == "overflow":
-                out[f] = torch.zeros(n, dtype=torch.int32, device=self.device)
-            else:
-                out[f] = torch.full((n, nstep) + tuple(size[x] for x in abi.ROLLOUT_SHAPES[f]), float("nan"), dtype=torch.float64, device=self.device)
+        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow" else _output(self.device, (n, nstep), abi.ROLLOUT_SHAPES[f], size)
+               for f in fields}
         self.batch.rollout(nstep, substeps, stream=self._stream(), **bufs, **out)
         return out
 
@@ -440,27 +450,17 @@ class MyoVecEnv:
         jacp / jacr [ns, 3, nv], all at the returned qpos; allocated per call.  One launch; not a state change (adopt a solution with
         set_state(qpos=...)).  A trajectory of T frames is one call on a batch of T envs."""
         torch, m, n = self.torch, self.mj_model, self.num_envs
-        fields = tuple(fields)
-        bad = [f for f in fields if f not in self.IK_FIELDS]
-        if bad:
-            raise KeyError("unknown ik fields %s (available: %s)" % (bad, list(self.IK_FIELDS)))
+        fields = _check_fields("ik", fields, self.IK_FIELDS)
         sid = [m.name2id("site", x) if isinstance(x, str) else int(x) for x in ([sites] if isinstance(sites, (str, int)) else sites)]
         ns = len(sid)
         if not 1 <= ns <= abi.IK_MAXSITE or any(not 0 <= x < m.nsite for x in sid):
             raise ValueError("sites must be 1..%d site names or ids in [0, %d), got %s" % (abi.IK_MAXSITE, m.nsite, sites))
-
-        def check(name, x, shape):
-            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
-                    or not x.is_contiguous()):
-                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
-                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
-                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
-        check("target_pos", target_pos, (n, ns, 3))
+        _check_f64("target_pos", target_pos, (n, ns, 3), self.device)
         bufs = {"target_pos": target_pos}
         for name, x, shape in (("target_quat", target_quat, (n, ns, 4)), ("qpos0", qpos_init, (n, m.nq)), ("qpos_ref", qpos_ref, (n, m.nq)),
                                ("site_weight", site_weight, (ns, 2))):
             if x is not None:
-                check("qpos_init" if name == "qpos0" else name, x, shape)
+                _check_f64("qpos_init" if name == "qpos0" else name, x, shape, self.device)
                 bufs[name] = x
         if dofs is not None:
             if isinstance(dofs, torch.Tensor) or isinstance(dofs, np.ndarray):
@@ -481,11 +481,7 @@ class MyoVecEnv:
         bufs["site_id"] = torch.as_tensor(np.asarray(sid, np.int32), device=self.device)
         bufs["site_quat"] = torch.as_tensor(np.ascontiguousarray(m.site_quat[sid], dtype=np.float64), device=self.device)
         size = dict(nq=m.nq, nv=m.nv, ns=ns)
-        out = {}
-        for f in set(fields) | {"qpos"}:
-            shape = (n,) + tuple(size[x] if isinstance(x, str) else x for x in abi.IK_SHAPES[f])
-            out[f] = (torch.full(shape, -1, dtype=torch.int32, device=self.device) if f in ("niter", "converged")
-                      else torch.full(shape, float("nan"), dtype=torch.float64, device=self.device))
+        out = {f: _output(self.device, (n,), abi.IK_SHAPES[f], size, f in ("niter", "converged")) for f in set(fields) | {"qpos"}}
         self.batch.ik(params, stream=self._stream(), **bufs, **out)
         return {f: out[f] for f in fields}
 
@@ -516,10 +512,7 @@ class MyoVecEnv:
         iterative solver each column carries solver noise of order solver_tolerance / eps, as in MuJoCo; MyoVecEnv(...,
         solver_tolerance=...) tightens it.  Two launches (the nominal interval, then one warp per (env, column))."""
         torch = self.torch
-        fields = tuple(fields)
-        bad = [f for f in fields if f not in self.FD_FIELDS]
-        if bad:
-            raise KeyError("unknown transition_fd fields %s (available: %s)" % (bad, list(self.FD_FIELDS)))
+        fields = _check_fields("transition_fd", fields, self.FD_FIELDS)
         if "A" not in fields and "B" not in fields:
             raise ValueError("transition_fd needs at least one of the fields A and B")
         m, n = self.mj_model, self.num_envs
@@ -530,31 +523,15 @@ class MyoVecEnv:
             raise ValueError("eps must be finite and > 0, got %r" % eps)
         if centered not in (0, 1, False, True):
             raise ValueError("centered must be a bool, got %r" % (centered,))
-
-        def check(name, x, shape):
-            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
-                    or not x.is_contiguous()):
-                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
-                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
-                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
-        check("ctrl", ctrl, (n, m.nu))
+        _check_f64("ctrl", ctrl, (n, m.nu), self.device)
         bufs = {"ctrl": ctrl}
         if qfrc_applied is not None:
-            check("qfrc_applied", qfrc_applied, (n, m.nv))
+            _check_f64("qfrc_applied", qfrc_applied, (n, m.nv), self.device)
             bufs["qfrc_applied"] = qfrc_applied
-        width = dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,))
-        for k, v in (initial_state or {}).items():
-            if k not in width:
-                raise KeyError("unknown initial_state key %r (available: %s)" % (k, list(width)))
-            if v is not None:
-                check("initial_state[%r]" % k, v, (n,) + width[k])
-                bufs[abi.ROLLOUT_STATE[k]] = v
-        nx = 2 * m.nv + m.na
-        shape = dict(A=(n, nx, nx), B=(n, nx, m.nu))
-        out = {}
-        for f in fields:
-            out[f] = (torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow"
-                      else torch.full(shape[f], float("nan"), dtype=torch.float64, device=self.device))
+        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,)), n, self.device))
+        size, trailing = dict(nx=2 * m.nv + m.na, nu=m.nu), dict(A=("nx", "nx"), B=("nx", "nu"))
+        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow" else _output(self.device, (n,), trailing[f], size)
+               for f in fields}
         params = abi.MyoFdParams(eps=eps, centered=int(bool(centered)), substeps=substeps)
         self.batch.transition_fd(params, stream=self._stream(), **bufs, **out)
         return out
@@ -575,21 +552,11 @@ class MyoVecEnv:
         converged (int32) and residual (|G a + r - t|_inf, converged when <= tol max(1, |t|_inf)); allocated per call.  One launch; not a
         state change."""
         torch, m, n = self.torch, self.mj_model, self.num_envs
-        fields = tuple(fields)
-        bad = [f for f in fields if f not in self.STATIC_OPT_FIELDS]
-        if bad:
-            raise KeyError("unknown static_opt fields %s (available: %s)" % (bad, list(self.STATIC_OPT_FIELDS)))
-
-        def check(name, x, shape):
-            if (not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.device != self.device or tuple(x.shape) != tuple(shape)
-                    or not x.is_contiguous()):
-                raise ValueError("%s must be a contiguous float64 tensor of shape %s on %s, got %s" % (name, tuple(shape), self.device, (
-                    type(x).__name__, getattr(x, "dtype", None), getattr(x, "device", None), tuple(getattr(x, "shape", ())),
-                    x.is_contiguous() if isinstance(x, torch.Tensor) else None)))
+        fields = _check_fields("static_opt", fields, self.STATIC_OPT_FIELDS)
 
         def positive(name, x, width):
             if isinstance(x, torch.Tensor):
-                check(name, x, (width,))
+                _check_f64(name, x, (width,), self.device)
             else:
                 v = np.asarray(x, dtype=np.float64)
                 if v.shape not in ((), (width,)):
@@ -598,22 +565,18 @@ class MyoVecEnv:
             if not bool(torch.all(torch.isfinite(x) & (x > 0))):
                 raise ValueError("%s must be finite and > 0" % name)
             return x
-        check("qacc", qacc, (n, m.nv))
+        _check_f64("qacc", qacc, (n, m.nv), self.device)
         bufs = {"qacc": qacc, "reserve": positive("reserve", reserve, m.nv)}
         if weight is not None:
             bufs["weight"] = positive("weight", weight, m.nu)
         if warmstart is not None:
-            check("warmstart", warmstart, (n, m.nv))
+            _check_f64("warmstart", warmstart, (n, m.nv), self.device)
             bufs["lambda0"] = warmstart
         params = abi.MyoStaticOptParams(max_iter=int(max_iter), tol=float(tol))
         if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
             raise ValueError("static_opt needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (max_iter, tol))
         size = dict(nu=m.nu, nv=m.nv)
-        out = {}
-        for f in set(fields) | {"act"}:
-            shape = (n,) + tuple(size[x] for x in abi.STATIC_OPT_SHAPES[f])
-            out[f] = (torch.full(shape, -1, dtype=torch.int32, device=self.device) if f in ("niter", "converged")
-                      else torch.full(shape, float("nan"), dtype=torch.float64, device=self.device))
+        out = {f: _output(self.device, (n,), abi.STATIC_OPT_SHAPES[f], size, f in ("niter", "converged")) for f in set(fields) | {"act"}}
         flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
         self.batch.static_opt(params, stream=self._stream(), flags=flags, **bufs, **out)
         return {f: out[f] for f in fields}

@@ -30,34 +30,49 @@ def build_native():
         return build()
 
 
+def _declare(L):
+    """The prototypes of the oracle's own oracle_* functions on library L."""
+    L.oracle_create.restype = ctypes.c_void_p
+    L.oracle_create.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+    L.oracle_field.restype = ctypes.POINTER(ctypes.c_double)
+    L.oracle_field.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
+    L.oracle_ifield.restype = ctypes.POINTER(ctypes.c_int)
+    L.oracle_ifield.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
+    for f in ("oracle_forward", "oracle_step", "oracle_reset", "oracle_destroy"):
+        getattr(L, f).argtypes = [ctypes.c_void_p]
+        getattr(L, f).restype = None
+    L.oracle_step_n.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    L.oracle_step_n.restype = None
+    L.oracle_info.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    L.oracle_info.restype = ctypes.c_int
+    return L
+
+
 def lib():
     global _LIB
     if _LIB is None:
-        L = ctypes.CDLL(os.environ.get("MYO_ORACLE_LIB") or build())
-        L.oracle_create.restype = ctypes.c_void_p
-        L.oracle_create.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        L.oracle_field.restype = ctypes.POINTER(ctypes.c_double)
-        L.oracle_field.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
-        L.oracle_ifield.restype = ctypes.POINTER(ctypes.c_int)
-        L.oracle_ifield.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
-        for f in ("oracle_forward", "oracle_step", "oracle_reset", "oracle_destroy"):
-            getattr(L, f).argtypes = [ctypes.c_void_p]
-            getattr(L, f).restype = None
-        L.oracle_step_n.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.oracle_step_n.restype = None
-        L.oracle_info.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.oracle_info.restype = ctypes.c_int
-        _LIB = L
+        _LIB = _declare(ctypes.CDLL(os.environ.get("MYO_ORACLE_LIB") or build()))
     return _LIB
 
 
-class Oracle:
-    """One env of the CPU oracle.  `I`, `D` are the packed model blob (myosuite_b200.blob.pack)."""
+def build_extension(source):
+    """Compile `source`, a C file that includes the oracle's source and adds oracle_* functions of its own, with the flags of
+    oracle/Makefile (less its warnings) into a fresh temporary directory (the source tree may be read-only).  Returns the CDLL with
+    the oracle's prototypes declared; the caller declares its own."""
+    name = os.path.splitext(os.path.basename(source))[0]
+    so = os.path.join(tempfile.mkdtemp(prefix="myo_%s_" % name), "libmyo_%s.so" % name)
+    subprocess.check_call(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-shared", "-o", so, source, "-lm"])
+    return _declare(ctypes.CDLL(so))
 
-    def __init__(self, I, D):
+
+class Oracle:
+    """One env of the CPU oracle.  `I`, `D` are the packed model blob (myosuite_b200.blob.pack); `L` is the library that runs it (None:
+    the oracle's own, lib(); an extension's from build_extension)."""
+
+    def __init__(self, I, D, L=None):
         self._I = np.ascontiguousarray(I, dtype=np.int32)
         self._D = np.ascontiguousarray(D, dtype=np.float64)
-        self._L = lib()
+        self._L = L or lib()
         self._h = self._L.oracle_create(self._I.ctypes.data, self._D.ctypes.data)
         if not self._h:
             raise RuntimeError("oracle_create failed (blob magic/version)")

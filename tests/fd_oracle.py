@@ -1,49 +1,30 @@
 """MuJoCo's mjd_transitionFD on the CPU oracle (tests/fd_oracle.c): the rollout oracle's source plus integratePos, differentiatePos and
 oracle_transition_fd, compiled once per process into a temporary directory (the source tree may be read-only)."""
 import ctypes
+import functools
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+from oracle.oracle_py import build_extension
 from rollout_oracle import AppliedOracle
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
 
 
+@functools.cache
 def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="myo_fd_oracle_"), "libmyo_fd_oracle.so")
-        # the flags of oracle/Makefile
-        subprocess.check_call(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-shared", "-o", so, os.path.join(_HERE, "fd_oracle.c"), "-lm"])
-        L = ctypes.CDLL(so)
-        vp, i, d = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
-        L.oracle_create.restype = vp
-        L.oracle_create.argtypes = [vp, vp]
-        L.oracle_field.restype = ctypes.POINTER(d)
-        L.oracle_field.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(i)]
-        L.oracle_ifield.restype = ctypes.POINTER(ctypes.c_int)
-        L.oracle_ifield.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(i)]
-        for f in ("oracle_forward", "oracle_step", "oracle_reset", "oracle_destroy"):
-            getattr(L, f).argtypes = [vp]
-            getattr(L, f).restype = None
-        L.oracle_step_n.argtypes = [vp, i]
-        L.oracle_step_n.restype = None
-        L.oracle_info.argtypes = [vp, i]
-        L.oracle_info.restype = i
-        for f in ("oracle_forward_applied", "oracle_step_applied"):
-            getattr(L, f).argtypes = [vp, vp]
-            getattr(L, f).restype = None
-        L.oracle_integrate_pos.argtypes = [vp, vp, vp, d]
-        L.oracle_differentiate_pos.argtypes = [vp, vp, d, vp, vp]
-        L.oracle_transition_fd.argtypes = [vp, vp, vp, d, i, i, vp, vp]
-        for f in ("oracle_integrate_pos", "oracle_differentiate_pos", "oracle_transition_fd"):
-            getattr(L, f).restype = None
-        _LIB = L
-    return _LIB
+    L = build_extension(os.path.join(_HERE, "fd_oracle.c"))
+    vp, i, d = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
+    for f in ("oracle_forward_applied", "oracle_step_applied"):
+        getattr(L, f).argtypes = [vp, vp]
+        getattr(L, f).restype = None
+    L.oracle_integrate_pos.argtypes = [vp, vp, vp, d]
+    L.oracle_differentiate_pos.argtypes = [vp, vp, d, vp, vp]
+    L.oracle_transition_fd.argtypes = [vp, vp, vp, d, i, i, vp, vp]
+    for f in ("oracle_integrate_pos", "oracle_differentiate_pos", "oracle_transition_fd"):
+        getattr(L, f).restype = None
+    return L
 
 
 def _arr(x, n):
@@ -57,13 +38,7 @@ class FdOracle(AppliedOracle):
     mj_differentiatePos.  The state set on it is the start; transition_fd leaves it as it was."""
 
     def __init__(self, I, D):
-        self._I = np.ascontiguousarray(I, dtype=np.int32)
-        self._D = np.ascontiguousarray(D, dtype=np.float64)
-        self._L = lib()
-        self._h = self._L.oracle_create(self._I.ctypes.data, self._D.ctypes.data)
-        if not self._h:
-            raise RuntimeError("oracle_create failed (blob magic/version)")
-        self._applied = np.zeros(len(super(AppliedOracle, self).f("qvel")))
+        super().__init__(I, D, lib())
 
     def integrate_pos(self, qpos, v, scale):
         q = _arr(qpos, len(self.f("qpos"))).copy()

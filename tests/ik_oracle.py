@@ -1,47 +1,27 @@
 """mj_jacSite and inverse kinematics on the CPU oracle (tests/ik_oracle.c): the oracle library's source plus oracle_jac_site and oracle_ik,
 compiled once per process into a temporary directory (the source tree may be read-only)."""
 import ctypes
+import functools
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-from oracle.oracle_py import Oracle
+from oracle.oracle_py import Oracle, build_extension
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
 # the defaults of MyoVecEnv.ik (myosuite_b200/vec_env.py: MyoVecEnv.IK_DEFAULTS)
 DEFAULTS = dict(max_iter=200, tol=1e-6, damping=1e-3, max_step=0.5, posture=0.0, eq_weight=1.0)
 
 
+@functools.cache
 def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="myo_ik_oracle_"), "libmyo_ik_oracle.so")
-        # the flags of oracle/Makefile
-        subprocess.check_call(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-shared", "-o", so, os.path.join(_HERE, "ik_oracle.c"), "-lm"])
-        L = ctypes.CDLL(so)
-        L.oracle_create.restype = ctypes.c_void_p
-        L.oracle_create.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        L.oracle_field.restype = ctypes.POINTER(ctypes.c_double)
-        L.oracle_field.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
-        L.oracle_ifield.restype = ctypes.POINTER(ctypes.c_int)
-        L.oracle_ifield.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
-        for f in ("oracle_forward", "oracle_step", "oracle_reset", "oracle_destroy"):
-            getattr(L, f).argtypes = [ctypes.c_void_p]
-            getattr(L, f).restype = None
-        L.oracle_step_n.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.oracle_step_n.restype = None
-        L.oracle_info.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.oracle_info.restype = ctypes.c_int
-        L.oracle_jac_site.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
-        L.oracle_jac_site.restype = None
-        L.oracle_ik.argtypes = ([ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 7 + [ctypes.c_int] + [ctypes.c_double] * 5
-                                + [ctypes.c_void_p] * 7)
-        L.oracle_ik.restype = None
-        _LIB = L
-    return _LIB
+    L = build_extension(os.path.join(_HERE, "ik_oracle.c"))
+    L.oracle_jac_site.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 5
+    L.oracle_jac_site.restype = None
+    L.oracle_ik.argtypes = ([ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 7 + [ctypes.c_int] + [ctypes.c_double] * 5
+                            + [ctypes.c_void_p] * 7)
+    L.oracle_ik.restype = None
+    return L
 
 
 def _ptr(a):
@@ -52,12 +32,7 @@ class IkOracle(Oracle):
     """The oracle with mj_jacSite and oracle_ik.  `site_quat` is the model's mjModel.site_quat (the blob carries no site frames)."""
 
     def __init__(self, I, D, site_quat):
-        self._I = np.ascontiguousarray(I, dtype=np.int32)
-        self._D = np.ascontiguousarray(D, dtype=np.float64)
-        self._L = lib()
-        self._h = self._L.oracle_create(self._I.ctypes.data, self._D.ctypes.data)
-        if not self._h:
-            raise RuntimeError("oracle_create failed (blob magic/version)")
+        super().__init__(I, D, lib())
         self.site_quat = np.ascontiguousarray(site_quat, dtype=np.float64)
         self.nv = len(self.f("qvel"))
 
