@@ -283,6 +283,51 @@ typedef struct {
 } myo_static_opt_buffers;
 typedef struct { int32_t max_iter; double tol; } myo_static_opt_params;
 
+/* Caller-owned device buffers of myo_batch_cmc: computed muscle control (OpenSim's CMC, MyoSuite tutorial 9) of every env along its own
+ * reference motion, T = nstep frames.  From the start state s_0 (qpos0 ... time0, or the bound buffer of the same name, as
+ * myo_rollout_buffers takes it) each frame t = 0 .. T-1 runs
+ *   1. qacc_des_t = ref_qacc[t] + kv (ref_qvel[t] - qvel_t) + kp dq,  dq = mj_differentiatePos(qpos_t, ref_qpos[t]) (dt = 1: the tangent
+ *      space, so free and ball joints are handled), products elementwise over the dofs;
+ *   2. myo_batch_static_opt's problem at s_t for qacc_des_t with the call's flags, weight, reserve, max_iter and tol, warm-started from
+ *      lambda_{t-1} (lambda_{-1} = lambda0, or 0): a*_t, r_t = reserve_force, lambda_t;
+ *   3. the excitation u_t that, held for `substeps` mj_steps of the muscle activation dynamics from act_t, brings act to a*_t at the end of
+ *      the interval, clipped to ctrlrange intersected with [0, 1] (myo_static_opt_buffers.ctrl at substeps = 1; bisection over the k-step
+ *      map otherwise, on the monotonicity in ctrl that the one-step bisection assumes);
+ *   4. one myo_batch_rollout interval of `substeps` mj_steps from s_t with ctrl u_t and qfrc_applied r_t, which gives s_{t+1}.
+ * Steps 2 and 4 are myo_batch_static_opt and myo_batch_rollout themselves: row t of the outputs is bit-identical to those calls run from
+ * row t-1's state (s_0 for t = 0).  Row t holds the frame's solve and the state after its interval (myo_rollout_buffers' meaning).
+ * Every output is nullable; only the non-null ones are written. */
+typedef struct {
+  const double* ref_qpos;      /* [n, nstep, nq] in, required: reference positions */
+  const double* ref_qvel;      /* [n, nstep, nv] in, required */
+  const double* ref_qacc;      /* [n, nstep, nv] in, required */
+  const double* kp;            /* [nv] in, required: position gains (>= 0; not checked on the device) */
+  const double* kv;            /* [nv] in, required: velocity gains (>= 0) */
+  const double* weight;        /* [nu] nullable (1): w > 0, as myo_static_opt_buffers.weight */
+  const double* reserve;       /* [nv] in, required: rho > 0 */
+  const double* lambda0;       /* [n, nv] nullable (0): warm start of frame 0's dual */
+  const double* qpos0;         /* [n, nq] start state, nullable field by field (bound buffers), as myo_rollout_buffers */
+  const double* qvel0;         /* [n, nv] */
+  const double* act0;          /* [n, na] */
+  const double* qacc_warmstart0; /* [n, nv] */
+  const double* time0;         /* [n] */
+  double* qacc_des;            /* [n, nstep, nv] out */
+  double* ctrl;                /* [n, nstep, nu] out: u_t */
+  double* act_opt;             /* [n, nstep, nu] out: a*_t */
+  double* reserve_force;       /* [n, nstep, nv] out: r_t */
+  double* lambda;              /* [n, nstep, nv] out: lambda_t */
+  int32_t* niter;              /* [n, nstep] out */
+  int32_t* converged;          /* [n, nstep] out */
+  double* residual;            /* [n, nstep] out */
+  double* qpos;                /* [n, nstep, nq] out: s_{t+1} */
+  double* qvel;                /* [n, nstep, nv] out */
+  double* act;                 /* [n, nstep, na] out */
+  double* qacc;                /* [n, nstep, nv] out: mjData.qacc, the next interval's warm start */
+  double* time;                /* [n, nstep] out */
+  int32_t* overflow;           /* [n] out: myo_rollout_buffers.overflow's meaning over every interval */
+} myo_cmc_buffers;
+typedef struct { int32_t max_iter, substeps; double tol; } myo_cmc_params;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -381,6 +426,17 @@ int myo_batch_transition_fd(myo_batch* b, const myo_fd_buffers* d, const myo_fd_
  * weight and reserve.  Replaces the per-frame SLSQP / OSQP solves of MyoSuite
  * tutorials 6_Inverse_Dynamics (get_ctrl) and 9_Computed_muscle_control. */
 int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* d, const myo_static_opt_params* p, int flags, void* stream);
+
+/* Computed muscle control of every env over nstep frames (myo_cmc_buffers, myo_cmc_params), all on `stream` with no host synchronisation;
+ * flags: MYO_INV_* as myo_batch_static_opt's.  Launches per call: nstep (3 + (substeps > 1) + R) + 1, where R = 1 when the batch's
+ * rollouts run on the load-sorted map (a regroup launch before each interval) and 0 otherwise: per frame the qacc_des stage (which also
+ * stores the previous frame's row), myo_static_opt_kernel, the k-step excitation when substeps > 1, and the rollout interval; then one
+ * stage launch that stores the last row.  No bound buffer is written and the env's episode is left alone, as with myo_batch_rollout.  The
+ * per-frame scratch is allocated by the first call.  Fails before any launch on a null batch, buffers or params, a null ref_qpos,
+ * ref_qvel, ref_qacc, kp, kv or reserve, an unbound batch, unknown flag bits, nstep < 1, substeps < 1, tol < 0, max_iter < 0, a
+ * non-finite tol, a model with more than 64 dofs, or a per-env slice without room for the dual Newton's arrays.  Replaces the per-frame
+ * loop of MyoSuite tutorials 6_Inverse_Dynamics and 9_Computed_muscle_control. */
+int myo_batch_cmc(myo_batch* b, const myo_cmc_buffers* d, const myo_cmc_params* p, int nstep, int flags, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

@@ -127,11 +127,28 @@ class MyoStaticOptParams(ctypes.Structure):
     _fields_ = [("max_iter", c_i32), ("tol", c_f64)]
 
 
+# myo_cmc_buffers / myo_cmc_params (include/myo_b200.h): computed muscle control of myo_batch_cmc.  Inputs, start state, then the outputs
+# -> trailing shape after [n, nstep] in the model's sizes (niter and converged int32; overflow is [n], int32)
+CMC_FIELDS = ["ref_qpos", "ref_qvel", "ref_qacc", "kp", "kv", "weight", "reserve", "lambda0", "qpos0", "qvel0", "act0", "qacc_warmstart0", "time0",
+              "qacc_des", "ctrl", "act_opt", "reserve_force", "lambda", "niter", "converged", "residual", "qpos", "qvel", "act", "qacc", "time",
+              "overflow"]
+CMC_SHAPES = {"qacc_des": ("nv",), "ctrl": ("nu",), "act_opt": ("nu",), "reserve_force": ("nv",), "lambda": ("nv",), "niter": (), "converged": (),
+              "residual": (), "qpos": ("nq",), "qvel": ("nv",), "act": ("na",), "qacc": ("nv",), "time": ()}
+
+
+class MyoCmcBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in CMC_FIELDS]
+
+
+class MyoCmcParams(ctypes.Structure):
+    _fields_ = [("max_iter", c_i32), ("substeps", c_i32), ("tol", c_f64)]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
            "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout",
-           "myo_batch_ik", "myo_batch_transition_fd", "myo_batch_static_opt"]
+           "myo_batch_ik", "myo_batch_transition_fd", "myo_batch_static_opt", "myo_batch_cmc"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -194,6 +211,7 @@ def _bind(L):
     L.myo_batch_ik.argtypes = [c_vp, ctypes.POINTER(MyoIkBuffers), ctypes.POINTER(MyoIkParams), c_vp]
     L.myo_batch_transition_fd.argtypes = [c_vp, ctypes.POINTER(MyoFdBuffers), ctypes.POINTER(MyoFdParams), c_vp]
     L.myo_batch_static_opt.argtypes = [c_vp, ctypes.POINTER(MyoStaticOptBuffers), ctypes.POINTER(MyoStaticOptParams), ctypes.c_int, c_vp]
+    L.myo_batch_cmc.argtypes = [c_vp, ctypes.POINTER(MyoCmcBuffers), ctypes.POINTER(MyoCmcParams), ctypes.c_int, ctypes.c_int, c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -332,6 +350,12 @@ class Batch:
         and act are required), a MyoStaticOptParams and MYO_INV_* flags."""
         d = _buffers(MyoStaticOptBuffers, tensors)
         _check(self.L.myo_batch_static_opt(self.handle, ctypes.byref(d), ctypes.byref(params), flags, stream), self.L)
+
+    def cmc(self, params, nstep, stream=None, flags=0, **tensors):
+        """Computed muscle control (myo_batch_cmc) over nstep frames with the given torch CUDA tensors (names of CMC_FIELDS: ref_qpos,
+        ref_qvel, ref_qacc, kp, kv and reserve are required), a MyoCmcParams and MYO_INV_* flags."""
+        d = _buffers(MyoCmcBuffers, tensors)
+        _check(self.L.myo_batch_cmc(self.handle, ctypes.byref(d), ctypes.byref(params), nstep, flags, stream), self.L)
 
     @property
     def launches(self):

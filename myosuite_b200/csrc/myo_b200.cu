@@ -1021,7 +1021,7 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   bool big; double* dCarry; LazyShape roll_shape; bool roll_regroup, roll_balanced;
   // transition FD (myo_batch_transition_fd): launch shape of myo_fd_kernel for fd_items work items, and its per-slot rows
   LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes;
-  LazyShape so_shape; int so_off[8]; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt
+  LazyShape so_shape; int so_off[8]; LazyShape cmc_shape; double* dCmc; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt or myo_batch_cmc; myo_cmc_kernel's launch shape and the per-frame rows (cmc_rows), set by the first myo_batch_cmc
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1180,7 +1180,7 @@ static void data_release(myo_batch* b) {
   cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
   memset(&b->data, 0, sizeof(b->data)); b->data_shape = LazyShape(); }
 extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
-  cudaFree(b->dCarry); cudaFree(b->dFdRows); data_release(b); delete b; }
+  cudaFree(b->dCarry); cudaFree(b->dFdRows); cudaFree(b->dCmc); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
 // Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 9) written):
@@ -1377,12 +1377,12 @@ extern "C" int myo_batch_rollout(myo_batch* b, const myo_rollout_buffers* r, int
   return roll_run(b, r, nstep, substeps, stream);
 }
 
-// The launches of a checked rollout, on the current device: the carry from the start state, then one launch per interval
-static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
+// The carry of a checked rollout, on the current device: the start state from the caller's rows (r's *0 fields) or the bound buffers, and
+// r->overflow cleared; no launch
+static int roll_carry(myo_batch* b, const myo_rollout_buffers* r, cudaStream_t st, myo_buffers& c) {
   if (!b->roll_shape.ready) { if (const int rc = roll_setup(b)) { cudaFree(b->dCarry); b->dCarry = nullptr; return rc; } }
-  const DevModel& d = b->dm; const size_t n = b->n_env; cudaStream_t st = (cudaStream_t)stream;
-  // the carry: the start state, from the caller's rows or the bound buffers
-  myo_buffers c; memset(&c, 0, sizeof(c));
+  const DevModel& d = b->dm; const size_t n = b->n_env;
+  memset(&c, 0, sizeof(c));
   c.qpos = b->dCarry; c.qvel = c.qpos + n*d.nq; c.act = c.qvel + n*d.nv; c.qacc_warmstart = c.act + n*d.na; c.time = c.qacc_warmstart + n*d.nv;
   const myo_buffers& q = b->bufs;
   const struct { double* dst; const double* src; int width; } init[5] = {{c.qpos, r->qpos0 ? r->qpos0 : q.qpos, d.nq}, {c.qvel, r->qvel0 ? r->qvel0 : q.qvel, d.nv},
@@ -1393,15 +1393,30 @@ static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int s
     else CUDA_OK(cudaMemsetAsync(f.dst, 0, n*f.width*8, st)); }      // (an unbound time buffer: the rollout starts at 0)
   if (r->overflow) CUDA_OK(cudaMemsetAsync(r->overflow, 0, n*4, st));
   c.env_prm = q.env_prm; c.overflow = r->overflow;
+  return 0;
+}
+// The StepArgs of the intervals of r (rows [n, nstep]) over the carry c, on the rollout's slot map
+static StepArgs roll_args(const myo_batch* b, const myo_buffers& c, const myo_rollout_buffers* r, int nstep, int substeps) {
   StepArgs a = physics_args(b, substeps); a.b = c; a.roll = *r; a.roll_nstep = nstep; a.n_env = b->n_env; a.balanced = b->roll_balanced;
-  const LaunchShape& s = b->roll_shape.s;
   if (b->roll_regroup) { a.load = b->dLoad; a.perm = b->dPerm; a.perm_rounds = b->perm_rounds; a.load_wn = LOAD_WN; a.load_wi = LOAD_WI; }
+  return a;
+}
+// Interval a.roll_t: the regroup launch when the rollouts run on the load-sorted map, then the rollout kernel
+static int roll_interval(myo_batch* b, const StepArgs& a, cudaStream_t st) {
+  const LaunchShape& s = b->roll_shape.s;
+  if (b->roll_regroup) { myo_regroup_kernel<<<1, 1024, 0, st>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots); b->launches++; }
+  if (b->use_w14) myo_roll_kernel_w14<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+  else myo_roll_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+// The launches of a checked rollout, on the current device: the carry from the start state, then one launch per interval
+static int roll_run(myo_batch* b, const myo_rollout_buffers* r, int nstep, int substeps, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream; myo_buffers c;
+  if (const int rc = roll_carry(b, r, st, c)) return rc;
+  StepArgs a = roll_args(b, c, r, nstep, substeps);
   for (int t = 0; t < nstep; t++) {
     a.roll_t = t;
-    if (b->roll_regroup) { myo_regroup_kernel<<<1, 1024, 0, st>>>(b->dLoad, b->dPerm, b->n_env, s.grid, s.warps, b->perm_slots); b->launches++; }
-    if (b->use_w14) myo_roll_kernel_w14<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
-    else myo_roll_kernel<<<s.grid, s.warps*32, s.smem, st>>>(b->dm, a);
-    CUDA_OK(cudaGetLastError()); b->launches++; }
+    if (const int rc = roll_interval(b, a, st)) return rc; }
   return 0;
 }
 
@@ -1544,4 +1559,116 @@ extern "C" int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* 
   const LaunchShape& s = b->so_shape.s;
   myo_static_opt_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+// ------------------------------------------------------------------ computed muscle control (myo_batch_cmc)
+// Each frame is the unchanged myo_static_opt_kernel and rollout interval launches, with this kernel around them (include/myo_b200.h states
+// the loop).  One env per warp on the balanced map.  Stage 0 of frame t (t = 0 .. nstep): row t - 1 of the caller's outputs, the frame's
+// solve from the per-frame rows and the state after its interval from the rollout carry (which holds s_t); then, for t < nstep, qacc_des_t
+// from the carry and the reference rows, into the per-frame row the static optimisation reads.  Stage 1 (substeps > 1): the excitation
+// over the interval, from the carry's act and a*, in place of the static optimisation's one-step ctrl (which it then does not write).
+// Per-frame rows, [n, width] each (cmc_rows): qacc_des, a*, ctrl, reserve force, lambda of even and of odd frames, residual, niter | converged.
+struct CmcArgs { myo_cmc_buffers d; myo_buffers c; int n_env, nstep, t, stage, substeps;
+  double *qdes, *act, *ctrl, *rf, *lam, *res; int32_t *niter, *conv; };      // lam: the rows frame t - 1 wrote
+
+// act after k mj_steps of the activation dynamics with ctrl c held (c already inside ctrlrange)
+__device__ __forceinline__ double cmc_act_after(const double* dyn, double c, double act, double h, int k) {
+  for (int j = 0; j < k; j++) act = so_act_next(dyn, c, act, h);
+  return act; }
+
+// the excitation that, held for k steps, takes act to a, inside [lo, hi]: so_excitation's bisection over the k-step map
+__device__ __forceinline__ double cmc_excitation(const double* dyn, double act, double a, double h, int k, double lo, double hi) {
+  if (cmc_act_after(dyn, hi, act, h, k) <= a) return hi;
+  if (cmc_act_after(dyn, lo, act, h, k) >= a) return lo;
+  for (int it = 0; it < 200; it++) { const double mid = 0.5*(lo + hi); if (!(mid > lo && mid < hi)) break;
+    if (cmc_act_after(dyn, mid, act, h, k) < a) lo = mid; else hi = mid; }
+  return fabs(cmc_act_after(dyn, lo, act, h, k) - a) <= fabs(cmc_act_after(dyn, hi, act, h, k) - a) ? lo : hi;
+}
+
+extern "C" __global__ void __launch_bounds__(320) myo_cmc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ CmcArgs a) {
+  WARP_KERNEL_PROLOGUE(m, true)
+  const myo_cmc_buffers& d = a.d; const myo_buffers& c = a.c; const int nq = m.nq, nv = m.nv, nu = m.nu, na = m.na, lane = w.lane;
+  FOR_EACH_WARP_ENV(env, a.n_env) {
+    if (a.stage == 1) {
+      const idx_t* acls = CI(PA_cls); const double* __restrict__ PAc = GD(PA_d);
+      for (int i = lane; i < nu; i += 32) { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; const double dyn[3] = {LDC(ag), LDC(ag + 1), LDC(ag + 2)};
+        const bool lim = LDC(ag + 15) != 0; const double lo = lim ? fmax(LDC(ag + 13), 0.0) : 0.0, hi = lim ? fmin(LDC(ag + 14), 1.0) : 1.0;
+        a.ctrl[(size_t)env*nu + i] = cmc_excitation(dyn, c.act[(size_t)env*na + i], a.act[(size_t)env*nu + i], m.timestep, a.substeps, lo, hi); }
+      continue; }
+    if (a.t > 0) { const size_t row = (size_t)env*a.nstep + a.t - 1;
+      for (int i = lane; i < nu; i += 32) { const size_t o = (size_t)env*nu + i;
+        if (d.ctrl) d.ctrl[row*nu + i] = a.ctrl[o];
+        if (d.act_opt) d.act_opt[row*nu + i] = a.act[o]; }
+      for (int i = lane; i < nv; i += 32) { const size_t o = (size_t)env*nv + i;
+        if (d.reserve_force) d.reserve_force[row*nv + i] = a.rf[o];
+        if (d.lambda) d.lambda[row*nv + i] = a.lam[o];
+        if (d.qvel) d.qvel[row*nv + i] = c.qvel[o];
+        if (d.qacc) d.qacc[row*nv + i] = c.qacc_warmstart[o]; }
+      if (d.qpos) for (int i = lane; i < nq; i += 32) d.qpos[row*nq + i] = c.qpos[(size_t)env*nq + i];
+      if (d.act) for (int i = lane; i < na; i += 32) d.act[row*na + i] = c.act[(size_t)env*na + i];
+      if (lane == 0) { if (d.niter) d.niter[row] = a.niter[env]; if (d.converged) d.converged[row] = a.conv[env];
+        if (d.residual) d.residual[row] = a.res[env]; if (d.time) d.time[row] = c.time[env]; } }
+    if (a.t < a.nstep) { const size_t row = (size_t)env*a.nstep + a.t;
+      differentiate_pos(m, w, S_g, c.qpos + (size_t)env*nq, d.ref_qpos + row*nq);
+      __syncwarp();
+      for (int i = lane; i < nv; i += 32) {
+        const double v = d.ref_qacc[row*nv + i] + d.kv[i]*(d.ref_qvel[row*nv + i] - c.qvel[(size_t)env*nv + i]) + d.kp[i]*S_g[i];
+        a.qdes[(size_t)env*nv + i] = v;
+        if (d.qacc_des) d.qacc_des[row*nv + i] = v; } }
+    __syncwarp();
+  }
+}
+static_assert(sizeof(DevModel) + sizeof(CmcArgs) <= 4096, "myo_cmc_kernel's arguments fit the 4 KB kernel parameter space");
+
+// The per-frame rows of myo_batch_cmc (CmcArgs), allocated by the first call
+static int cmc_rows(myo_batch* b, CmcArgs& a, double* lam[2]) {
+  const size_t n = b->n_env, nv = b->dm.nv, nu = b->dm.nu;
+  if (!b->dCmc) CUDA_OK(cudaMalloc(&b->dCmc, n*(4*nv + 2*nu + 2)*8));
+  a.qdes = b->dCmc; a.act = a.qdes + n*nv; a.ctrl = a.act + n*nu; a.rf = a.ctrl + n*nu; lam[0] = a.rf + n*nv; lam[1] = lam[0] + n*nv;
+  a.res = lam[1] + n*nv; a.niter = (int32_t*)(a.res + n); a.conv = a.niter + n;
+  return 0;
+}
+
+extern "C" int myo_batch_cmc(myo_batch* b, const myo_cmc_buffers* d, const myo_cmc_params* p, int nstep, int flags, void* stream) {
+  if (!b || !d || !p) return fail("myo_batch_cmc: null");
+  if (!d->ref_qpos || !d->ref_qvel || !d->ref_qacc || !d->kp || !d->kv || !d->reserve) return fail("myo_batch_cmc: ref_qpos, ref_qvel, ref_qacc, kp, kv and reserve are required");
+  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_cmc: unknown flag bits");
+  if (const int rc = require_bound(b)) return rc;
+  if (nstep < 1 || p->substeps < 1) return fail("myo_batch_cmc: nstep and substeps must be >= 1");
+  if (!std::isfinite(p->tol)) return fail("myo_batch_cmc: non-finite parameter");
+  if (p->tol < 0 || p->max_iter < 0) return fail("myo_batch_cmc: needs tol >= 0 and max_iter >= 0");
+  if (b->dm.nv > 64) return fail("myo_batch_cmc: models with more than 64 dofs are not supported");
+  CUDA_OK(cudaSetDevice(b->device)); cudaStream_t st = (cudaStream_t)stream;
+  if (!b->so_shape.ready && so_plan(b->dm, b->so_off)) return -1;
+  if (analysis_shape(b, (const void*)myo_static_opt_kernel, b->so_shape) || analysis_shape(b, (const void*)myo_cmc_kernel, b->cmc_shape)) return -1;
+  CmcArgs ca; memset(&ca, 0, sizeof(ca)); double* lam[2];
+  if (const int rc = cmc_rows(b, ca, lam)) return rc;
+  // the rollout's carry from the start state; its intervals read the frame's ctrl and reserve force rows
+  myo_rollout_buffers r; memset(&r, 0, sizeof(r));
+  r.ctrl = ca.ctrl; r.qfrc_applied = ca.rf; r.qpos0 = d->qpos0; r.qvel0 = d->qvel0; r.act0 = d->act0; r.qacc_warmstart0 = d->qacc_warmstart0; r.time0 = d->time0;
+  r.overflow = d->overflow;
+  myo_buffers c;
+  if (const int rc = roll_carry(b, &r, st, c)) return rc;
+  const StepArgs ra = roll_args(b, c, &r, 1, p->substeps);
+  SoArgs so; memset(&so, 0, sizeof(so));
+  so.d.qacc = ca.qdes; so.d.weight = d->weight; so.d.reserve = d->reserve; so.d.act = ca.act; so.d.reserve_force = ca.rf; so.d.ctrl = p->substeps == 1 ? ca.ctrl : nullptr;
+  so.d.niter = ca.niter; so.d.converged = ca.conv; so.d.residual = ca.res;
+  so.p.max_iter = p->max_iter; so.p.tol = p->tol; so.b = c; so.n_env = b->n_env; so.flags = flags;
+  so.o_H = b->so_off[0]; so.o_x = b->so_off[1]; so.o_l = b->so_off[2]; so.o_cg = b->so_off[3]; so.o_tf = b->so_off[4]; so.o_s = b->so_off[5]; so.o_gm = b->so_off[6]; so.o_bm = b->so_off[7];
+  ca.d = *d; ca.c = c; ca.n_env = b->n_env; ca.nstep = nstep; ca.substeps = p->substeps;
+  const LaunchShape &sc = b->cmc_shape.s, &ss = b->so_shape.s;
+  for (int t = 0; ; t++) {
+    ca.t = t; ca.stage = 0; ca.lam = lam[(t + 1) & 1];
+    myo_cmc_kernel<<<sc.grid, sc.warps*32, sc.smem, st>>>(b->dm, ca);
+    CUDA_OK(cudaGetLastError()); b->launches++;
+    if (t == nstep) break;
+    so.d.lambda0 = t == 0 ? d->lambda0 : lam[(t + 1) & 1]; so.d.lambda = lam[t & 1];
+    myo_static_opt_kernel<<<ss.grid, ss.warps*32, ss.smem, st>>>(b->dm, so);
+    CUDA_OK(cudaGetLastError()); b->launches++;
+    if (p->substeps > 1) { ca.stage = 1;
+      myo_cmc_kernel<<<sc.grid, sc.warps*32, sc.smem, st>>>(b->dm, ca);
+      CUDA_OK(cudaGetLastError()); b->launches++; }
+    if (const int rc = roll_interval(b, ra, st)) return rc;
+  }
+  return 0;
 }

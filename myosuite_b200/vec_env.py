@@ -581,6 +581,60 @@ class MyoVecEnv:
         self.batch.static_opt(params, stream=self._stream(), flags=flags, **bufs, **out)
         return {f: out[f] for f in fields}
 
+    CMC_FIELDS = tuple(abi.CMC_SHAPES) + ("overflow",)
+
+    def cmc(self, ref_qpos, ref_qvel, ref_qacc, kp, kv, reserve, weight=None, substeps=1, constraints=True, discrete=False, initial_state=None,
+            warmstart=None, max_iter=STATIC_OPT_DEFAULTS["max_iter"], tol=STATIC_OPT_DEFAULTS["tol"],
+            fields=("qpos", "qvel", "act", "ctrl", "act_opt", "reserve_force", "niter", "converged")):
+        """Computed muscle control of every env along its own reference motion (myo_batch_cmc; include/myo_b200.h states the loop): for
+        each frame t, the desired acceleration qacc_des = ref_qacc[:, t] + kv (ref_qvel[:, t] - qvel) + kp (ref_qpos[:, t] (-) qpos) ((-):
+        mj_differentiatePos), the static optimisation of static_opt() for it (reserve, weight, constraints, discrete, max_iter and tol as
+        there, warm-started from the previous frame's lambda, frame 0 from `warmstart` [num_envs, nv] or 0), the excitation that brings act
+        to the optimal activations at the end of `substeps` mj_steps with ctrl held, and that interval of rollout() with qfrc_applied = the
+        reserve forces.  ref_qpos [num_envs, T, nq], ref_qvel and ref_qacc [num_envs, T, nv] are contiguous float64 CUDA tensors on this
+        batch's device; kp and kv are gains >= 0, reserve and weight strengths > 0, each a scalar or a vector ([nv], weight [nu]).
+        initial_state as rollout()'s.  Returns {field: tensor [num_envs, T, ...]} of CMC_FIELDS: qacc_des, ctrl, act_opt (a*),
+        reserve_force, lambda [nv or nu], niter, converged (int32), residual, and the state after the frame's interval qpos, qvel, act,
+        qacc, time (rollout()'s rows); overflow [num_envs] int32.  Row t equals static_opt() and rollout() run from row t - 1's state, bit
+        for bit.  The tensors are allocated per call; the frames run on the device without a host synchronisation.  Not a state change."""
+        torch, m, n = self.torch, self.mj_model, self.num_envs
+        fields = _check_fields("cmc", fields, self.CMC_FIELDS)
+        substeps = int(substeps)
+        if substeps < 1:
+            raise ValueError("substeps must be >= 1, got %d" % substeps)
+        T = int(ref_qpos.shape[1]) if isinstance(ref_qpos, torch.Tensor) and ref_qpos.dim() == 3 else 0
+        if T < 1:
+            raise ValueError("ref_qpos must be a float64 tensor [num_envs, T >= 1, nq], got %s" % (tuple(getattr(ref_qpos, "shape", ())),))
+        _check_f64("ref_qpos", ref_qpos, (n, T, m.nq), self.device)
+        _check_f64("ref_qvel", ref_qvel, (n, T, m.nv), self.device)
+        _check_f64("ref_qacc", ref_qacc, (n, T, m.nv), self.device)
+
+        def vector(name, x, width, positive):
+            v = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+            if v.dtype.kind not in "biuf" or v.shape not in ((), (width,)):
+                raise ValueError("%s must be a scalar or of shape (%d,), got %s %s" % (name, width, v.dtype, v.shape))
+            v = np.broadcast_to(v.astype(np.float64), (width,))
+            if not np.all(np.isfinite(v) & ((v > 0) if positive else (v >= 0))):
+                raise ValueError("%s must be finite and %s" % (name, "> 0" if positive else ">= 0"))
+            return torch.as_tensor(v.copy(), device=self.device)
+        bufs = {"ref_qpos": ref_qpos, "ref_qvel": ref_qvel, "ref_qacc": ref_qacc, "kp": vector("kp", kp, m.nv, False),
+                "kv": vector("kv", kv, m.nv, False), "reserve": vector("reserve", reserve, m.nv, True)}
+        if weight is not None:
+            bufs["weight"] = vector("weight", weight, m.nu, True)
+        if warmstart is not None:
+            _check_f64("warmstart", warmstart, (n, m.nv), self.device)
+            bufs["lambda0"] = warmstart
+        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=()), n, self.device))
+        params = abi.MyoCmcParams(max_iter=int(max_iter), substeps=substeps, tol=float(tol))
+        if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
+            raise ValueError("cmc needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (max_iter, tol))
+        size = dict(nq=m.nq, nv=m.nv, nu=m.nu, na=m.na)
+        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow"
+               else _output(self.device, (n, T), abi.CMC_SHAPES[f], size, f in ("niter", "converged")) for f in fields}
+        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
+        self.batch.cmc(params, T, stream=self._stream(), flags=flags, **bufs, **out)
+        return out
+
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
         """Batched MujocoEnv.examine_policy_new (env_base.py:853-969): one episode per env, observations / actions stay on the device;
         returns (Trace with one "Trial<k>" group per env, summary dict).  See myosuite_b200/rollout.py."""
@@ -793,6 +847,20 @@ class MyoEnv:
         out = v.static_opt(as_dev(qacc, (1, -1)), reserve if np.ndim(reserve) == 0 else as_dev(reserve, (-1,)), weight=as_dev(weight, (-1,)),
                            constraints=constraints, discrete=discrete, warmstart=as_dev(warmstart, (1, -1)), fields=fields, **params)
         return {k: (int(x[0]) if k in ("niter", "converged") else (float(x[0]) if k == "residual" else x[0].cpu().numpy())) for k, x in out.items()}
+
+    def cmc(self, ref_qpos, ref_qvel, ref_qacc, kp, kv, reserve, weight=None, initial_state=None, warmstart=None,
+            fields=("qpos", "qvel", "act", "ctrl", "act_opt", "reserve_force", "niter", "converged"), **params):
+        """Computed muscle control of this env along a reference motion (MyoVecEnv.cmc): ref_qpos [T, nq], ref_qvel and ref_qacc [T, nv],
+        kp, kv, reserve (scalars or [nv]), weight [nu] or None, initial_state {key: array} or None (the current state), warmstart [nv] or
+        None; params: substeps, constraints, discrete, max_iter, tol.  Returns {field: numpy array [T, ...]} (overflow as an int).  Not a
+        state change."""
+        v = self.vec
+        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        T = np.asarray(ref_qpos).reshape(-1, self.mj_model.nq).shape[0]
+        st = None if initial_state is None else {k: as_dev(x, (1,) if k == "time" else (1, -1)) for k, x in initial_state.items()}
+        out = v.cmc(as_dev(ref_qpos, (1, T, -1)), as_dev(ref_qvel, (1, T, -1)), as_dev(ref_qacc, (1, T, -1)), kp, kv, reserve, weight=weight,
+                    initial_state=st, warmstart=as_dev(warmstart, (1, -1)), fields=fields, **params)
+        return {k: (int(x[0]) if k == "overflow" else x[0].cpu().numpy()) for k, x in out.items()}
 
     def mj_jacSite(self, site):
         """mujoco.mj_jacSite at the current state: (jacp [3, nv], jacr [3, nv]) as numpy arrays."""
