@@ -3,8 +3,9 @@
 CPU: the C ABI's buffer and parameter structs against the binding, and the k-step excitation (bisection over the k-step map of the
 activation dynamics) against the oracle's own activation dynamics stepped k times.
 GPU, on both row storages where the pattern exists: every row of the call bit-identical to static_opt() and rollout() run from the call's
-previous row; qacc_des against a numpy restatement; act at the end of a frame_skip interval against a*; tracking of the hand trajectory
-fixture and of references the simulator generated itself; batch independence, side effects, launch count and input checks; the single env.
+previous row, at substeps 1 and frame_skip; qacc_des against a numpy restatement; act at the end of a frame_skip interval against a*;
+tracking of the hand trajectory fixture and of references the simulator generated itself; batch independence, side effects, launch count
+and input checks; the single env.  (tests/test_cmc_reference.py holds the call to a CPU reference of the whole frame.)
 """
 import ctypes
 import os
@@ -139,39 +140,37 @@ def _row_state(out, start, t):
 
 
 # ----------------------------------------------------------------------------- GPU: the chain of public calls
-@pytest.mark.gpu
-@pytest.mark.parametrize("rows", ROWS)
-@pytest.mark.parametrize("case", list(CASES))
-def test_chain_identity_and_qacc_des(case, rows):
-    """64 envs, 8 frames, substeps 1, on a self-generated reference, with constraints, with constraints=False and with discrete=True: every
-    row bit-identical to static_opt(qacc_des[:, t], warmstart=lambda[:, t - 1]) and rollout(ctrl[:, t], qfrc_applied=reserve_force[:, t]),
-    both from the call's row t - 1; and qacc_des against its numpy restatement with FdOracle.differentiate_pos."""
+def _chain(case, rows, frame_skip):
+    """the chain of public calls at one substep per frame or at the task's frame_skip; there the call's ctrl is the k-step excitation, which
+    static_opt()'s one-step ctrl is not, so ctrl is left to test_excitation_over_interval"""
     import torch
     from fd_oracle import FdOracle
     env = _env(case, CHAIN_ENVS, rows)
     m, T = env.mj_model, CHAIN_FRAMES
+    k = env.n_frames if frame_skip else 1
     rho = CASE_RESERVE.get(case, RESERVE)
-    ref_qpos, ref_qvel, ref_qacc, start, _ = _self_reference(env, T, 1)
+    ref_qpos, ref_qvel, ref_qacc, start, _ = _self_reference(env, T, k)
     free = bool(np.any(np.asarray(m.jnt_type) == 0))
     fo = FdOracle(env.I, env.D)
     worst_q = 0.0
     for con, disc in ((True, False), (False, False), (False, True)):
-        out = env.cmc(ref_qpos, ref_qvel, ref_qacc, KP, KV, rho, constraints=con, discrete=disc, initial_state=start, fields=ALL)
+        out = env.cmc(ref_qpos, ref_qvel, ref_qacc, KP, KV, rho, substeps=k, constraints=con, discrete=disc, initial_state=start, fields=ALL)
         torch.cuda.synchronize()
-        assert torch.isfinite(out["qpos"]).all() and torch.all(out["niter"] >= 0)
+        assert torch.all(out["niter"] >= 0) and (torch.isfinite(out["qpos"]).all() or (k > 1 and case in DIVERGING))
         for t in range(T):
             s = _row_state(out, start, t)
-            for k in ("qpos", "qvel", "act"):
-                env.t[k].copy_(s[k])
+            for key in ("qpos", "qvel", "act"):
+                env.t[key].copy_(s[key])
             S = env.static_opt(out["qacc_des"][:, t].contiguous(), rho, constraints=con, discrete=disc,
                                warmstart=None if t == 0 else out["lambda"][:, t - 1].contiguous(),
                                fields=("act", "reserve_force", "ctrl", "lambda", "niter", "converged", "residual"))
             for a, b in (("act", "act_opt"), ("reserve_force", "reserve_force"), ("ctrl", "ctrl"), ("lambda", "lambda"), ("niter", "niter"),
                          ("converged", "converged"), ("residual", "residual")):
-                assert _same(S[a], out[b][:, t]), (con, disc, t, b)
-            r = env.rollout(out["ctrl"][:, t:t + 1].contiguous(), qfrc_applied=out["reserve_force"][:, t:t + 1].contiguous(), initial_state=s)
-            for k in STATE:
-                assert _same(r[k][:, 0], out[k][:, t]), (con, disc, t, k)
+                assert (a == "ctrl" and k > 1) or _same(S[a], out[b][:, t]), (con, disc, t, b)
+            r = env.rollout(out["ctrl"][:, t:t + 1].contiguous(), qfrc_applied=out["reserve_force"][:, t:t + 1].contiguous(), substeps=k,
+                            initial_state=s)
+            for key in STATE:
+                assert _same(r[key][:, 0], out[key][:, t]), (con, disc, t, key)
         # qacc_des = ref_qacc + kv (ref_qvel - qvel) + kp (ref_qpos (-) qpos) at each frame's start state
         H = _host(out)
         S0 = _host(start)
@@ -180,18 +179,40 @@ def test_chain_identity_and_qacc_des(case, rows):
             for t in range(T):
                 q = S0["qpos"][e] if t == 0 else H["qpos"][e, t - 1]
                 v = S0["qvel"][e] if t == 0 else H["qvel"][e, t - 1]
+                if not (np.isfinite(q).all() and np.isfinite(v).all()):        # a diverged row (bit-identical above all the same)
+                    continue
                 terms = np.stack([RA[e, t], KV * (RV[e, t] - v), KP * fo.differentiate_pos(q, RQ[e, t])])
                 err = np.abs(H["qacc_des"][e, t] - terms.sum(0)).max() / max(np.abs(terms).max(), 1e-300)
                 worst_q = max(worst_q, err)
                 assert err <= (QDES_REL_FREE if free else QDES_REL), (con, disc, e, t, err)
-    REPORT["chain %s[%s]" % (case, rows)] = "bit-identical over %d frames x 3 flag sets; qacc_des worst %.1e relative" % (T, worst_q)
-    print("\n" + REPORT["chain %s[%s]" % (case, rows)])
+    key = "chain %s[%s]%s" % (case, rows, "" if k == 1 else " k=%d" % k)
+    REPORT[key] = "bit-identical over %d frames x 3 flag sets; qacc_des worst %.1e relative" % (T, worst_q)
+    print("\n" + REPORT[key])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("rows", ROWS)
+@pytest.mark.parametrize("case", list(CASES))
+def test_chain_identity_and_qacc_des(case, rows):
+    """64 envs, 8 frames, substeps 1, on a self-generated reference, with constraints, with constraints=False and with discrete=True: every
+    row bit-identical to static_opt(qacc_des[:, t], warmstart=lambda[:, t - 1]) and rollout(ctrl[:, t], qfrc_applied=reserve_force[:, t]),
+    both from the call's row t - 1; and qacc_des against its numpy restatement with FdOracle.differentiate_pos."""
+    _chain(case, rows, False)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("rows", ROWS)
+@pytest.mark.parametrize("case", list(CASES))
+def test_chain_identity_at_frame_skip(case, rows):
+    """The same at substeps = frame_skip: act_opt, reserve_force, lambda, niter, converged and residual bit-identical to static_opt(), and
+    the state to rollout(ctrl[:, t], qfrc_applied=reserve_force[:, t], substeps=frame_skip), both from the call's row t - 1."""
+    _chain(case, rows, True)
 
 
 # ----------------------------------------------------------------------------- GPU: the excitation over a control interval
 @pytest.mark.gpu
 @pytest.mark.parametrize("rows", ROWS)
-@pytest.mark.parametrize("case", ["elbow", "hand_pose", "torso"])
+@pytest.mark.parametrize("case", list(CASES))
 def test_excitation_over_interval(case, rows):
     """substeps = frame_skip: the returned ctrl rolled out from each frame's start state (act := act_t) brings act to act_opt at the end of
     the interval where ctrl is not clipped; where it is clipped, a* is out of reach on that side."""
@@ -201,20 +222,24 @@ def test_excitation_over_interval(case, rows):
     ref_qpos, ref_qvel, ref_qacc, start, _ = _self_reference(env, T, k)
     out = env.cmc(ref_qpos, ref_qvel, ref_qacc, KP, KV, CASE_RESERVE.get(case, RESERVE), substeps=k, initial_state=start, fields=ALL)
     lo = np.array([R.ctrl_range(m, i)[0] for i in range(m.nu)]); hi = np.array([R.ctrl_range(m, i)[1] for i in range(m.nu)])
-    worst, clipped = 0.0, 0
+    worst, clipped, checked = 0.0, 0, 0
     for t in range(T):
         r = env.rollout(out["ctrl"][:, t:t + 1].contiguous(), qfrc_applied=out["reserve_force"][:, t:t + 1].contiguous(), substeps=k,
                         initial_state=_row_state(out, start, t))
         got, tgt, c = r["act"][:, 0].cpu().numpy(), out["act_opt"][:, t].cpu().numpy(), out["ctrl"][:, t].cpu().numpy()
-        assert np.array_equal(got, out["act"][:, t].cpu().numpy())
+        assert _same(r["act"][:, 0], out["act"][:, t])
+        live = np.isfinite(tgt).all(1) & np.isfinite(c).all(1)             # the envs whose frame starts from a finite row
+        got, tgt, c = got[live], tgt[live], c[live]
         free = (c > lo) & (c < hi)
         worst = max(worst, float(np.abs(got - tgt)[free].max()) if free.any() else 0.0)
         assert np.all(np.abs(got - tgt)[free] <= EXCITE_TOL), float(np.abs(got - tgt)[free].max())
         at_hi, at_lo = (c >= hi) & ~free, (c <= lo) & ~free
         assert np.all(got[at_hi] <= tgt[at_hi] + EXCITE_TOL) and np.all(got[at_lo] >= tgt[at_lo] - EXCITE_TOL)
         clipped += int((~free).sum())
-    assert torch.isfinite(out["ctrl"]).all()
-    REPORT["excite %s[%s]" % (case, rows)] = "k %d: worst |act - a*| %.1e where not clipped, %d clipped" % (k, worst, clipped)
+        checked += int(live.sum())
+    assert torch.isfinite(out["ctrl"]).all() or case in DIVERGING
+    REPORT["excite %s[%s]" % (case, rows)] = "k %d: worst |act - a*| %.1e where not clipped, %d clipped, %d of %d env-frames from finite rows" % (
+        k, worst, clipped, checked, CHAIN_ENVS * T)
     print("\n" + REPORT["excite %s[%s]" % (case, rows)])
 
 
@@ -254,29 +279,30 @@ def test_cmc_call_tracks_hand_trajectory():
     assert pooled >= TRACK_RATIO and moving.sum() >= 8 and np.all(ratio[moving] >= 8), (pooled, ratio)
 
 
-# (case, substeps) below the 10x bound on an H100 80GB HBM3 (700 W), with the measured pooled ratio.  With the per-model reserves the
-# muscles carry most of the force on the hands, and their activation lag limits the tracking; on the legs the reserves carry the unactuated
-# pelvis through changing ground contacts.  Held over a frame_skip interval the legs' and the held object's solutions diverge.
-BELOW_BOUND = {("hand_pose", "1"): "4.9x", ("hand_pose", "frame_skip"): "4.7x", ("reach", "1"): "2.8x", ("reach", "frame_skip"): "4.7x",
-               ("hold", "1"): "4.0x", ("hold", "frame_skip"): "diverges (NaN)", ("walk_fatigue", "1"): "0.7x",
-               ("walk_fatigue", "frame_skip"): "diverges (NaN)", ("stand", "1"): "1.0x", ("stand", "frame_skip"): "diverges (NaN)",
-               ("torso", "1"): "1.6x"}
+# Pooled ratios below the 10x bound on an NVIDIA H100 80GB HBM3 (700 W), and the floor each case is held to (0.8x the measured ratio, so
+# that a regression fails).  With the per-model reserves the muscles carry most of the force on the hands, and their activation lag
+# limits the tracking; on the legs the reserves carry the unactuated pelvis through changing ground contacts.
+BELOW_BOUND = {("hand_pose", "1"): 4.9, ("hand_pose", "frame_skip"): 4.7, ("reach", "1"): 2.8, ("reach", "frame_skip"): 4.7,
+               ("hold", "1"): 4.0, ("walk_fatigue", "1"): 0.7, ("stand", "1"): 1.0, ("torso", "1"): 1.6}
+FLOOR = 0.8
+# Held over frame_skip substeps, the reserve forces and a* solved at the frame's start state diverge on the held object and the legs:
+# the CPU reference of the same loop diverges as well (tests/test_cmc_reference.py, DESIGN.md section 4).
+DIVERGING = ("hold", "walk_fatigue", "stand")
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case,substeps", [pytest.param(c, k, marks=pytest.mark.xfail(reason="measured " + BELOW_BOUND[(c, k)], strict=False))
-                                           if (c, k) in BELOW_BOUND else (c, k) for c in CASES for k in ("1", "frame_skip")])
+@pytest.mark.parametrize("case,substeps", [(c, k) for c in CASES for k in ("1", "frame_skip")])
 def test_cmc_tracks_self_generated_reference(case, substeps):
     """On every base task, along a self-generated reference from a perturbed start, with the per-model reserves of test_static_opt.py: the
-    pooled RMS position error at least 10x below that of the same start with zero ctrl and no reserves.  The cases BELOW_BOUND lists
-    do not meet the bound; they run as expected failures and print their ratios."""
+    pooled RMS position error at least 10x below that of the same start with zero ctrl and no reserves; FLOOR x the measured ratio for
+    the cases BELOW_BOUND lists; and at frame_skip on the DIVERGING tasks, the divergence itself (a non-finite row or |qvel| > 1e3)."""
     import torch
     n, T = 256, 100
     env = _env(case, n)
     m, k = env.mj_model, (1 if substeps == "1" else env.n_frames)
     ref_qpos, ref_qvel, ref_qacc, start, goal = _self_reference(env, T, k)
     out = env.cmc(ref_qpos, ref_qvel, ref_qacc, KP, KV, CASE_RESERVE.get(case, RESERVE), substeps=k, initial_state=start,
-                  fields=("qpos", "reserve_force", "niter", "converged"))
+                  fields=("qpos", "qvel", "reserve_force", "niter", "converged"))
     passive = env.rollout(torch.zeros(n, T, m.nu, dtype=torch.float64, device=env.device), substeps=k, initial_state=start, fields=("qpos",))
     g = goal.cpu().numpy()
     # errors in the tangent space (free joints: position and rotation vector)
@@ -286,11 +312,21 @@ def test_cmc_tracks_self_generated_reference(case, substeps):
     e_c = np.array([[fo.differentiate_pos(g[e, t], Q[e, t]) for t in range(T)] for e in range(n)]) ** 2
     e_p = np.array([[fo.differentiate_pos(g[e, t], P[e, t]) for t in range(T)] for e in range(n)]) ** 2
     pooled = _pooled(e_p, e_c)
-    REPORT["track %s k=%d" % (case, k)] = ("pooled ratio %.1f (RMS CMC %.2e, passive %.2e), Newton steps %.2f, unconverged %.4f, RMS reserve force %.3g"
+    V = out["qvel"].cpu().numpy()
+    gone = ~(np.isfinite(Q).all(2) & (np.abs(np.nan_to_num(V, nan=np.inf)) <= 1e3).all(2))          # [n, T]
+    diverged = gone.any(1)
+    REPORT["track %s k=%d" % (case, k)] = ("pooled ratio %.1f (RMS CMC %.2e, passive %.2e), Newton steps %.2f, unconverged %.4f, RMS reserve force %.3g; "
+                                           "%d of %d envs diverge (first at frame %d)"
                                            % (pooled, np.sqrt(e_c.mean()), np.sqrt(e_p.mean()), out["niter"].double().mean().item(),
-                                              (out["converged"] != 1).double().mean().item(), out["reserve_force"].pow(2).mean().sqrt().item()))
+                                              (out["converged"] != 1).double().mean().item(), out["reserve_force"].pow(2).mean().sqrt().item(),
+                                              int(diverged.sum()), n, int(gone.any(0).argmax()) if diverged.any() else T))
     print("\n" + REPORT["track %s k=%d" % (case, k)])
-    assert pooled >= TRACK_RATIO, pooled
+    if substeps == "frame_skip" and case in DIVERGING:
+        assert diverged.any(), "the run no longer diverges: re-measure it and move the case to BELOW_BOUND or the 10x bound"
+    elif (case, substeps) in BELOW_BOUND:
+        assert not diverged.any() and pooled >= FLOOR * BELOW_BOUND[(case, substeps)], (pooled, BELOW_BOUND[(case, substeps)])
+    else:
+        assert not diverged.any() and pooled >= TRACK_RATIO, pooled
 
 
 # ----------------------------------------------------------------------------- GPU: batches, side effects, launches, checks

@@ -153,11 +153,14 @@ def _warm_env(case, rows, **kw):
     return env
 
 
-def kkt(env, S, qacc, rho, w, con=True, disc=False):
-    """The solver-independent certificate on every env: 0 <= a <= 1 exactly, a = clip(G' lambda / w, 0, 1) with G' lambda from the dense
-    moments and the returned gain, reserve_force = rho^2 lambda exactly, and the primal residual within the stop rule."""
+def kkt(env, S, qacc, rho, w, con=True, disc=False, rows=None):
+    """The solver-independent certificate on every env (or on the envs `rows` selects): 0 <= a <= 1 exactly, a = clip(G' lambda / w, 0, 1)
+    with G' lambda from the dense moments and the returned gain, reserve_force = rho^2 lambda exactly, and the primal residual within the
+    stop rule."""
     m = env.mj_model
     M = _host(env.inverse(qacc, constraints=con, discrete=disc, fields=("qfrc_inverse", "actuator_moment")))
+    if rows is not None:
+        M, S = {k: v[rows] for k, v in M.items()}, {k: v[rows] for k, v in S.items()}
     a, lam, g, b, r = S["act"], S["lambda"], S["muscle_gain"], S["muscle_bias"], S["reserve_force"]
     assert np.all((a >= 0) & (a <= 1))
     assert np.array_equal(r, (rho ** 2)[None, :] * lam)
