@@ -883,15 +883,21 @@ __device__ __forceinline__ double so_phi_diff(double s, double ds, double wm) {
 __device__ __forceinline__ double so_act_next(const double* dyn, double c, double act, double h) {
   const double dctrl = clipd(c, 0, 1) - act; return act + h*(dctrl*m_rcp(fmax(MYO_MINVAL, muscle_tau(dyn, dctrl, act)))); }
 
-// the excitation that takes act to a in one step, inside [lo, hi]
-__device__ __forceinline__ double so_excitation(const double* dyn, double act, double a, double h, double lo, double hi) {
-  if (dyn[2] < MYO_MINVAL) { const double dd = a - act; return clipd(act + dd*muscle_tau(dyn, dd, act)/h, lo, hi); }
-  if (so_act_next(dyn, hi, act, h) <= a) return hi;
-  if (so_act_next(dyn, lo, act, h) >= a) return lo;
-  for (int k = 0; k < 200; k++) { const double mid = 0.5*(lo + hi); if (!(mid > lo && mid < hi)) break;
-    if (so_act_next(dyn, mid, act, h) < a) lo = mid; else hi = mid; }
-  return fabs(so_act_next(dyn, lo, act, h) - a) <= fabs(so_act_next(dyn, hi, act, h) - a) ? lo : hi;
+// the excitation that, held for k mj_steps, takes act to a, inside [lo, hi]: in one step without smooth activation (dyn[2]) the closed
+// form of that step, otherwise bisection over the k-step map
+__device__ __forceinline__ double excitation(const double* dyn, double act, double a, double h, int k, double lo, double hi) {
+  if (k == 1 && dyn[2] < MYO_MINVAL) { const double dd = a - act; return clipd(act + dd*muscle_tau(dyn, dd, act)/h, lo, hi); }
+  const auto after = [&](double c) { double x = act; for (int j = 0; j < k; j++) x = so_act_next(dyn, c, x, h); return x; };
+  if (after(hi) <= a) return hi;
+  if (after(lo) >= a) return lo;
+  for (int it = 0; it < 200; it++) { const double mid = 0.5*(lo + hi); if (!(mid > lo && mid < hi)) break;
+    if (after(mid) < a) lo = mid; else hi = mid; }
+  return fabs(after(lo) - a) <= fabs(after(hi) - a) ? lo : hi;
 }
+
+// the range an excitation is clipped to, from the muscle's PA_d row ag: ctrlrange inside [0, 1] when ctrllimited, else [0, 1]
+__device__ __forceinline__ void excitation_range(const DevModel& m, const double* __restrict__ ag, double& lo, double& hi) {
+  const bool lim = LDC(ag + 15) != 0; lo = lim ? fmax(LDC(ag + 13), 0.0) : 0.0; hi = lim ? fmin(LDC(ag + 14), 1.0) : 1.0; }
 
 extern "C" __global__ void __launch_bounds__(320) myo_static_opt_kernel(const __grid_constant__ DevModel m, const __grid_constant__ SoArgs a) {
   WARP_KERNEL_PROLOGUE(m, true)
@@ -980,8 +986,8 @@ extern "C" __global__ void __launch_bounds__(320) myo_static_opt_kernel(const __
       d.act[o] = act;
       if (d.actuator_force) d.actuator_force[o] = gm[i]*act + bm[i];
       if (d.ctrl) { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; const double dyn[3] = {LDC(ag), LDC(ag + 1), LDC(ag + 2)};
-        const bool lim = LDC(ag + 15) != 0; const double lo = lim ? fmax(LDC(ag + 13), 0.0) : 0.0, hi = lim ? fmin(LDC(ag + 14), 1.0) : 1.0;
-        d.ctrl[o] = so_excitation(dyn, W_(act)[i], act, m.timestep, lo, hi); } }
+        double lo, hi; excitation_range(m, ag, lo, hi);
+        d.ctrl[o] = excitation(dyn, W_(act)[i], act, m.timestep, 1, lo, hi); } }
     __syncwarp();
   }
 }
@@ -1231,6 +1237,8 @@ extern "C" int myo_debug_chol_solve(int device, const double* H_host, double* x_
 }
 
 static int require_bound(const myo_batch* b) { return b->bound ? 0 : fail("batch has no bound buffers (call myo_batch_bind)"); }
+static int require_64_dofs(const myo_batch* b, const std::string& call) {      // the IK and static-optimisation kernels: two dofs per lane
+  return b->dm.nv > 64 ? fail(call + ": models with more than 64 dofs are not supported") : 0; }
 
 extern "C" int myo_batch_bind(myo_batch* b, const myo_buffers* bufs) {
   if (!b || !bufs) return fail("myo_batch_bind: null");
@@ -1466,7 +1474,7 @@ extern "C" int myo_batch_ik(myo_batch* b, const myo_ik_buffers* d, const myo_ik_
     return fail("myo_batch_ik: non-finite parameter");
   if (p->damping <= 0 || p->max_step <= 0 || p->tol < 0 || p->max_iter < 0 || p->posture_weight < 0 || p->eq_weight < 0)
     return fail("myo_batch_ik: needs damping > 0, max_step > 0, tol >= 0, max_iter >= 0, posture_weight >= 0 and eq_weight >= 0");
-  if (b->dm.nv > 64) return fail("myo_batch_ik: models with more than 64 dofs are not supported");
+  if (const int rc = require_64_dofs(b, "myo_batch_ik")) return rc;
   CUDA_OK(cudaSetDevice(b->device));
   int32_t sid[MYO_IK_MAXSITE]; cudaStream_t st = (cudaStream_t)stream;      // the site list decides the kernel arguments: read it back
   CUDA_OK(cudaMemcpyAsync(sid, d->site_id, (size_t)ns*4, cudaMemcpyDeviceToHost, st)); CUDA_OK(cudaStreamSynchronize(st));
@@ -1542,20 +1550,32 @@ static int so_plan(const DevModel& d, int* off) {
 
 static_assert(sizeof(DevModel) + sizeof(SoArgs) <= 4096, "myo_static_opt_kernel's arguments fit the 4 KB kernel parameter space");
 
+// The checks of the static optimisation's flags and parameters, shared by the calls that launch it (`call` names the call in the message)
+static int so_check(const myo_batch* b, const std::string& call, int flags, int max_iter, double tol) {
+  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail(call + ": unknown flag bits");
+  if (const int rc = require_bound(b)) return rc;
+  if (!std::isfinite(tol)) return fail(call + ": non-finite parameter");
+  if (tol < 0 || max_iter < 0) return fail(call + ": needs tol >= 0 and max_iter >= 0");
+  return require_64_dofs(b, call);
+}
+// myo_static_opt_kernel's scratch placement and launch shape, set by the first call that launches it; on the current device
+static int so_setup(myo_batch* b) {
+  return !b->so_shape.ready && so_plan(b->dm, b->so_off) ? -1 : analysis_shape(b, (const void*)myo_static_opt_kernel, b->so_shape); }
+// The SoArgs of a launch over the state buffers c, with every buffer of a.d null
+static SoArgs so_args(const myo_batch* b, int max_iter, double tol, int flags, const myo_buffers& c) {
+  SoArgs a; memset(&a, 0, sizeof(a));
+  a.p.max_iter = max_iter; a.p.tol = tol; a.b = c; a.n_env = b->n_env; a.flags = flags;
+  a.o_H = b->so_off[0]; a.o_x = b->so_off[1]; a.o_l = b->so_off[2]; a.o_cg = b->so_off[3]; a.o_tf = b->so_off[4]; a.o_s = b->so_off[5]; a.o_gm = b->so_off[6]; a.o_bm = b->so_off[7];
+  return a;
+}
+
 extern "C" int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* d, const myo_static_opt_params* p, int flags, void* stream) {
   if (!b || !d || !p) return fail("myo_batch_static_opt: null");
   if (!d->qacc || !d->reserve || !d->act) return fail("myo_batch_static_opt: qacc, reserve and act are required");
-  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_static_opt: unknown flag bits");
-  if (const int rc = require_bound(b)) return rc;
-  if (!std::isfinite(p->tol)) return fail("myo_batch_static_opt: non-finite parameter");
-  if (p->tol < 0 || p->max_iter < 0) return fail("myo_batch_static_opt: needs tol >= 0 and max_iter >= 0");
-  if (b->dm.nv > 64) return fail("myo_batch_static_opt: models with more than 64 dofs are not supported");
+  if (const int rc = so_check(b, "myo_batch_static_opt", flags, p->max_iter, p->tol)) return rc;
   CUDA_OK(cudaSetDevice(b->device));
-  if (!b->so_shape.ready && so_plan(b->dm, b->so_off)) return -1;
-  if (analysis_shape(b, (const void*)myo_static_opt_kernel, b->so_shape)) return -1;
-  SoArgs a; memset(&a, 0, sizeof(a));
-  a.d = *d; a.p = *p; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags;
-  a.o_H = b->so_off[0]; a.o_x = b->so_off[1]; a.o_l = b->so_off[2]; a.o_cg = b->so_off[3]; a.o_tf = b->so_off[4]; a.o_s = b->so_off[5]; a.o_gm = b->so_off[6]; a.o_bm = b->so_off[7];
+  if (so_setup(b)) return -1;
+  SoArgs a = so_args(b, p->max_iter, p->tol, flags, b->bufs); a.d = *d;
   const LaunchShape& s = b->so_shape.s;
   myo_static_opt_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
@@ -1571,20 +1591,6 @@ extern "C" int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* 
 struct CmcArgs { myo_cmc_buffers d; myo_buffers c; int n_env, nstep, t, stage, substeps;
   double *qdes, *act, *ctrl, *rf, *lam, *res; int32_t *niter, *conv; };      // lam: the rows frame t - 1 wrote
 
-// act after k mj_steps of the activation dynamics with ctrl c held (c already inside ctrlrange)
-__device__ __forceinline__ double cmc_act_after(const double* dyn, double c, double act, double h, int k) {
-  for (int j = 0; j < k; j++) act = so_act_next(dyn, c, act, h);
-  return act; }
-
-// the excitation that, held for k steps, takes act to a, inside [lo, hi]: so_excitation's bisection over the k-step map
-__device__ __forceinline__ double cmc_excitation(const double* dyn, double act, double a, double h, int k, double lo, double hi) {
-  if (cmc_act_after(dyn, hi, act, h, k) <= a) return hi;
-  if (cmc_act_after(dyn, lo, act, h, k) >= a) return lo;
-  for (int it = 0; it < 200; it++) { const double mid = 0.5*(lo + hi); if (!(mid > lo && mid < hi)) break;
-    if (cmc_act_after(dyn, mid, act, h, k) < a) lo = mid; else hi = mid; }
-  return fabs(cmc_act_after(dyn, lo, act, h, k) - a) <= fabs(cmc_act_after(dyn, hi, act, h, k) - a) ? lo : hi;
-}
-
 extern "C" __global__ void __launch_bounds__(320) myo_cmc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ CmcArgs a) {
   WARP_KERNEL_PROLOGUE(m, true)
   const myo_cmc_buffers& d = a.d; const myo_buffers& c = a.c; const int nq = m.nq, nv = m.nv, nu = m.nu, na = m.na, lane = w.lane;
@@ -1592,8 +1598,8 @@ extern "C" __global__ void __launch_bounds__(320) myo_cmc_kernel(const __grid_co
     if (a.stage == 1) {
       const idx_t* acls = CI(PA_cls); const double* __restrict__ PAc = GD(PA_d);
       for (int i = lane; i < nu; i += 32) { const double* __restrict__ ag = PAc + acls[i]*PA_STRIDE; const double dyn[3] = {LDC(ag), LDC(ag + 1), LDC(ag + 2)};
-        const bool lim = LDC(ag + 15) != 0; const double lo = lim ? fmax(LDC(ag + 13), 0.0) : 0.0, hi = lim ? fmin(LDC(ag + 14), 1.0) : 1.0;
-        a.ctrl[(size_t)env*nu + i] = cmc_excitation(dyn, c.act[(size_t)env*na + i], a.act[(size_t)env*nu + i], m.timestep, a.substeps, lo, hi); }
+        double lo, hi; excitation_range(m, ag, lo, hi);
+        a.ctrl[(size_t)env*nu + i] = excitation(dyn, c.act[(size_t)env*na + i], a.act[(size_t)env*nu + i], m.timestep, a.substeps, lo, hi); }
       continue; }
     if (a.t > 0) { const size_t row = (size_t)env*a.nstep + a.t - 1;
       for (int i = lane; i < nu; i += 32) { const size_t o = (size_t)env*nu + i;
@@ -1632,15 +1638,10 @@ static int cmc_rows(myo_batch* b, CmcArgs& a, double* lam[2]) {
 extern "C" int myo_batch_cmc(myo_batch* b, const myo_cmc_buffers* d, const myo_cmc_params* p, int nstep, int flags, void* stream) {
   if (!b || !d || !p) return fail("myo_batch_cmc: null");
   if (!d->ref_qpos || !d->ref_qvel || !d->ref_qacc || !d->kp || !d->kv || !d->reserve) return fail("myo_batch_cmc: ref_qpos, ref_qvel, ref_qacc, kp, kv and reserve are required");
-  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_cmc: unknown flag bits");
-  if (const int rc = require_bound(b)) return rc;
   if (nstep < 1 || p->substeps < 1) return fail("myo_batch_cmc: nstep and substeps must be >= 1");
-  if (!std::isfinite(p->tol)) return fail("myo_batch_cmc: non-finite parameter");
-  if (p->tol < 0 || p->max_iter < 0) return fail("myo_batch_cmc: needs tol >= 0 and max_iter >= 0");
-  if (b->dm.nv > 64) return fail("myo_batch_cmc: models with more than 64 dofs are not supported");
+  if (const int rc = so_check(b, "myo_batch_cmc", flags, p->max_iter, p->tol)) return rc;
   CUDA_OK(cudaSetDevice(b->device)); cudaStream_t st = (cudaStream_t)stream;
-  if (!b->so_shape.ready && so_plan(b->dm, b->so_off)) return -1;
-  if (analysis_shape(b, (const void*)myo_static_opt_kernel, b->so_shape) || analysis_shape(b, (const void*)myo_cmc_kernel, b->cmc_shape)) return -1;
+  if (so_setup(b) || analysis_shape(b, (const void*)myo_cmc_kernel, b->cmc_shape)) return -1;
   CmcArgs ca; memset(&ca, 0, sizeof(ca)); double* lam[2];
   if (const int rc = cmc_rows(b, ca, lam)) return rc;
   // the rollout's carry from the start state; its intervals read the frame's ctrl and reserve force rows
@@ -1650,11 +1651,9 @@ extern "C" int myo_batch_cmc(myo_batch* b, const myo_cmc_buffers* d, const myo_c
   myo_buffers c;
   if (const int rc = roll_carry(b, &r, st, c)) return rc;
   const StepArgs ra = roll_args(b, c, &r, 1, p->substeps);
-  SoArgs so; memset(&so, 0, sizeof(so));
+  SoArgs so = so_args(b, p->max_iter, p->tol, flags, c);
   so.d.qacc = ca.qdes; so.d.weight = d->weight; so.d.reserve = d->reserve; so.d.act = ca.act; so.d.reserve_force = ca.rf; so.d.ctrl = p->substeps == 1 ? ca.ctrl : nullptr;
   so.d.niter = ca.niter; so.d.converged = ca.conv; so.d.residual = ca.res;
-  so.p.max_iter = p->max_iter; so.p.tol = p->tol; so.b = c; so.n_env = b->n_env; so.flags = flags;
-  so.o_H = b->so_off[0]; so.o_x = b->so_off[1]; so.o_l = b->so_off[2]; so.o_cg = b->so_off[3]; so.o_tf = b->so_off[4]; so.o_s = b->so_off[5]; so.o_gm = b->so_off[6]; so.o_bm = b->so_off[7];
   ca.d = *d; ca.c = c; ca.n_env = b->n_env; ca.nstep = nstep; ca.substeps = p->substeps;
   const LaunchShape &sc = b->cmc_shape.s, &ss = b->so_shape.s;
   for (int t = 0; ; t++) {

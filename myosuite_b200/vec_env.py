@@ -45,6 +45,71 @@ def _output(device, lead, trailing, size, int32=False):
     return torch.full(shape, -1, dtype=torch.int32, device=device) if int32 else torch.full(shape, float("nan"), dtype=torch.float64, device=device)
 
 
+def _outputs(device, fields, lead, shapes, size):
+    """Fresh output tensors {field: tensor} of the analysis calls: overflow the [n] int32 zero tensor (lead = (n, ...)), every other field
+    _output(device, lead, shapes[field], size), int32 for niter and converged."""
+    import torch
+    return {f: torch.zeros(lead[0], dtype=torch.int32, device=device) if f == "overflow"
+            else _output(device, lead, shapes[f], size, f in ("niter", "converged")) for f in fields}
+
+
+def _flags(constraints, discrete):
+    """The MYO_INV_* flags of the constraints / discrete arguments (mjDSBL_CONSTRAINT, mjENBL_INVDISCRETE)."""
+    return (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
+
+
+def _check_substeps(substeps):
+    """substeps as an int, ValueError unless >= 1."""
+    substeps = int(substeps)
+    if substeps < 1:
+        raise ValueError("substeps must be >= 1, got %d" % substeps)
+    return substeps
+
+
+def _check_solver(call, params, max_iter, tol):
+    """params (a ctypes struct with max_iter and tol), ValueError unless it holds max_iter >= 0 and a finite tol >= 0; the message quotes
+    the caller's max_iter and tol."""
+    if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
+        raise ValueError("%s needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (call, max_iter, tol))
+    return params
+
+
+def _vector(name, x, width, device, positive=True):
+    """A per-dof or per-muscle parameter: a number, array or tensor of any numeric dtype, device and layout, of shape () or (width,), as a
+    contiguous float64 [width] tensor on `device`; ValueError unless every entry is finite and > 0 (>= 0 when not `positive`)."""
+    import torch
+    v = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+    if v.dtype.kind not in "biuf" or v.shape not in ((), (width,)):
+        raise ValueError("%s must be a scalar or of shape (%d,), got %s %s" % (name, width, v.dtype, v.shape))
+    v = np.broadcast_to(v.astype(np.float64), (width,))
+    if not np.all(np.isfinite(v) & ((v > 0) if positive else (v >= 0))):
+        raise ValueError("%s must be finite and %s" % (name, "> 0" if positive else ">= 0"))
+    return torch.as_tensor(v.copy(), device=device)
+
+
+def _state_width(m, time=True):
+    """initial_state key -> trailing shape after [n] for model m (_initial_state's `width`); time only for the calls that take it."""
+    width = dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,))
+    if time:
+        width["time"] = ()
+    return width
+
+
+def _row0(out):
+    """Row 0 of every tensor of `out` {field: tensor [n, ...]} as numpy, in one device-to-host copy: each field keeps its trailing shape and
+    its dtype (int32, else float64), and a field with one value per env becomes a Python int or float."""
+    import torch
+    if not out:
+        return {}
+    flat = torch.cat([x[0].reshape(-1).double() for x in out.values()]).cpu().numpy()
+    res, o = {}, 0
+    for k, x in out.items():
+        a = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
+        a = a.astype(np.int32) if x.dtype == torch.int32 else a
+        res[k] = a.item() if a.ndim == 0 else a
+    return res
+
+
 def _initial_state(initial_state, width, n, device):
     """The start-state fields (abi.ROLLOUT_STATE) of an `initial_state` dict: KeyError for a key not in `width` (key -> trailing shape
     after [n]), ValueError for a tensor that is not a contiguous float64 [n, width] on `device`; a None value is left out."""
@@ -393,8 +458,7 @@ class MyoVecEnv:
         for f in outs:
             if f not in self._inv:
                 self._inv[f] = _output(self.device, (n,), abi.INVERSE_SHAPES[f], size)
-        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
-        self.batch.inverse(stream=self._stream(), flags=flags, qacc=qacc.contiguous(), **{f: self._inv[f] for f in outs})
+        self.batch.inverse(stream=self._stream(), flags=_flags(constraints, discrete), qacc=qacc.contiguous(), **{f: self._inv[f] for f in outs})
         return {f: self._inv[f] for f in fields}
 
     ROLLOUT_FIELDS = tuple(abi.ROLLOUT_SHAPES) + ("overflow",)
@@ -414,9 +478,7 @@ class MyoVecEnv:
         torch = self.torch
         fields = _check_fields("rollout", fields, self.ROLLOUT_FIELDS)
         m, n = self.mj_model, self.num_envs
-        substeps = int(substeps)
-        if substeps < 1:
-            raise ValueError("substeps must be >= 1, got %d" % substeps)
+        substeps = _check_substeps(substeps)
         nstep = int(ctrl.shape[1]) if isinstance(ctrl, torch.Tensor) and ctrl.dim() == 3 else 0
         if nstep < 1:
             raise ValueError("ctrl must be a float64 tensor [num_envs, nstep >= 1, nu], got %s" % (tuple(getattr(ctrl, "shape", ())),))
@@ -425,10 +487,8 @@ class MyoVecEnv:
         if qfrc_applied is not None:
             _check_f64("qfrc_applied", qfrc_applied, (n, nstep, m.nv), self.device)
             bufs["qfrc_applied"] = qfrc_applied
-        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=()), n, self.device))
-        size = dict(nq=m.nq, nv=m.nv, na=m.na)
-        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow" else _output(self.device, (n, nstep), abi.ROLLOUT_SHAPES[f], size)
-               for f in fields}
+        bufs.update(_initial_state(initial_state, _state_width(m), n, self.device))
+        out = _outputs(self.device, fields, (n, nstep), abi.ROLLOUT_SHAPES, dict(nq=m.nq, nv=m.nv, na=m.na))
         self.batch.rollout(nstep, substeps, stream=self._stream(), **bufs, **out)
         return out
 
@@ -480,8 +540,7 @@ class MyoVecEnv:
             raise ValueError("ik needs max_iter >= 0, tol >= 0, damping > 0, max_step > 0, posture >= 0 and eq_weight >= 0, all finite")
         bufs["site_id"] = torch.as_tensor(np.asarray(sid, np.int32), device=self.device)
         bufs["site_quat"] = torch.as_tensor(np.ascontiguousarray(m.site_quat[sid], dtype=np.float64), device=self.device)
-        size = dict(nq=m.nq, nv=m.nv, ns=ns)
-        out = {f: _output(self.device, (n,), abi.IK_SHAPES[f], size, f in ("niter", "converged")) for f in set(fields) | {"qpos"}}
+        out = _outputs(self.device, set(fields) | {"qpos"}, (n,), abi.IK_SHAPES, dict(nq=m.nq, nv=m.nv, ns=ns))
         self.batch.ik(params, stream=self._stream(), **bufs, **out)
         return {f: out[f] for f in fields}
 
@@ -511,14 +570,11 @@ class MyoVecEnv:
         661 torso envs), B num_envs * nx * nu * 8.  Not a state change: the call advances nothing and writes no env buffer.  With the
         iterative solver each column carries solver noise of order solver_tolerance / eps, as in MuJoCo; MyoVecEnv(...,
         solver_tolerance=...) tightens it.  Two launches (the nominal interval, then one warp per (env, column))."""
-        torch = self.torch
         fields = _check_fields("transition_fd", fields, self.FD_FIELDS)
         if "A" not in fields and "B" not in fields:
             raise ValueError("transition_fd needs at least one of the fields A and B")
         m, n = self.mj_model, self.num_envs
-        substeps, eps = int(substeps), float(eps)
-        if substeps < 1:
-            raise ValueError("substeps must be >= 1, got %d" % substeps)
+        substeps, eps = _check_substeps(substeps), float(eps)
         if not (np.isfinite(eps) and eps > 0):
             raise ValueError("eps must be finite and > 0, got %r" % eps)
         if centered not in (0, 1, False, True):
@@ -528,10 +584,8 @@ class MyoVecEnv:
         if qfrc_applied is not None:
             _check_f64("qfrc_applied", qfrc_applied, (n, m.nv), self.device)
             bufs["qfrc_applied"] = qfrc_applied
-        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,)), n, self.device))
-        size, trailing = dict(nx=2 * m.nv + m.na, nu=m.nu), dict(A=("nx", "nx"), B=("nx", "nu"))
-        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow" else _output(self.device, (n,), trailing[f], size)
-               for f in fields}
+        bufs.update(_initial_state(initial_state, _state_width(m, time=False), n, self.device))
+        out = _outputs(self.device, fields, (n,), dict(A=("nx", "nx"), B=("nx", "nu")), dict(nx=2 * m.nv + m.na, nu=m.nu))
         params = abi.MyoFdParams(eps=eps, centered=int(bool(centered)), substeps=substeps)
         self.batch.transition_fd(params, stream=self._stream(), **bufs, **out)
         return out
@@ -545,40 +599,26 @@ class MyoVecEnv:
         problem and the solver): the activations a in [0, 1] and reserve generalized forces r of least 1/2 sum w a^2 + 1/2 sum (r / reserve)^2
         whose muscle and reserve forces produce the acceleration qacc, i.e. G a + r = qfrc_inverse(qacc) - AM' bias.  qacc [num_envs, nv]
         as inverse() takes it, with its constraints and discrete flags; reserve: the reserve strengths rho > 0, a scalar or [nv] (no
-        default: the right scale differs by orders of magnitude between models); weight: muscle weights [nu] > 0 (None: 1); warmstart:
-        the dual lambda [num_envs, nv] of an earlier call (None: 0).  Tensors are contiguous float64 CUDA tensors on this batch's device.
+        default: the right scale differs by orders of magnitude between models); weight: muscle weights > 0, a scalar or [nu] (None: 1);
+        warmstart: the dual lambda [num_envs, nv] of an earlier call (None: 0).  reserve and weight may be numbers, arrays or tensors of
+        any numeric dtype, device and layout (copied to this batch's device as float64); qacc and warmstart are contiguous float64 CUDA
+        tensors on this batch's device.
         Returns {field: tensor [num_envs, ...]} of STATIC_OPT_FIELDS: act, reserve_force [nv], ctrl (the excitation that takes the current
         act to a in one mj_step, clipped to ctrlrange), actuator_force, muscle_gain, muscle_bias [nu], qfrc_inverse, lambda [nv], niter,
         converged (int32) and residual (|G a + r - t|_inf, converged when <= tol max(1, |t|_inf)); allocated per call.  One launch; not a
         state change."""
-        torch, m, n = self.torch, self.mj_model, self.num_envs
+        m, n = self.mj_model, self.num_envs
         fields = _check_fields("static_opt", fields, self.STATIC_OPT_FIELDS)
-
-        def positive(name, x, width):
-            if isinstance(x, torch.Tensor):
-                _check_f64(name, x, (width,), self.device)
-            else:
-                v = np.asarray(x, dtype=np.float64)
-                if v.shape not in ((), (width,)):
-                    raise ValueError("%s must be a scalar or of shape (%d,), got %s" % (name, width, v.shape))
-                x = torch.as_tensor(np.broadcast_to(v, (width,)).copy(), device=self.device)
-            if not bool(torch.all(torch.isfinite(x) & (x > 0))):
-                raise ValueError("%s must be finite and > 0" % name)
-            return x
         _check_f64("qacc", qacc, (n, m.nv), self.device)
-        bufs = {"qacc": qacc, "reserve": positive("reserve", reserve, m.nv)}
+        bufs = {"qacc": qacc, "reserve": _vector("reserve", reserve, m.nv, self.device)}
         if weight is not None:
-            bufs["weight"] = positive("weight", weight, m.nu)
+            bufs["weight"] = _vector("weight", weight, m.nu, self.device)
         if warmstart is not None:
             _check_f64("warmstart", warmstart, (n, m.nv), self.device)
             bufs["lambda0"] = warmstart
-        params = abi.MyoStaticOptParams(max_iter=int(max_iter), tol=float(tol))
-        if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
-            raise ValueError("static_opt needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (max_iter, tol))
-        size = dict(nu=m.nu, nv=m.nv)
-        out = {f: _output(self.device, (n,), abi.STATIC_OPT_SHAPES[f], size, f in ("niter", "converged")) for f in set(fields) | {"act"}}
-        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
-        self.batch.static_opt(params, stream=self._stream(), flags=flags, **bufs, **out)
+        params = _check_solver("static_opt", abi.MyoStaticOptParams(max_iter=int(max_iter), tol=float(tol)), max_iter, tol)
+        out = _outputs(self.device, set(fields) | {"act"}, (n,), abi.STATIC_OPT_SHAPES, dict(nu=m.nu, nv=m.nv))
+        self.batch.static_opt(params, stream=self._stream(), flags=_flags(constraints, discrete), **bufs, **out)
         return {f: out[f] for f in fields}
 
     CMC_FIELDS = tuple(abi.CMC_SHAPES) + ("overflow",)
@@ -592,47 +632,32 @@ class MyoVecEnv:
         there, warm-started from the previous frame's lambda, frame 0 from `warmstart` [num_envs, nv] or 0), the excitation that brings act
         to the optimal activations at the end of `substeps` mj_steps with ctrl held, and that interval of rollout() with qfrc_applied = the
         reserve forces.  ref_qpos [num_envs, T, nq], ref_qvel and ref_qacc [num_envs, T, nv] are contiguous float64 CUDA tensors on this
-        batch's device; kp and kv are gains >= 0, reserve and weight strengths > 0, each a scalar or a vector ([nv], weight [nu]).
+        batch's device; kp and kv are gains >= 0, reserve and weight strengths > 0, each a scalar or a vector ([nv], weight [nu]) given
+        as in static_opt(): a number, array or tensor of any numeric dtype, device and layout.
         initial_state as rollout()'s.  Returns {field: tensor [num_envs, T, ...]} of CMC_FIELDS: qacc_des, ctrl, act_opt (a*),
         reserve_force, lambda [nv or nu], niter, converged (int32), residual, and the state after the frame's interval qpos, qvel, act,
         qacc, time (rollout()'s rows); overflow [num_envs] int32.  Row t equals static_opt() and rollout() run from row t - 1's state, bit
         for bit.  The tensors are allocated per call; the frames run on the device without a host synchronisation.  Not a state change."""
         torch, m, n = self.torch, self.mj_model, self.num_envs
         fields = _check_fields("cmc", fields, self.CMC_FIELDS)
-        substeps = int(substeps)
-        if substeps < 1:
-            raise ValueError("substeps must be >= 1, got %d" % substeps)
+        substeps = _check_substeps(substeps)
         T = int(ref_qpos.shape[1]) if isinstance(ref_qpos, torch.Tensor) and ref_qpos.dim() == 3 else 0
         if T < 1:
             raise ValueError("ref_qpos must be a float64 tensor [num_envs, T >= 1, nq], got %s" % (tuple(getattr(ref_qpos, "shape", ())),))
         _check_f64("ref_qpos", ref_qpos, (n, T, m.nq), self.device)
         _check_f64("ref_qvel", ref_qvel, (n, T, m.nv), self.device)
         _check_f64("ref_qacc", ref_qacc, (n, T, m.nv), self.device)
-
-        def vector(name, x, width, positive):
-            v = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
-            if v.dtype.kind not in "biuf" or v.shape not in ((), (width,)):
-                raise ValueError("%s must be a scalar or of shape (%d,), got %s %s" % (name, width, v.dtype, v.shape))
-            v = np.broadcast_to(v.astype(np.float64), (width,))
-            if not np.all(np.isfinite(v) & ((v > 0) if positive else (v >= 0))):
-                raise ValueError("%s must be finite and %s" % (name, "> 0" if positive else ">= 0"))
-            return torch.as_tensor(v.copy(), device=self.device)
-        bufs = {"ref_qpos": ref_qpos, "ref_qvel": ref_qvel, "ref_qacc": ref_qacc, "kp": vector("kp", kp, m.nv, False),
-                "kv": vector("kv", kv, m.nv, False), "reserve": vector("reserve", reserve, m.nv, True)}
+        bufs = {"ref_qpos": ref_qpos, "ref_qvel": ref_qvel, "ref_qacc": ref_qacc, "kp": _vector("kp", kp, m.nv, self.device, positive=False),
+                "kv": _vector("kv", kv, m.nv, self.device, positive=False), "reserve": _vector("reserve", reserve, m.nv, self.device)}
         if weight is not None:
-            bufs["weight"] = vector("weight", weight, m.nu, True)
+            bufs["weight"] = _vector("weight", weight, m.nu, self.device)
         if warmstart is not None:
             _check_f64("warmstart", warmstart, (n, m.nv), self.device)
             bufs["lambda0"] = warmstart
-        bufs.update(_initial_state(initial_state, dict(qpos=(m.nq,), qvel=(m.nv,), act=(m.na,), qacc_warmstart=(m.nv,), time=()), n, self.device))
-        params = abi.MyoCmcParams(max_iter=int(max_iter), substeps=substeps, tol=float(tol))
-        if not (params.max_iter >= 0 and params.tol >= 0 and np.isfinite(params.tol)):
-            raise ValueError("cmc needs max_iter >= 0 and a finite tol >= 0, got max_iter %r, tol %r" % (max_iter, tol))
-        size = dict(nq=m.nq, nv=m.nv, nu=m.nu, na=m.na)
-        out = {f: torch.zeros(n, dtype=torch.int32, device=self.device) if f == "overflow"
-               else _output(self.device, (n, T), abi.CMC_SHAPES[f], size, f in ("niter", "converged")) for f in fields}
-        flags = (0 if constraints else abi.INV_NOCONSTRAINT) | (abi.INV_DISCRETE if discrete else 0)
-        self.batch.cmc(params, T, stream=self._stream(), flags=flags, **bufs, **out)
+        bufs.update(_initial_state(initial_state, _state_width(m), n, self.device))
+        params = _check_solver("cmc", abi.MyoCmcParams(max_iter=int(max_iter), substeps=substeps, tol=float(tol)), max_iter, tol)
+        out = _outputs(self.device, fields, (n, T), abi.CMC_SHAPES, dict(nq=m.nq, nv=m.nv, nu=m.nu, na=m.na))
+        self.batch.cmc(params, T, stream=self._stream(), flags=_flags(constraints, discrete), **bufs, **out)
         return out
 
     def examine_policy(self, policy, horizon=None, mode="exploration", seed=None, generator=None, keep_obs=True):
@@ -669,17 +694,9 @@ class _DataView:
     def _fetch(self):
         v = self._vec
         if self._version != v.state_version:
-            m = v.mj_model
             out = v.data()
-            parts = [("qpos", v.t["qpos"][0]), ("qvel", v.t["qvel"][0]), ("act", v.t["act"][0, :m.na]), ("time", v.t["time"][:1])]
-            parts += [(f, out[f][0]) for f in v.DATA_FIELDS]
-            flat = v.torch.cat([x.reshape(-1).double() for _, x in parts]).cpu().numpy()
-            d, o = {}, 0
-            for k, x in parts:
-                a = flat[o:o + x.numel()].reshape(tuple(x.shape)); o += x.numel()
-                d[k] = a.astype(np.int32) if x.dtype == v.torch.int32 else a
-            d["time"], d["ncon"] = float(d["time"][0]), int(d["ncon"])
-            self._d, self._version = d, v.state_version
+            self._d = _row0(dict(qpos=v.t["qpos"], qvel=v.t["qvel"], act=v.t["act"][:, :v.mj_model.na], time=v.t["time"], **out))
+            self._version = v.state_version
         return self._d
 
     def __getattr__(self, k):
@@ -792,18 +809,21 @@ class MyoEnv:
         r = self._fetch()
         return r["obs"], r["reward"], r["done"], self.get_env_infos()
 
+    def _dev(self, x, shape):
+        """An array-like input as a contiguous float64 tensor of `shape` on the env's device; None stays None."""
+        v = self.vec
+        return None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+
+    def _state(self, initial_state):
+        """An initial_state {key: array} as {key: [1, width] tensor} ([1] for time); None stays None."""
+        return None if initial_state is None else {k: self._dev(x, (1,) if k == "time" else (1, -1)) for k, x in initial_state.items()}
+
     def mj_inverse(self, qacc, constraints=True, discrete=False):
         """mujoco.mj_inverse for this env at its current state: {field: numpy array} of MyoVecEnv.inverse's INVERSE_FIELDS (qfrc_inverse,
         qfrc_constraint, contact_force [maxcon, 6], actuator_moment [nu, nv]) for the acceleration qacc [nv].  One launch, one
         device-to-host copy."""
         v = self.vec
-        q = v.torch.as_tensor(np.asarray(qacc, dtype=np.float64).reshape(1, -1), device=v.device)
-        out = v.inverse(q, constraints=constraints, discrete=discrete, fields=v.INVERSE_FIELDS)
-        flat = v.torch.cat([x[0].reshape(-1) for x in out.values()]).cpu().numpy()
-        res, o = {}, 0
-        for k, x in out.items():
-            res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
-        return res
+        return _row0(v.inverse(self._dev(qacc, (1, -1)), constraints=constraints, discrete=discrete, fields=v.INVERSE_FIELDS))
 
     def mj_rollout(self, ctrl, qfrc_applied=None, substeps=1, initial_state=None):
         """mujoco.mj_step rollout of this env (MyoVecEnv.rollout): ctrl [nstep, nu] is MuJoCo's ctrl, not the action (no sigmoid remap:
@@ -811,56 +831,39 @@ class MyoEnv:
         initial_state {key: array} or None (the current state).  Returns {field: numpy array [nstep, ...]} of qpos, qvel, act, qacc, time
         and the int overflow flag.  The env's own state is left as it was.  One device-to-host copy."""
         v = self.vec
-        torch = v.torch
-        as_dev = lambda x, shape: torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
-        c = np.asarray(ctrl, dtype=np.float64)
-        nstep = c.reshape(-1, self.mj_model.nu).shape[0]
-        q = None if qfrc_applied is None else as_dev(qfrc_applied, (1, nstep, self.mj_model.nv))
-        st = None if initial_state is None else {k: as_dev(x, (1,) if k == "time" else (1, -1)) for k, x in initial_state.items()}
-        out = v.rollout(as_dev(c, (1, nstep, -1)), qfrc_applied=q, substeps=substeps, initial_state=st, fields=v.ROLLOUT_FIELDS)
-        flat = torch.cat([x[0].reshape(-1).double() for x in out.values()]).cpu().numpy()
-        res, o = {}, 0
-        for k, x in out.items():
-            res[k] = flat[o:o + x[0].numel()].reshape(tuple(x.shape[1:])); o += x[0].numel()
-        res["overflow"] = int(res["overflow"])
-        return res
+        nstep = np.asarray(ctrl, dtype=np.float64).reshape(-1, self.mj_model.nu).shape[0]
+        return _row0(v.rollout(self._dev(ctrl, (1, nstep, -1)), qfrc_applied=self._dev(qfrc_applied, (1, nstep, self.mj_model.nv)), substeps=substeps,
+                               initial_state=self._state(initial_state), fields=v.ROLLOUT_FIELDS))
 
     def mj_ik(self, sites, target_pos, target_quat=None, qpos_init=None, qpos_ref=None, dofs=None, site_weight=None,
               fields=("qpos", "niter", "converged", "err"), **params):
         """Inverse kinematics of this env (MyoVecEnv.ik): target_pos [ns, 3], target_quat [ns, 4] or None, qpos_init / qpos_ref [nq] or
         None, dofs and site_weight as there; params: max_iter, tol, damping, max_step, posture, eq_weight.  Returns {field: numpy array}
-        (niter and converged as ints).  Not a state change.  One device-to-host copy per field."""
-        v = self.vec
-        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        (niter and converged as ints).  Not a state change.  One device-to-host copy."""
         ns = 1 if isinstance(sites, (str, int)) else len(sites)
-        out = v.ik(sites, as_dev(target_pos, (1, ns, 3)), target_quat=as_dev(target_quat, (1, ns, 4)), qpos_init=as_dev(qpos_init, (1, -1)),
-                   qpos_ref=as_dev(qpos_ref, (1, -1)), dofs=dofs, site_weight=as_dev(site_weight, (ns, 2)), fields=fields, **params)
-        return {k: (int(x[0]) if k in ("niter", "converged") else x[0].cpu().numpy()) for k, x in out.items()}
+        return _row0(self.vec.ik(sites, self._dev(target_pos, (1, ns, 3)), target_quat=self._dev(target_quat, (1, ns, 4)),
+                                 qpos_init=self._dev(qpos_init, (1, -1)), qpos_ref=self._dev(qpos_ref, (1, -1)), dofs=dofs,
+                                 site_weight=self._dev(site_weight, (ns, 2)), fields=fields, **params))
 
     def static_opt(self, qacc, reserve, weight=None, constraints=True, discrete=False, warmstart=None, fields=("act", "reserve_force", "ctrl"),
                    **params):
         """Muscle static optimisation of this env at its current state (MyoVecEnv.static_opt): qacc [nv], reserve (scalar or [nv]),
-        weight [nu] or None, warmstart [nv] or None; params: max_iter, tol.  Returns {field: numpy array} (niter and converged as ints).
-        Not a state change.  One device-to-host copy per field."""
-        v = self.vec
-        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
-        out = v.static_opt(as_dev(qacc, (1, -1)), reserve if np.ndim(reserve) == 0 else as_dev(reserve, (-1,)), weight=as_dev(weight, (-1,)),
-                           constraints=constraints, discrete=discrete, warmstart=as_dev(warmstart, (1, -1)), fields=fields, **params)
-        return {k: (int(x[0]) if k in ("niter", "converged") else (float(x[0]) if k == "residual" else x[0].cpu().numpy())) for k, x in out.items()}
+        weight [nu] or None, warmstart [nv] or None; params: max_iter, tol.  Returns {field: numpy array} (niter and converged as ints,
+        residual as a float).  Not a state change.  One device-to-host copy."""
+        return _row0(self.vec.static_opt(self._dev(qacc, (1, -1)), reserve if np.ndim(reserve) == 0 else self._dev(reserve, (-1,)),
+                                         weight=self._dev(weight, (-1,)), constraints=constraints, discrete=discrete,
+                                         warmstart=self._dev(warmstart, (1, -1)), fields=fields, **params))
 
     def cmc(self, ref_qpos, ref_qvel, ref_qacc, kp, kv, reserve, weight=None, initial_state=None, warmstart=None,
             fields=("qpos", "qvel", "act", "ctrl", "act_opt", "reserve_force", "niter", "converged"), **params):
         """Computed muscle control of this env along a reference motion (MyoVecEnv.cmc): ref_qpos [T, nq], ref_qvel and ref_qacc [T, nv],
         kp, kv, reserve (scalars or [nv]), weight [nu] or None, initial_state {key: array} or None (the current state), warmstart [nv] or
         None; params: substeps, constraints, discrete, max_iter, tol.  Returns {field: numpy array [T, ...]} (overflow as an int).  Not a
-        state change."""
-        v = self.vec
-        as_dev = lambda x, shape: None if x is None else v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
+        state change.  One device-to-host copy."""
         T = np.asarray(ref_qpos).reshape(-1, self.mj_model.nq).shape[0]
-        st = None if initial_state is None else {k: as_dev(x, (1,) if k == "time" else (1, -1)) for k, x in initial_state.items()}
-        out = v.cmc(as_dev(ref_qpos, (1, T, -1)), as_dev(ref_qvel, (1, T, -1)), as_dev(ref_qacc, (1, T, -1)), kp, kv, reserve, weight=weight,
-                    initial_state=st, warmstart=as_dev(warmstart, (1, -1)), fields=fields, **params)
-        return {k: (int(x[0]) if k == "overflow" else x[0].cpu().numpy()) for k, x in out.items()}
+        return _row0(self.vec.cmc(self._dev(ref_qpos, (1, T, -1)), self._dev(ref_qvel, (1, T, -1)), self._dev(ref_qacc, (1, T, -1)), kp, kv, reserve,
+                                  weight=weight, initial_state=self._state(initial_state), warmstart=self._dev(warmstart, (1, -1)), fields=fields,
+                                  **params))
 
     def mj_jacSite(self, site):
         """mujoco.mj_jacSite at the current state: (jacp [3, nv], jacr [3, nv]) as numpy arrays."""
@@ -871,15 +874,9 @@ class MyoEnv:
         """mujoco.mjd_transitionFD of this env (MyoVecEnv.transition_fd) over one interval of `substeps` mj_steps: ctrl [nu] is MuJoCo's
         ctrl, qfrc_applied [nv] or None, initial_state {key: array} or None (the current state).  Returns numpy (A [nx, nx], B [nx, nu]),
         nx = 2 nv + na.  Not a state change.  One device-to-host copy."""
-        v = self.vec
-        as_dev = lambda x, shape: v.torch.as_tensor(np.asarray(x, dtype=np.float64).reshape(shape), device=v.device).contiguous()
-        q = None if qfrc_applied is None else as_dev(qfrc_applied, (1, self.mj_model.nv))
-        st = None if initial_state is None else {k: as_dev(x, (1, -1)) for k, x in initial_state.items()}
-        out = v.transition_fd(as_dev(ctrl, (1, self.mj_model.nu)), eps=eps, centered=flg_centered, substeps=substeps, qfrc_applied=q,
-                              initial_state=st)
-        nx = out["A"].shape[1]
-        flat = v.torch.cat([out["A"][0].reshape(-1), out["B"][0].reshape(-1)]).cpu().numpy()
-        return flat[:nx * nx].reshape(nx, nx), flat[nx * nx:].reshape(nx, -1)
+        r = _row0(self.vec.transition_fd(self._dev(ctrl, (1, self.mj_model.nu)), eps=eps, centered=flg_centered, substeps=substeps,
+                                         qfrc_applied=self._dev(qfrc_applied, (1, self.mj_model.nv)), initial_state=self._state(initial_state)))
+        return r["A"], r["B"]
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)
     def get_obs_dict(self, *sim_args):
