@@ -328,6 +328,43 @@ typedef struct {
 } myo_cmc_buffers;
 typedef struct { int32_t max_iter, substeps; double tol; } myo_cmc_params;
 
+/* Caller-owned device buffers of myo_batch_inverse_fd: MuJoCo's mjd_inverseFD, finite-difference Jacobians of the inverse dynamics.  For
+ * each env, at the start state (qpos, qvel, act) and the caller's qacc, let
+ *   f(q, v, a) = qfrc_inverse(q, v, a)                     (actuation = 0)
+ *   f(q, v, a) = qfrc_inverse(q, v, a) - qfrc_actuator(q, v, act)   (actuation = 1: flg_actuation, the residual the muscles do not supply,
+ *                                                            myo_static_opt_buffers' t before the muscle bias is taken out)
+ *   qfrc_inverse is myo_batch_inverse's, with the same MYO_INV_* flags and the per-env overrides (env_prm); qfrc_actuator is the readout's
+ *   (myo_data_buffers.qfrc_actuator).  Every actuator on this path is a muscle, whose force reads act, not ctrl: ctrl is not an input.
+ *   Differences are forward only, as in MuJoCo: row i of a block is (f(x + eps e_i) - f(x)) * (1 / eps), with 1 / eps the IEEE-rounded
+ *   reciprocal (myo_fd_params' rule).  The qpos perturbation is mj_integratePos(qpos, e_i, eps) (free joints included); the qvel and qacc
+ *   perturbations add eps to entry i.  Every pass, nominal and perturbed, starts from the start state with cold inverse-wrap roots.
+ *   Layout is MuJoCo's, DfDq[env][i][j] = d f_j / d q_i (the same for DfDv and DfDa): transposed with respect to the control-theory
+ *   convention and to myo_fd_buffers.A, whose A[i][j] = d x'_i / d x_j.  MuJoCo's API reference for mjd_inverseFD: "Finite differenced
+ *   Jacobians of (force, sensors) = mj_inverse(state, acceleration) ... Output dimensions (transposed w.r.t Control Theory convention):
+ *   DfDq: (nv x nv), DfDv: (nv x nv), DfDa: (nv x nv) ... flg_actuation specifies whether to subtract qfrc_actuator from qfrc_inverse".
+ *   Precision: the inside-wrap root solve (wrap2d_inside) starts cold in every pass and stops on a tolerance, |residual| <= 1e-6 on the
+ *   angle equation (at most 20 Newton steps from z = 1 - 1e-7), not at machine precision.  Where a perturbation changes the step at which
+ *   it stops, the root moves by up to that tolerance over the equation's slope, so DfDq rows of dofs that move a tendon with an inside
+ *   wrap carry noise of order that tolerance / eps, as MuJoCo's FD does.  The contact and the active constraint rows are those of each
+ *   pass's own state: a perturbation that changes them gives that column a jump, as in MuJoCo.  The product build stores the contact
+ *   Jacobian rows with 36 mantissa bits (p48), so with constraints the columns of a state with active contacts carry that rounding, of
+ *   order 2^-36 |J' efc_force| / eps (measured: up to 3e-6 x the env's largest force term per unit of q, on the hold task at eps = 1e-4);
+ *   the f64-rows build (MYO_F64_ROWS) does not.
+ *   Not provided: the sensor blocks DsDq, DsDv, DsDa (there are no device sensors), DmDq, centred differences, xfrc_applied and analytic
+ *   derivatives. */
+typedef struct {
+  const double* qacc;            /* [n, nv] in, required */
+  const double* qpos0;           /* [n, nq] start state, nullable field by field (bound buffers), as myo_fd_buffers */
+  const double* qvel0;           /* [n, nv] */
+  const double* act0;            /* [n, na] */
+  double* DfDq;                  /* [n, nv, nv] out, nullable (at least one of DfDq, DfDv, DfDa): DfDq[i][j] = d f_j / d q_i */
+  double* DfDv;                  /* [n, nv, nv] out, nullable */
+  double* DfDa;                  /* [n, nv, nv] out, nullable */
+  double* qfrc_inverse;          /* [n, nv] out, nullable: the nominal f (minus qfrc_actuator with actuation) */
+  int32_t* overflow;             /* [n] out, nullable: set when the nominal or any perturbed pass dropped contacts (myo_fd_buffers.overflow) */
+} myo_inverse_fd_buffers;
+typedef struct { double eps; int32_t actuation; } myo_inverse_fd_params;
+
 const char* myo_last_error(void);
 int myo_version(void);       /* 2: myo_buffers ends with final_obs.  Version 1 ended with overflow: a caller built against that header passes a
                                 smaller struct, so callers check that this matches the version of the header they were compiled against */
@@ -437,6 +474,14 @@ int myo_batch_static_opt(myo_batch* b, const myo_static_opt_buffers* d, const my
  * non-finite tol, a model with more than 64 dofs, or a per-env slice without room for the dual Newton's arrays.  Replaces the per-frame
  * loop of MyoSuite tutorials 6_Inverse_Dynamics and 9_Computed_muscle_control. */
 int myo_batch_cmc(myo_batch* b, const myo_cmc_buffers* d, const myo_cmc_params* p, int nstep, int flags, void* stream);
+
+/* Finite-difference Jacobians of the inverse dynamics of every env (myo_inverse_fd_buffers, myo_inverse_fd_params); flags: MYO_INV_* as
+ * myo_batch_inverse's.  Two launches on `stream`: the nominal f of every env, then one warp per (env, column) of the requested blocks.
+ * No bound buffer is written and nothing is advanced; the nominal rows are allocated by the first call.  Fails before any launch on a null
+ * batch, buffers, params or qacc, DfDq, DfDv and DfDa all null, an unbound batch, unknown flag bits, eps not finite or not > 0, actuation
+ * not in {0, 1}, or n_env x columns beyond int32.  Replaces mujoco.mjd_inverseFD (inverse-dynamics trajectory optimisation: muscle-driven
+ * direct collocation, MJPC's direct optimiser and batch estimator, static optimisation along a motion, system identification). */
+int myo_batch_inverse_fd(myo_batch* b, const myo_inverse_fd_buffers* d, const myo_inverse_fd_params* p, int flags, void* stream);
 
 /* number of kernel launches issued by this batch so far (bench.py's gpu_launches claim) */
 int64_t myo_batch_launch_count(const myo_batch* b);

@@ -144,11 +144,25 @@ class MyoCmcParams(ctypes.Structure):
     _fields_ = [("max_iter", c_i32), ("substeps", c_i32), ("tol", c_f64)]
 
 
+# myo_inverse_fd_buffers / myo_inverse_fd_params (include/myo_b200.h): finite-difference Jacobians of the inverse dynamics of
+# myo_batch_inverse_fd.  Inputs, start state, then the outputs -> trailing shape after [n] in the model's sizes (overflow is [n], int32)
+INVERSE_FD_FIELDS = ["qacc", "qpos0", "qvel0", "act0", "DfDq", "DfDv", "DfDa", "qfrc_inverse", "overflow"]
+INVERSE_FD_SHAPES = {"DfDq": ("nv", "nv"), "DfDv": ("nv", "nv"), "DfDa": ("nv", "nv"), "qfrc_inverse": ("nv",)}
+
+
+class MyoInverseFdBuffers(ctypes.Structure):
+    _fields_ = [(n, c_vp) for n in INVERSE_FD_FIELDS]
+
+
+class MyoInverseFdParams(ctypes.Structure):
+    _fields_ = [("eps", c_f64), ("actuation", c_i32)]
+
+
 EXPORTS = ["myo_last_error", "myo_version", "myo_model_from_blob", "myo_model_dims", "myo_model_destroy", "myo_batch_create",
            "myo_batch_bind", "myo_batch_destroy", "myo_batch_obs_dim", "myo_batch_reset", "myo_batch_step",
            "myo_batch_forward_debug", "myo_batch_launch_count", "myo_batch_observe", "myo_debug_chol_solve",
            "myo_batch_launch_info", "myo_batch_debug_perm", "myo_model_layout", "myo_batch_data", "myo_batch_inverse", "myo_batch_rollout",
-           "myo_batch_ik", "myo_batch_transition_fd", "myo_batch_static_opt", "myo_batch_cmc"]
+           "myo_batch_ik", "myo_batch_transition_fd", "myo_batch_static_opt", "myo_batch_cmc", "myo_batch_inverse_fd"]
 
 # myo_model_layout slots (include/myo_b200.h): persistent offsets and sizes, scratch offsets and sizes, then the scalars
 LAYOUT_PERSISTENT = ("qpos", "qvel", "act", "qws", "dax", "dan", "qM", "fsm", "eprm", "wz", "cnt", "scr")
@@ -212,6 +226,7 @@ def _bind(L):
     L.myo_batch_transition_fd.argtypes = [c_vp, ctypes.POINTER(MyoFdBuffers), ctypes.POINTER(MyoFdParams), c_vp]
     L.myo_batch_static_opt.argtypes = [c_vp, ctypes.POINTER(MyoStaticOptBuffers), ctypes.POINTER(MyoStaticOptParams), ctypes.c_int, c_vp]
     L.myo_batch_cmc.argtypes = [c_vp, ctypes.POINTER(MyoCmcBuffers), ctypes.POINTER(MyoCmcParams), ctypes.c_int, ctypes.c_int, c_vp]
+    L.myo_batch_inverse_fd.argtypes = [c_vp, ctypes.POINTER(MyoInverseFdBuffers), ctypes.POINTER(MyoInverseFdParams), ctypes.c_int, c_vp]
     L.myo_batch_launch_count.argtypes = [c_vp]
     L.myo_batch_launch_count.restype = c_i64
     L.myo_debug_chol_solve.argtypes = [ctypes.c_int, c_vp, c_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]
@@ -356,6 +371,12 @@ class Batch:
         ref_qvel, ref_qacc, kp, kv and reserve are required), a MyoCmcParams and MYO_INV_* flags."""
         d = _buffers(MyoCmcBuffers, tensors)
         _check(self.L.myo_batch_cmc(self.handle, ctypes.byref(d), ctypes.byref(params), nstep, flags, stream), self.L)
+
+    def inverse_fd(self, params, stream=None, flags=0, **tensors):
+        """Finite-difference Jacobians of the inverse dynamics (myo_batch_inverse_fd) with the given torch CUDA tensors (names of
+        INVERSE_FD_FIELDS: qacc and at least one of DfDq, DfDv, DfDa are required), a MyoInverseFdParams and MYO_INV_* flags."""
+        d = _buffers(MyoInverseFdBuffers, tensors)
+        _check(self.L.myo_batch_inverse_fd(self.handle, ctypes.byref(d), ctypes.byref(params), flags, stream), self.L)
 
     @property
     def launches(self):

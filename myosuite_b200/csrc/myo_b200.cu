@@ -672,11 +672,22 @@ extern "C" __global__ void __launch_bounds__(320) myo_data_kernel(const __grid_c
 //   vg / vp      vg holds B qacc, then M^-1 B qacc, then qfrc_constraint; vp is not used
 //   efR, efV     jar (read again by the contact-force decoding); efV: aref, then the row forces -D jar (folded by rows_applyT_add)
 struct InvArgs { myo_inverse_buffers d; myo_buffers b; int n_env, flags; };
-// One env's inverse up to its outputs (myo_inverse_kernel, myo_static_opt_kernel): leaves M qacc in S_Ma, qfrc_passive - qfrc_bias in fsm
-// and qfrc_constraint in S_g, so that qfrc_inverse = S_Ma - fsm - S_g; qacc and actuator_moment (nullable) are the whole batch's rows
-__device__ __forceinline__ void inverse_pass(const DevModel& m, const Warp w, const myo_buffers& b, int env, const double* qacc, double* actuator_moment, bool constraints, bool discrete) {
+// The hooks of inverse_pass: state(m, w) runs on the loaded state before the kinematics, qacc(i, x) gives entry i of the acceleration from
+// the caller's x, and where ACT holds the member `actuation` adds the tendon and actuation phases.  NoPerturb (myo_inverse_kernel,
+// myo_static_opt_kernel) compiles away: ACT is a compile-time false, so its passes are the same code as before the hooks.
+struct NoPerturb { static constexpr bool ACT = false;
+  __device__ __forceinline__ void state(const DevModel&, const Warp) const {}
+  __device__ __forceinline__ double qacc(int, double x) const { return x; } };
+// One env's inverse up to its outputs (myo_inverse_kernel, myo_static_opt_kernel, myo_inverse_fd_kernel): leaves M qacc in S_Ma,
+// qfrc_passive - qfrc_bias in fsm and qfrc_constraint in S_g, so that qfrc_inverse = S_Ma - fsm - S_g; qacc and actuator_moment (nullable)
+// are the whole batch's rows.  With p.actuation the tendon and actuation phases of the forward pass run after the kinematics and fsm holds
+// qfrc_passive + qfrc_actuator - qfrc_bias, so that S_Ma - fsm - S_g = qfrc_inverse - qfrc_actuator (muscle force from act).
+template <class P = NoPerturb>
+__device__ __forceinline__ void inverse_pass(const DevModel& m, const Warp w, const myo_buffers& b, int env, const double* qacc, double* actuator_moment, bool constraints, bool discrete,
+                                             const P& p = P()) {
   if (w.lane < CNT_N) ((int*)(smem + w.base + m.o_cnt))[w.lane] = 0;
   load_env_state(m, w, b, env);
+  p.state(m, w);
   phase_kinematics(m, w);
   if (actuator_moment) { phase_tendon_all(m, w);      // dense [nu, nv]: gear x the tendon moment
     const idx_t* at = CI(PA_tendon); const idx_t* nadr = CI(PT_nz_adr); const idx_t* nzd = CI(PNZ_dof); const double* __restrict__ PAm = GD(PAM_d); const double* mom = SCR(s_mom);
@@ -684,13 +695,16 @@ __device__ __forceinline__ void inverse_pass(const DevModel& m, const Warp w, co
       for (int k = 0; k < m.nv; k++) row[k] = 0;
       for (int z = nadr[t]; z < nadr[t+1]; z++) row[nzd[z]] += gear*mom[z]; }
     __syncwarp(); }
-  { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; }
+  if constexpr (P::ACT) {
+    if (p.actuation) { phase_tendon_all(m, w); phase_actuation(m, w, false, W_(act), nullptr, nullptr); }      // (ctrl only enters act_dot, which is not integrated)
+    else { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; } }
+  else { const double* dofp = CD(PDOF_d); for (int i = w.lane; i < m.nv; i += 32) W_(fsm)[i] = -dofp[2*i+1]*W_(qvel)[i]; }
   __syncwarp();
   phase_body_inertia(m, w); phase_crb(m, w); phase_bias(m, w);       // fsm = qfrc_passive - qfrc_bias
   if (constraints) { phase_collision(m, w); phase_constraints(m, w); }
   const int nefc = WI_(nefc);
   for (int r = w.lane; r < nefc; r += 32) S_jv[r] = S_aref[r];
-  for (int i = w.lane; i < m.nv; i += 32) S_a[i] = qacc[(size_t)env*m.nv + i];
+  for (int i = w.lane; i < m.nv; i += 32) S_a[i] = p.qacc(i, qacc[(size_t)env*m.nv + i]);
   __syncwarp();
   if (discrete) {      // (M + h B) qacc = M qacc_c: qacc_c = qacc + h M^-1 B qacc, with the integrator's choice of solver
     const double* dofp = CD(PDOF_d);      // (the program drops the tree-sparse lists where that choice is dense and no Newton step is sparse)
@@ -721,6 +735,43 @@ extern "C" __global__ void __launch_bounds__(320) myo_inverse_kernel(const __gri
     __syncwarp();
   }
 }
+
+// ------------------------------------------------------------------ inverse-dynamics FD (myo_batch_inverse_fd)
+// f = qfrc_inverse (- qfrc_actuator) of inverse_pass at the start state and at one forward perturbation per work item (include/myo_b200.h
+// states the semantics).  Stage 0: one env per warp on the balanced map, the nominal f of every env into the library's rows `nom` (and
+// qfrc_inverse).  Stage 1: work item k = env * ncol + column on the contiguous map, so that the warps of a round are neighbouring columns
+// of one env; column c perturbs block blk[c / nv] at dof c % nv and writes row c % nv of that block, (f - nom) * rinv.  Nothing is stored
+// back; each pass starts from the start state with cold inverse-wrap roots.
+struct InvFdArgs { myo_inverse_fd_buffers d; myo_buffers b; double* nom; double eps, rinv; int n_env, ncol, stage, flags, actuation, blk[3]; };
+// the perturbation of one column: blk 0 qpos (mj_integratePos(qpos, e_col, eps)), 1 qvel[col] += eps, 2 qacc[col] += eps, -1 none
+struct FdPerturb { static constexpr bool ACT = true; int blk, col; double eps; bool actuation;
+  __device__ __forceinline__ void state(const DevModel& m, const Warp w) const {
+    if (blk == 0) {      // through the Newton gradient's scratch (written again before inverse_pass reads it)
+      for (int i = w.lane; i < m.nv; i += 32) S_g[i] = i == col ? 1.0 : 0.0;
+      __syncwarp();
+      integrate_pos(m, w, W_(qpos), S_g, eps); }
+    else if (blk == 1 && w.lane == 0) W_(qvel)[col] += eps;
+    __syncwarp(); }
+  __device__ __forceinline__ double qacc(int i, double x) const { return blk == 2 && i == col ? x + eps : x; } };
+
+extern "C" __global__ void __launch_bounds__(320) myo_inverse_fd_kernel(const __grid_constant__ DevModel m, const __grid_constant__ InvFdArgs a) {
+  WARP_KERNEL_PROLOGUE(m, true)
+  const myo_inverse_fd_buffers& d = a.d; const bool constraints = !(a.flags & MYO_INV_NOCONSTRAINT), discrete = a.flags & MYO_INV_DISCRETE;
+  const int nv = m.nv, bal = a.stage == 0, n_item = bal ? a.n_env : a.n_env*a.ncol;
+  for (int per_cta = SLOTS_PER_CTA(bal, n_item, (int)gridDim.x, nw), j = wid; j < per_cta; j += nw) {
+    const int slot = slot_env(bal, (int)blockIdx.x, (int)gridDim.x, nw, j - wid, wid); if (slot >= n_item) break;
+    const int env = bal ? slot : slot/a.ncol, c = slot - env*a.ncol;
+    const FdPerturb p = {bal ? -1 : a.blk[c/nv], c % nv, a.eps, a.actuation != 0};
+    inverse_pass(m, w, a.b, env, d.qacc, nullptr, constraints, discrete, p);
+    const double* nom = a.nom + (size_t)env*nv;
+    if (bal) for (int i = w.lane; i < nv; i += 32) { const double v = S_Ma[i] - W_(fsm)[i] - S_g[i]; a.nom[(size_t)env*nv + i] = v; if (d.qfrc_inverse) d.qfrc_inverse[(size_t)env*nv + i] = v; }
+    else { double* out = (p.blk == 0 ? d.DfDq : p.blk == 1 ? d.DfDv : d.DfDa) + ((size_t)env*nv + p.col)*nv;
+      for (int i = w.lane; i < nv; i += 32) out[i] = (S_Ma[i] - W_(fsm)[i] - S_g[i] - nom[i])*a.rinv; }
+    if (d.overflow && w.lane == 0) { if (bal) d.overflow[env] = WI_(overflow); else if (WI_(overflow)) d.overflow[env] = 1; }      // (every stage-1 writer stores 1)
+    __syncwarp();
+  }
+}
+static_assert(sizeof(DevModel) + sizeof(InvFdArgs) <= 4096, "myo_inverse_fd_kernel's arguments fit the 4 KB kernel parameter space");
 
 // ------------------------------------------------------------------ inverse kinematics (myo_batch_ik)
 // Damped least squares to site targets (include/myo_b200.h: myo_ik_buffers), one env per warp on the balanced map.  Each warp runs its own
@@ -1027,7 +1078,10 @@ struct myo_batch { const myo_model* model; int device, n_env; myo_task_cfg cfg; 
   bool big; double* dCarry; LazyShape roll_shape; bool roll_regroup, roll_balanced;
   // transition FD (myo_batch_transition_fd): launch shape of myo_fd_kernel for fd_items work items, and its per-slot rows
   LaunchShape fd_shape; long long fd_items; double* dFdRows; size_t fd_rows_bytes;
-  LazyShape so_shape; int so_off[8]; LazyShape cmc_shape; double* dCmc; };      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt or myo_batch_cmc; myo_cmc_kernel's launch shape and the per-frame rows (cmc_rows), set by the first myo_batch_cmc
+  LazyShape so_shape; int so_off[8]; LazyShape cmc_shape; double* dCmc;      // myo_static_opt_kernel's launch shape and scratch placement (so_plan), set by the first myo_batch_static_opt or myo_batch_cmc; myo_cmc_kernel's launch shape and the per-frame rows (cmc_rows), set by the first myo_batch_cmc
+  // inverse-dynamics FD (myo_batch_inverse_fd): launch shapes of myo_inverse_fd_kernel's stage 0 (per env) and stage 1 (ifd_items work
+  // items), and the nominal rows [n, nv], allocated by the first call
+  LazyShape ifd_shape; LaunchShape ifd_item_shape; long long ifd_items; double* dIfdNom; };
 
 extern "C" const char* myo_last_error(void) { return g_err.c_str(); }
 extern "C" int myo_version(void) { return 2; }     // 2: myo_buffers.final_obs appended
@@ -1186,7 +1240,7 @@ static void data_release(myo_batch* b) {
   cudaFree(b->dRI); cudaFree(b->dRD); cudaFree(b->dPose); b->dRI = nullptr; b->dRD = nullptr; b->dPose = nullptr;
   memset(&b->data, 0, sizeof(b->data)); b->data_shape = LazyShape(); }
 extern "C" void myo_batch_destroy(myo_batch* b) { if (!b) return; cudaSetDevice(b->device); cudaFree(b->dI); cudaFree(b->dD); cudaFree(b->dCtrl); cudaFree(b->dLoad); cudaFree(b->dPerm);
-  cudaFree(b->dCarry); cudaFree(b->dFdRows); cudaFree(b->dCmc); data_release(b); delete b; }
+  cudaFree(b->dCarry); cudaFree(b->dFdRows); cudaFree(b->dCmc); cudaFree(b->dIfdNom); data_release(b); delete b; }
 extern "C" int myo_batch_obs_dim(const myo_batch* b) { return b ? b->obs_dim : -1; }
 extern "C" int64_t myo_batch_launch_count(const myo_batch* b) { return b ? b->launches : -1; }
 // Launch shape of the product kernels' env steps, as launch() and env_kernel_body use it.  Fields (first min(n, 9) written):
@@ -1349,6 +1403,42 @@ extern "C" int myo_batch_inverse(myo_batch* b, const myo_inverse_buffers* d, int
   if (analysis_shape(b, (const void*)myo_inverse_kernel, b->inv_shape)) return -1;
   InvArgs a; a.d = *d; a.b = b->bufs; a.n_env = b->n_env; a.flags = flags; const LaunchShape& s = b->inv_shape.s;
   myo_inverse_kernel<<<s.grid, s.warps*32, s.smem, (cudaStream_t)stream>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++; return 0;
+}
+
+// Inverse-dynamics FD: stage 0 (the nominal f per env, on the balanced map), then stage 1 (one warp per (env, column) of the requested blocks,
+// on the contiguous map), both on `stream`; the start state is the caller's rows or the bound buffers, read only.
+extern "C" int myo_batch_inverse_fd(myo_batch* b, const myo_inverse_fd_buffers* d, const myo_inverse_fd_params* p, int flags, void* stream) {
+  if (!b || !d || !p) return fail("myo_batch_inverse_fd: null");
+  if (!d->qacc) return fail("myo_batch_inverse_fd: qacc is required");
+  if (!d->DfDq && !d->DfDv && !d->DfDa) return fail("myo_batch_inverse_fd: at least one of DfDq, DfDv and DfDa is required");
+  if (const int rc = require_bound(b)) return rc;
+  if (flags & ~(MYO_INV_NOCONSTRAINT | MYO_INV_DISCRETE)) return fail("myo_batch_inverse_fd: unknown flag bits");
+  if (!std::isfinite(p->eps) || !(p->eps > 0)) return fail("myo_batch_inverse_fd: eps must be finite and > 0");
+  if (p->actuation != 0 && p->actuation != 1) return fail("myo_batch_inverse_fd: actuation must be 0 or 1");
+  InvFdArgs a; memset(&a, 0, sizeof(a)); int nblk = 0;
+  if (d->DfDq) a.blk[nblk++] = 0;
+  if (d->DfDv) a.blk[nblk++] = 1;
+  if (d->DfDa) a.blk[nblk++] = 2;
+  const DevModel& dm = b->dm; const long long items = (long long)b->n_env*nblk*dm.nv;
+  if (items > 0x7fffffffLL) return fail("myo_batch_inverse_fd: n_env * columns must fit in int32");
+  CUDA_OK(cudaSetDevice(b->device)); cudaStream_t st = (cudaStream_t)stream;
+  if (analysis_shape(b, (const void*)myo_inverse_fd_kernel, b->ifd_shape)) return -1;
+  if (b->ifd_items != items) { cudaDeviceProp prop; CUDA_OK(cudaGetDeviceProperties(&prop, b->device));
+    if (launch_shape((const void*)myo_inverse_fd_kernel, prop, dm.n_per_warp*8, b->const_bytes, (int)items, false, 0, b->ifd_item_shape)) return -1;
+    b->ifd_items = items; }
+  if (!b->dIfdNom) CUDA_OK(cudaMalloc(&b->dIfdNom, (size_t)b->n_env*imax(dm.nv, 1)*8));
+  const myo_buffers& q = b->bufs;
+  myo_buffers& c = a.b;      // the start state, read only
+  c.qpos = d->qpos0 ? (double*)d->qpos0 : q.qpos; c.qvel = d->qvel0 ? (double*)d->qvel0 : q.qvel; c.act = d->act0 ? (double*)d->act0 : q.act;
+  c.qacc_warmstart = q.qacc_warmstart; c.env_prm = q.env_prm;
+  a.d = *d; a.nom = b->dIfdNom; a.eps = p->eps; a.rinv = 1.0/p->eps; a.n_env = b->n_env; a.ncol = nblk*dm.nv; a.flags = flags; a.actuation = p->actuation;
+  const LaunchShape &s0 = b->ifd_shape.s, &s1 = b->ifd_item_shape;
+  a.stage = 0;
+  myo_inverse_fd_kernel<<<s0.grid, s0.warps*32, s0.smem, st>>>(b->dm, a);
+  CUDA_OK(cudaGetLastError()); b->launches++;
+  a.stage = 1;
+  myo_inverse_fd_kernel<<<s1.grid, s1.warps*32, s1.smem, st>>>(b->dm, a);
   CUDA_OK(cudaGetLastError()); b->launches++; return 0;
 }
 

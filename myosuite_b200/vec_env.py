@@ -590,6 +590,37 @@ class MyoVecEnv:
         self.batch.transition_fd(params, stream=self._stream(), **bufs, **out)
         return out
 
+    INVERSE_FD_FIELDS = tuple(abi.INVERSE_FD_SHAPES) + ("overflow",)
+
+    def inverse_fd(self, qacc, eps=1e-6, actuation=False, constraints=True, discrete=False, initial_state=None, fields=("DfDq", "DfDv", "DfDa")):
+        """MuJoCo's mjd_inverseFD for every env (myo_batch_inverse_fd; include/myo_b200.h states it in full): forward-difference
+        Jacobians of f = qfrc_inverse, or of qfrc_inverse - qfrc_actuator with actuation=True (flg_actuation: the generalized force the
+        muscles at the current act do not supply), in qpos (through mj_integratePos), qvel and qacc, at the start state and the acceleration
+        qacc [num_envs, nv] (a contiguous float64 CUDA tensor on this batch's device).  constraints and discrete as inverse()'s.
+        initial_state: {"qpos", "qvel", "act": float64 tensor [num_envs, width]}; a key left out is taken from the env's current state.
+        Returns {field: tensor [num_envs, ...]} of INVERSE_FD_FIELDS: DfDq, DfDv, DfDa [nv, nv] in MuJoCo's layout, DfDq[e, i, j] =
+        d f_j / d q_i (transposed with respect to transition_fd()'s A), qfrc_inverse [nv] (the nominal f) and overflow [num_envs] int32 (set
+        where the nominal or a perturbed pass dropped contacts).  Allocated per call: each block takes num_envs * nv^2 * 8 bytes.  Two
+        launches (the nominal, then one warp per (env, column)); not a state change."""
+        fields = _check_fields("inverse_fd", fields, self.INVERSE_FD_FIELDS)
+        if not {"DfDq", "DfDv", "DfDa"} & set(fields):
+            raise ValueError("inverse_fd needs at least one of the fields DfDq, DfDv and DfDa")
+        m, n = self.mj_model, self.num_envs
+        eps = float(eps)
+        if not (np.isfinite(eps) and eps > 0):
+            raise ValueError("eps must be finite and > 0, got %r" % eps)
+        if actuation not in (0, 1, False, True):
+            raise ValueError("actuation must be a bool, got %r" % (actuation,))
+        _check_f64("qacc", qacc, (n, m.nv), self.device)
+        width = _state_width(m, time=False)
+        del width["qacc_warmstart"]            # (no pass reads the warm start)
+        bufs = {"qacc": qacc}
+        bufs.update(_initial_state(initial_state, width, n, self.device))
+        out = _outputs(self.device, fields, (n,), abi.INVERSE_FD_SHAPES, dict(nv=m.nv))
+        params = abi.MyoInverseFdParams(eps=eps, actuation=int(bool(actuation)))
+        self.batch.inverse_fd(params, stream=self._stream(), flags=_flags(constraints, discrete), **bufs, **out)
+        return out
+
     STATIC_OPT_FIELDS = tuple(abi.STATIC_OPT_SHAPES)
     STATIC_OPT_DEFAULTS = dict(max_iter=50, tol=1e-12)
 
@@ -877,6 +908,14 @@ class MyoEnv:
         r = _row0(self.vec.transition_fd(self._dev(ctrl, (1, self.mj_model.nu)), eps=eps, centered=flg_centered, substeps=substeps,
                                          qfrc_applied=self._dev(qfrc_applied, (1, self.mj_model.nv)), initial_state=self._state(initial_state)))
         return r["A"], r["B"]
+
+    def mjd_inverseFD(self, qacc, eps=1e-6, flg_actuation=False, constraints=True, discrete=False, initial_state=None):
+        """mujoco.mjd_inverseFD of this env (MyoVecEnv.inverse_fd) at the acceleration qacc [nv]: initial_state {key: array} of qpos,
+        qvel, act or None (the current state).  Returns numpy (DfDq, DfDv, DfDa), each [nv, nv] in MuJoCo's layout (DfDq[i, j] =
+        d f_j / d q_i).  Not a state change.  One device-to-host copy."""
+        r = _row0(self.vec.inverse_fd(self._dev(qacc, (1, self.mj_model.nv)), eps=eps, actuation=flg_actuation, constraints=constraints,
+                                      discrete=discrete, initial_state=self._state(initial_state)))
+        return r["DfDq"], r["DfDv"], r["DfDa"]
 
     # ---- dicts (env_base.py:409-432, task get_obs_dict / get_reward_dict)
     def get_obs_dict(self, *sim_args):

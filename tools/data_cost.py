@@ -19,7 +19,13 @@ The "fd" case (MyoVecEnv.transition_fd, myo_batch_transition_fd): the hand, 4096
 and centred A and B at substeps 1 and frame_skip, and the host loop of rollout calls (one per column) that the rollout API alone allows
 for the same forward A and B at substeps 1; then the single env (MyoEnv.mjd_transitionFD, the device call alone, the host loop) on the
 hand and the legs, beside the C reference (tests/fd_oracle.c) on one host core.  --fd-reps rounds (x4 for the single env).
---cases selects cases by name (the fd case runs only when named)."""
+
+The "inverse_fd" case (MyoVecEnv.inverse_fd, myo_batch_inverse_fd): the hand pose at 4096 envs, the hold and the legs (walk) at 2048, the
+elbow at 4096 and the torso at 661, at the readout's qacc, in alternating order with one env step: all three blocks with constraints,
+without them and with actuation, and the host loop that inverse() alone allows for the same Jacobians: 3 nv + 1 inverse() calls (hinge and
+slide qpos columns only; a free joint's rotation would need its quaternion update on the host as well), each after setting the bound state
+or qacc of its column, with the bound state restored at the end.  --fd-reps rounds.
+--cases selects cases by name (the fd and inverse_fd cases run only when named)."""
 import argparse
 import json
 import os
@@ -227,6 +233,75 @@ def fd_case(args):
     return out
 
 
+IFD_CASES = (("hand_pose", "myoHandPoseRandom-v0", 4096), ("hold", "myoHandObjHoldRandom-v0", 2048), ("walk", "myoLegWalk-v0", 2048),
+             ("elbow", "myoElbowPose1D6MRandom-v0", 4096), ("torso", "myoTorsoPoseFixed-v0", 661))
+
+
+def _ifd_host_loop(env, qacc):
+    """DfDq (hinge / slide columns), DfDv and DfDa the way inverse() alone allows: one call per column after setting the bound qpos, qvel
+    or the qacc of that column, then the bound state restored"""
+    import torch
+    m, eps = env.mj_model, 1e-6
+    keep = {k: env.t[k].clone() for k in ("qpos", "qvel")}
+    f0 = env.inverse(qacc)["qfrc_inverse"].clone()
+    cols = []
+    for j in range(m.njnt):
+        if m.jnt_type[j] in (2, 3):
+            env.t["qpos"][:, m.jnt_qposadr[j]] += eps
+            cols.append((env.inverse(qacc)["qfrc_inverse"] - f0) * (1 / eps))
+            env.t["qpos"].copy_(keep["qpos"])
+    for i in range(m.nv):
+        env.t["qvel"][:, i] += eps
+        cols.append((env.inverse(qacc)["qfrc_inverse"] - f0) * (1 / eps))
+        env.t["qvel"].copy_(keep["qvel"])
+    for i in range(m.nv):
+        a = qacc.clone(); a[:, i] += eps
+        cols.append((env.inverse(a)["qfrc_inverse"] - f0) * (1 / eps))
+    return torch.stack(cols, 1)
+
+
+def inverse_fd_case(args):
+    """inverse_fd beside one env step and beside the host loop of inverse() calls, on every IFD_CASES batch"""
+    import numpy as np
+    import torch
+    from myosuite_b200 import vec_env
+    out = {}
+    for name, eid, n in IFD_CASES:
+        env = vec_env.MyoVecEnv(eid, n, seed=0)
+        m = env.mj_model
+        env.reset(seed=0)
+        stream = torch.cuda.current_stream(env.device)
+        g = torch.Generator(device="cpu").manual_seed(0)
+        acts = [(torch.rand(n, m.nu, generator=g) * 2 - 1).to(env.device) for _ in range(8)]
+        for k in range(4):
+            env.step(acts[k])
+        qacc = env.data("qacc")["qacc"].clone()
+        hinge = sum(1 for j in range(m.njnt) if m.jnt_type[j] in (2, 3))
+        calls = {"step": lambda k: env.step(acts[k % 8]),
+                 "inverse_fd": lambda k: env.inverse_fd(qacc), "inverse_fd_free": lambda k: env.inverse_fd(qacc, constraints=False),
+                 "inverse_fd_actuation": lambda k: env.inverse_fd(qacc, actuation=True), "host_loop": lambda k: _ifd_host_loop(env, qacc)}
+        for k in range(2):
+            for f in calls.values():
+                f(k)
+        torch.cuda.synchronize()
+        order = list(calls)
+        t = {k: [] for k in order}
+        for r in range(args.fd_reps):
+            for k in (order if r % 2 == 0 else order[::-1]):
+                t[k].append(_timed(stream, lambda: calls[k](r)))
+        s = {k: dict(median_us=float(np.median(v)), min_us=float(np.min(v)), max_us=float(np.max(v))) for k, v in t.items()}
+        for k in order[1:]:
+            s[k]["per_step"] = s[k]["median_us"] / s["step"]["median_us"]
+        s["host_loop_calls"] = 1 + hinge + 2 * m.nv
+        out[name] = dict(env_id=eid, n_env=n, nv=m.nv, **s)
+        print("inverse_fd %-9s n %4d nv %2d  step %8.1f us | " % (name, n, m.nv, s["step"]["median_us"])
+              + "  ".join("%s %9.1f us (%.2f step)" % (k, s[k]["median_us"], s[k]["per_step"]) for k in order[1:])
+              + " | host loop: %d calls, %.1fx the device call" % (s["host_loop_calls"], s["host_loop"]["median_us"] / s["inverse_fd"]["median_us"]), flush=True)
+        del env, calls
+        torch.cuda.empty_cache()
+    return out
+
+
 def main():
     import numpy as np
     import torch
@@ -293,6 +368,8 @@ def main():
         res["cases"]["ik"] = ik_case(args)
     if "fd" in want:
         res["cases"]["fd"] = fd_case(args)
+    if "inverse_fd" in want:
+        res["cases"]["inverse_fd"] = inverse_fd_case(args)
     res["gpu_after"] = gpu_info()
     print("GPU [name, power limit, SM clock, max SM clock, throttle reasons] before: %s after: %s" % (res["gpu_before"], res["gpu_after"]))
     if args.out:
